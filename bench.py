@@ -3,21 +3,25 @@
     python bench.py [--config c2|c4|c5] [--gpus N] [--steps K] [--warmup W] [--impl ours|reference|gpu_reference]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
-Workloads (BASELINE.json `configs`; shapes pinned by SURVEY.md section 8d):
+Workloads (shapes pinned by SURVEY.md section 8d):
   c2 (default, the configuration the metric is quoted on)  GPTDolomite Granite-3B-code shape, 32L / 2560d / 32 heads hd 80 /
-      F 10240 / V 49152, bf16, seq 4096 padding-free pretraining, synthetic packed tokens
+      F 10240 / V 49152, bf16, seq 4096 padding-free pretraining, synthetic packed tokens; one sequence per GPU per step
+      fits an 80 GB H100 next to the fp32 master weights and AdamW state (~63 GB) without activation checkpointing
   c4  MoEDolomite 24L / 2048d / 16 heads hd 128 / 8 experts top-2 (F 4096 each) / V 50304, seq 2048 pretraining
   c5  Llama-3-8B shape through the `import_from_huggingface` config conversion (32L / 4096d / 32 heads, 8 KV heads, hd 128 /
       F 14336 / V 128256, untied head, no bias), seq 8192 padding-free FINETUNING (ModelWrapperForFinetuning, ragged examples
       with masked prompts), block activation checkpointing
+  c4 and c5 keep 87 GB / 129 GB of fp32 master weights, gradients and AdamW state: on 80 GB GPUs they run sharded
+      over several GPUs
 
 Prints ONE JSON line on rank 0 (contract in the task statement):
   value        whole-job tokens/s with the batches already resident in HBM (device-timed, max over ranks)
   e2e          the same metric through the reference-facing wrapper call (`model({"text": cpu_tensor})` /
                `model({"input_ids": lists, "labels": lists})`) with HOST buffers: H2D of the step's tokens and D2H of the
                loss inside the timed region
-  roofline     dominant kernel = the tcgen05 GEMM: algorithmic FLOPs of every GEMM launch / CUDA-event time of that
-               launch, measured live inside the timed region, against the measured bf16 peak (MEASURED_PEAKS.json)
+  roofline     dominant kernel = the wgmma GEMM: algorithmic FLOPs of every GEMM launch / CUDA-event time of that
+               launch, measured live inside the timed region, against the bf16 peak (MEASURED_PEAKS.json if present, else
+               the H100 SXM data sheet: 989 TFLOP/s dense bf16, 3.35 TB/s, for a card allowed 700 W)
   gpu_reference  (N = 1) the reference's own PyTorch / flash-attn path (oracle/gpu_reference.py: cuBLAS nn.Linear,
                flash_attn_varlen_func, eager RMSNorm / RoPE / SwiGLU / CE, autograd, torch AdamW) timed on the same GPU,
                same shape -- the kernel-for-kernel baseline this engine has to beat
@@ -52,7 +56,7 @@ LLAMA3_8B_HF = dict(model_type="llama", vocab_size=128256, max_position_embeddin
                     bos_token_id=128000, eos_token_id=128001)
 
 WORKLOADS = {
-    "c2": dict(seq=4096, mbs=6, kind="pretraining", checkpoint_every=None,
+    "c2": dict(seq=4096, mbs=1, kind="pretraining", checkpoint_every=None,
                text="GPTDolomite Granite-3B-code shape (32L/2560d/hd80/F10240/V49152, 3.48B params) bf16 seq4096 padding-free, "
                     "full train step (fwd+bwd+reduce-scatter+clip+AdamW)"),
     "c4": dict(seq=2048, mbs=8, kind="pretraining", checkpoint_every=None,
@@ -98,11 +102,11 @@ def measured_peaks() -> dict:
         d = json.load(open(p))
         d["source"] = "measured"
         return d
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)"""
+    """nvidia-smi clocks / throttle reasons during the timed region"""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -305,6 +309,34 @@ class _FinetuneFeed:
         return {"input_ids": ids, "labels": labels}
 
 
+def dump_outputs(out_dir: str, engine, loss_hist: list, rank: int, sample: int = 1 << 22) -> None:
+    """What the timed training step hands back after its LAST timed step, as .npy files (float64 / float32) under out_dir:
+    loss.npy (the loss of every timed step, last = the last one), params.npy / grads.npy (the fp32 master parameters after
+    the optimizer step and their gradients, at `sample` fixed positions of the flat parameter vector of this rank: the same
+    positions for the same model, seed 0).  About 32 MB; the inputs and the initialisation are seeded and every reduction
+    of the step sums in a fixed order, so two runs with the same arguments write the same bytes and two builds can be
+    compared output for output."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    sfx = "" if rank == 0 else f"_rank{rank}"
+    np.save(os.path.join(out_dir, f"loss{sfx}.npy"), np.array([float(x) for x in torch.stack(loss_hist).tolist()], np.float64))
+    sizes = [u.master.numel() for u in engine.units]
+    total = sum(sizes)
+    idx = np.unique(np.random.default_rng(0).integers(0, total, size=min(sample, total), dtype=np.int64))
+    params, grads, lo = [], [], 0
+    for u, n in zip(engine.units, sizes):
+        sel = idx[(idx >= lo) & (idx < lo + n)] - lo
+        if sel.size:
+            t = torch.from_numpy(sel).to(u.master.device)
+            params.append(u.master.detach().index_select(0, t).float().cpu())
+            grads.append(u.master.grad.index_select(0, t).float().cpu())
+        lo += n
+    np.save(os.path.join(out_dir, f"params{sfx}.npy"), torch.cat(params).numpy())
+    np.save(os.path.join(out_dir, f"grads{sfx}.npy"), torch.cat(grads).numpy())
+
+
 def run_ours(args) -> None:
     import torch
     import torch.distributed as dist
@@ -421,6 +453,8 @@ def run_ours(args) -> None:
     e1.record()
     sync_all()
     ms_resident = e0.elapsed_time(e1) / args.steps
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, engine, loss_hist, rank)
     launches = _lib.total_kernel_launches()
     gemm_records = K.gemm_timer
     K.gemm_timer = None
@@ -486,10 +520,6 @@ def run_ours(args) -> None:
         gemm_tflops = gemm_flops / (gemm_ms * 1e-3) / 1e12 if gemm_ms > 0 else None
         peak = peaks["bf16_tflops_sustained"]
         h2d = wrapper.h2d_bytes_per_step if not finetune else (3 * mbs * seq * 8 + (4 * mbs + 1) * 4)
-        traffic = None
-        tpath = os.path.join(ROOT, "profiles", "r02_gemm_traffic_table.json")
-        if os.path.exists(tpath):  # written by tools/gemm_traffic_table.py from `ncu --set full` captures of this library
-            traffic = json.load(open(tpath))
         line = {
             "metric": "tokens_per_sec", "value": value, "unit": "tokens/s", "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": ms_resident, "higher_is_better": True, "scaling": "weak",
@@ -504,10 +534,9 @@ def run_ours(args) -> None:
                 "activation_checkpointing": f"every {ckpt_every} block(s)" if ckpt_every else None,
                 "packing": "ragged" if (args.ragged or finetune) else "uniform",
                 "communication_dtype": args.comm_dtype,
-                "gemm_schedule": ("cluster launch control (one cluster per tile, work stealing)" if K.get_option("gemm_dynamic")
-                                  else f"static persistent workers, {K.get_option('gemm_sm_margin')} SMs left to NCCL"),
+                "gemm_schedule": f"static persistent workers, {K.get_option('gemm_sm_margin')} SMs left to NCCL",
                 "attention_cta_order": "heads fastest, longest tiles first" if K.get_option("attn_head_fastest") else "tiles fastest",
-                "l2": "working set (parameters + activations per step, tens of GB) far exceeds the 126 MB L2; four resident "
+                "l2": "working set (parameters + activations per step, tens of GB) far exceeds the 50 MB L2; four resident "
                       "batches are used in turn; no explicit flush",
             },
             "tokens_per_sec_per_gpu": value / world,
@@ -522,15 +551,10 @@ def run_ours(args) -> None:
             "gpu_launches": launches,
             "peak_hbm_gb": torch.cuda.max_memory_allocated(dev) / 1e9,
             "roofline": {
-                "bound": "tensor", "kernel": "gemm_bf16_kernel (tcgen05, all nn.Linear fwd/dgrad/wgrad + LM head"
+                "bound": "tensor", "kernel": "gemm_bf16_kernel (wgmma, all nn.Linear fwd/dgrad/wgrad + LM head"
                                              + (", grouped expert GEMMs)" if cfg.get("model_type") == "moe_dolomite" else ")"),
                 "achieved": gemm_tflops, "peak": peak, "unit": "TFLOP/s",
                 "frac": (gemm_tflops / peak) if gemm_tflops else None,
-                # dram__bytes_read.sum + dram__bytes_write.sum per launch from `ncu --set full` captures of THIS library,
-                # one row per GEMM shape of the step (null until the capture script has run for this commit)
-                "traffic": (traffic or {}).get("dominant_launch_dram_bytes"),
-                "traffic_algorithmic": (traffic or {}).get("dominant_launch_algorithmic_bytes"),
-                "traffic_source": "profiles/r02_gemm_traffic_table.json" if traffic else None,
                 "peak_source": f"{peaks['source']} bf16_tflops_sustained (kernel timed inside a long step)",
                 "launches_timed": len(gemm_records), "share_of_step": gemm_ms / (ms_resident * args.steps),
             },
@@ -563,19 +587,22 @@ def main() -> None:
     ap.add_argument("--impl", default="ours", choices=["ours", "reference", "gpu_reference"])
     ap.add_argument("--config", default="c2", choices=sorted(WORKLOADS))
     ap.add_argument("--mbs", type=int, default=None,
-                    help="sequences per GPU per step; default per workload (c2: 6 x 4096 fills ~146 of 180 GB, measured 41.1 k / "
-                         "42.1 k / 42.3 k tokens/s at 4 / 6 / 7)")
+                    help="sequences per GPU per step; default per workload (c2: 1 x 4096 on an 80 GB H100 at a 700 W power "
+                         "limit measured 14.5 k tokens/s; 2 or more sequences only fit with --checkpoint-every 1)")
     ap.add_argument("--ref-mbs", type=int, default=None, help="micro-batch of the gpu_reference arm (eager autograd keeps more)")
     ap.add_argument("--layers", type=int, default=None, help="override the depth (probes only: a shallower model is not the workload)")
     ap.add_argument("--ragged", action="store_true")
     ap.add_argument("--comm-dtype", default="bf16", choices=["bf16", "fp32"])
     ap.add_argument("--fsdp-mode", default="reshard", choices=["reshard", "resident"],
-                    help="N > 1: reshard = the reference's stage 3 (FULL_SHARD); resident = parameters stay gathered (B200 option)")
+                    help="N > 1: reshard = the reference's stage 3 (FULL_SHARD); resident = parameters stay gathered")
     ap.add_argument("--checkpoint-every", type=int, default=None)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-gpu-reference", action="store_true")
     ap.add_argument("--profile-step", default=None, metavar="JSON",
                     help="diagnostic: write per-kernel device times of one extra (untimed) step to this file")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed (losses, a fixed sample of the "
+                         "updated fp32 parameters and of their gradients) as .npy files under DIR")
     args = ap.parse_args()
     wl = WORKLOADS[args.config]
     if args.mbs is None:

@@ -55,7 +55,8 @@ SIGNATURES: dict[str, tuple] = {
     "dolomite_b200_add_scaled": (_I, [_P, _P, _P, _F, _L, _P]),
     "dolomite_b200_dropout_fwd": (_I, [_P, _P, _P, _L, _F, _F, _U, _U, _P]),
     "dolomite_b200_dropout_bwd": (_I, [_P, _P, _L, _F, _F, _U, _U, _P]),
-    "dolomite_b200_sumsq_accum": (_I, [_P, _L, _P, _P]),
+    "dolomite_b200_sumsq_workspace_bytes": (_L, []),
+    "dolomite_b200_sumsq_accum": (_I, [_P, _L, _P, _P, _P]),
     "dolomite_b200_clip_coef": (_I, [_P, _F, _P, _P, _P]),
     "dolomite_b200_adamw_step": (_I, [_P, _P, _P, _P, _P, _L, _F, _F, _F, _F, _F, _L, _P, _P]),
     "dolomite_b200_cast_f32_to_bf16": (_I, [_P, _P, _L, _P]),
@@ -133,7 +134,7 @@ KERNELS_PER_CALL = {
     "dolomite_b200_gelu_bwd": 1, "dolomite_b200_swiglu_fwd": 1, "dolomite_b200_swiglu_bwd": 1, "dolomite_b200_swiglu_bwd_bias": 1,
     "dolomite_b200_embedding_fwd": 1,
     "dolomite_b200_embedding_bwd": 1, "dolomite_b200_cross_entropy_fwd_bwd": 3, "dolomite_b200_colsum_accum": 1,
-    "dolomite_b200_scale_bf16_by_device_scalar": 1, "dolomite_b200_add_scaled": 1, "dolomite_b200_sumsq_accum": 1,
+    "dolomite_b200_scale_bf16_by_device_scalar": 1, "dolomite_b200_add_scaled": 1, "dolomite_b200_sumsq_accum": 2,
     "dolomite_b200_clip_coef": 1, "dolomite_b200_adamw_step": 1, "dolomite_b200_cast_f32_to_bf16": 1,
     "dolomite_b200_accum_bf16_into_f32": 1, "dolomite_b200_gemm_bf16": 1, "dolomite_b200_attn_varlen_fwd": 1,
     "dolomite_b200_attn_varlen_bwd": 3, "dolomite_b200_attn_varlen_fwd_dropout": 1, "dolomite_b200_attn_varlen_bwd_dropout": 3,

@@ -1,9 +1,9 @@
-"""Build the C-ABI CUDA library (sm_100a only) in-tree with nvcc.
+"""Build the C-ABI CUDA library (sm_90a, H100) in-tree with nvcc.
 
     python -m dolomite_engine_b200.build [--force] [--verbose]
 
-Produces dolomite_engine_b200/lib/libdolomite_b200.so.  nvcc cross-compiles without a GPU; the built .so is
-git-ignored but travels to the GPU box with the gpurun snapshot.
+Produces dolomite_engine_b200/lib/libdolomite_b200.so (and the host library libdolomite_data.so).  nvcc cross-compiles
+without a GPU; the built libraries are git-ignored build products.
 """
 
 from __future__ import annotations
@@ -25,7 +25,7 @@ INCLUDE = os.path.join(os.path.dirname(_HERE), "include")
 
 NVCC_FLAGS = [
     "-gencode",
-    "arch=compute_100a,code=sm_100a",
+    "arch=compute_90a,code=sm_90a",
     "-lineinfo",
     "-O3",
     "-std=c++17",
@@ -88,7 +88,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         if r[2]:
             sys.stderr.write(r[2])
     if rebuilt or not os.path.exists(LIB_PATH):
-        cmd = [_nvcc(), "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB_PATH, *objs]
+        cmd = [_nvcc(), "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB_PATH, *objs]
         proc = subprocess.run(cmd, capture_output=True, text=True)
         if proc.returncode != 0:
             raise RuntimeError(f"link failed:\n{proc.stdout}\n{proc.stderr}")

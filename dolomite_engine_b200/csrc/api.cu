@@ -25,24 +25,21 @@ extern "C" const char* dolomite_b200_last_error() { return g_err; }
 
 extern "C" int dolomite_b200_abi_version() { return DOLOMITE_B200_ABI_VERSION; }
 
+// gemm_cta_pair, attn_fwd_split, attn_bwd_variant, attn_bwd_ablate, gemm_dynamic and gemm_f32_tma_epilogue select kernel
+// variants of other GPU generations: sm_90 has one kernel for each of these jobs, so their values are only stored and
+// reported back (callers written for the ABI keep working).
 static int g_gemm_cta_pair = 1;
 static int g_gemm_sm_margin = 0;
 int dolo_option_gemm_sm_margin() { return g_gemm_sm_margin; }
-int dolo_option_gemm_cta_pair() { return g_gemm_cta_pair; }
 static int g_attn_fwd_split = 1;
-int dolo_option_attn_fwd_split() { return g_attn_fwd_split; }
 static int g_attn_bwd_variant = 2;
-int dolo_option_attn_bwd_variant() { return g_attn_bwd_variant; }
 static int g_attn_head_fastest = 8;
 int dolo_option_attn_head_fastest() { return g_attn_head_fastest; }
 static int g_attn_bwd_ablate = 0;
-int dolo_option_attn_bwd_ablate() { return g_attn_bwd_ablate; }
 static int g_gemm_l2_hints = 1;
 int dolo_option_gemm_l2_hints() { return g_gemm_l2_hints; }
-static int g_gemm_dynamic = 1;  // default since call 85: +1.4 ... +2.1 % on the C2 step, no SM margin next to NCCL
-int dolo_option_gemm_dynamic() { return g_gemm_dynamic; }
+static int g_gemm_dynamic = 1;
 static int g_gemm_f32_tma_epilogue = 0;
-int dolo_option_gemm_f32_tma_epilogue() { return g_gemm_f32_tma_epilogue; }
 
 extern "C" int dolomite_b200_set_option(const char* key, int value) {
     if (key != nullptr && strcmp(key, "gemm_sm_margin") == 0) {
@@ -105,10 +102,10 @@ extern "C" int dolomite_b200_get_option(const char* key, int* value) {
 int dolo_num_sms() {
     static int cached[64] = {0};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
     if (cached[dev] == 0) {
         int n = 0;
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
         cached[dev] = n;
     }
     return cached[dev];
@@ -180,29 +177,5 @@ int dolo_make_tmap(CUtensorMap* out, const void* base, int elem_bytes, int rank,
             (unsigned long long)(rank > 2 ? dims[2] : 0), (unsigned long long)(rank > 1 ? strides_bytes[1] : 0), box[0],
             rank > 1 ? box[1] : 0, rank > 2 ? box[2] : 0, int(sw));
     }
-    return DOLO_OK;
-}
-
-// DEBUG (not part of the ABI, used by tools/gpu_probe.py): `ctas` CTAs that each hold an SM (64 KB of shared memory: a GEMM
-// CTA does not fit next to it) and spin for `cycles` clocks -- a stand-in for a concurrent NCCL kernel on a one-GPU box.
-namespace {
-__global__ void __launch_bounds__(128, 1) debug_hold_sms_kernel(long long cycles, unsigned* sink) {
-    extern __shared__ uint8_t hold[];
-    const long long t0 = clock64();
-    unsigned acc = 0;
-    while (clock64() - t0 < cycles) acc += hold[(threadIdx.x * 37) & 0xFFFF];
-    if (acc == 0xFFFFFFFFu && sink != nullptr) *sink = acc;
-}
-}  // namespace
-
-extern "C" int dolomite_b200_debug_hold_sms(int ctas, long long cycles, void* stream) {
-    DOLO_REQUIRE(ctas >= 1 && ctas <= 148 && cycles >= 0 && cycles <= 20000000000ll, "debug_hold_sms: bad arguments");
-    static bool attr_set = false;
-    if (!attr_set) {
-        DOLO_CUDA_OK(cudaFuncSetAttribute(debug_hold_sms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 65536));
-        attr_set = true;
-    }
-    debug_hold_sms_kernel<<<ctas, 128, 65536, static_cast<cudaStream_t>(stream)>>>(cycles, nullptr);
-    DOLO_LAUNCH_OK("debug_hold_sms");
     return DOLO_OK;
 }

@@ -1,16 +1,5 @@
-// Packed var-len causal attention backward on tcgen05 (autograd of flash_attn_varlen_func,
+// Packed var-len causal attention backward on wgmma (autograd of flash_attn_varlen_func,
 // attention/padding_free.py:51-62).
-//
-// One CTA = one 128-row key/value tile of one kv-head group of one document; it loops over the query heads of the
-// group and the query tiles i >= j (causal) and keeps dK_j, dV_j accumulating in TMEM.  Everything is computed in
-// the "transposed" frame (TMEM lane == key row) so that P^T and dS^T can be fed back to the tensor core straight
-// from TMEM as the A operand:
-//     S^T  = K_j Q_i^T            (SS)           dP^T = V_j dO_i^T             (SS)
-//     P^T  = exp2(S^T*scale - LSE_i) ,  dS^T = scale * P^T o (dP^T - Delta_i)     (softmax warps, one key row / thread)
-//     dV_j += P^T dO_i            (TS, B = dO MN-major)
-//     dK_j += dS^T Q_i            (TS, B = Q  MN-major)
-//     dQ_i  = dS K_j              (SS, A = dS^T staged in smem as an MN-major operand, B = K MN-major)
-// dQ_i tiles are reduced across CTAs with fp32 vector atomics into a workspace and converted at the end.
 #include "attention_common.cuh"
 #include "../../include/dolomite_b200.h"
 
@@ -18,12 +7,9 @@ using namespace dolo;
 
 namespace {
 
-constexpr int BWD_THREADS = 192;
-
 struct BwdParams {
     const float* lse;      // [n_heads, T]
     const float* delta;    // [n_heads, T]
-    float* dq_accum;       // [n_heads, T, HD] fp32 (a query tile of one head is one contiguous slab)
     __nv_bfloat16* dqkv;   // [T, row_stride]
     int64_t row_stride;
     const int32_t* cu_seqlens;
@@ -31,18 +17,11 @@ struct BwdParams {
     int64_t T;
     int n_groups, q_per_group, n_heads;
     float scale, scale_log2;
-    int head_chunk;    // CTA order (attention_common.cuh: attn_cta_order): kv groups per chunk, 0 = tiles fastest (round 1)
-    int n_tile_slots;  // upper bound of the number of key tiles (the grid has n_tile_slots x n_groups CTAs)
+    int head_chunk;    // CTA order (attention_common.cuh: attn_cta_order): kv groups per chunk, 0 = tiles fastest
+    int head_chunk_q;  // the same for the query heads of the dQ kernel
+    int n_tile_slots;  // upper bound of the number of 128-row key (dK/dV) or query (dQ) tiles of a head
     AttnDropout drop;  // attention-probability dropout of the forward being differentiated (threshold 0: none)
-    int ablate;  // TIMING EXPERIMENTS ONLY (wrong results): see dolo_option_attn_bwd_ablate
-    unsigned long long* trace;  // DEBUG timeline buffer (5 roles x 2048 events) or nullptr
-    int trace_cta;
 };
-
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
-    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d)
-                 : "memory");
-}
 
 // Delta[h, t] = sum_d dO[t, h, d] * O[t, h, d].  Block = DELTA_TOK tokens: every thread takes 16-byte vectors of dO and O
 // (coalesced over the whole [tokens, heads*hd] slab) and leaves its 8-product partial in shared memory; the partials of a
@@ -79,428 +58,214 @@ __global__ void __launch_bounds__(256)
     }
 }
 
-// dq_accum (fp32 [n_heads, T, hd]) -> bf16 q slots of dqkv
-// (`scale`: the pipelined kernel accumulates dS' K with dS' = P o (dP - delta), the softmax scale is applied here)
-__global__ void attn_dq_finalize_kernel(const float* __restrict__ acc, __nv_bfloat16* __restrict__ dqkv,
-                                        int64_t row_stride, int64_t T, int n_groups, int q_per_group, int hd, float scale) {
-    const int n_heads = n_groups * q_per_group;
-    const int vec_per_row = n_heads * hd / 4;
-    const int64_t total = T * vec_per_row;
-    for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += int64_t(gridDim.x) * blockDim.x) {
-        const int64_t t = i / vec_per_row;
-        const int e = int(i - t * vec_per_row) * 4;
-        const int h = e / hd, d = e - h * hd;
-        const int g = h / q_per_group, s = h - g * q_per_group;
-        const float4 v = *reinterpret_cast<const float4*>(acc + (int64_t(h) * T + t) * hd + d);
-        __nv_bfloat16* dst = dqkv + t * row_stride + int64_t(g * (q_per_group + 2) + s) * hd + d;
-        uint2 o;
-        o.x = pack_bf16(v.x * scale, v.y * scale);
-        o.y = pack_bf16(v.z * scale, v.w * scale);
-        *reinterpret_cast<uint2*>(dst) = o;
-    }
-}
+// One CTA = one 128-row key/value tile of one kv-head group of one document, two warpgroups of 64 key rows each; it loops
+// over the query heads of the group and the 64-row query tiles that see the key tile (causal) and keeps dK_j, dV_j
+// accumulating in registers.  Everything is computed in the "transposed" frame (accumulator row == key row) so that P^T and
+// dS^T feed the tensor core straight from registers as the A operand.  Per step, every warpgroup runs
+//     S^T  = K_j Q_i^T            (SS)           dP^T = V_j dO_i^T             (SS)
+//     P^T  = exp2(S^T*scale - LSE_i) ,  dS^T = scale * P^T o (dP^T - Delta_i)     (registers)
+//     dV_j += P^T dO_i            (RS, B = dO MN-major)
+//     dK_j += dS^T Q_i            (RS, B = Q  MN-major)
+// Thread 0 also issues the TMA loads (K_j, V_j once; Q_i, dO_i through a 2-stage ring).
+// dQ has its own kernel (attn_dq_kernel below: one CTA per query tile walks the key tiles in order), so that every
+// gradient is summed in a fixed order and the backward is bit-identical from run to run -- adding the dQ contributions
+// of the key-tile CTAs with atomics would not be.
+constexpr int BWD_THREADS = 256;
+constexpr int BWD_QT = 64;  // query rows per step
+constexpr int QDO_STAGES = 2;
 
 template <int HD>
 __global__ void __launch_bounds__(BWD_THREADS, 1)
     attn_bwd_kernel(const __grid_constant__ CUtensorMap tq64, const __grid_constant__ CUtensorMap tqR,
-                    const __grid_constant__ CUtensorMap to64, const __grid_constant__ CUtensorMap toR,
-                    const __grid_constant__ CUtensorMap tdq, const BwdParams p) {
+                    const __grid_constant__ CUtensorMap to64, const __grid_constant__ CUtensorMap toR, const BwdParams p) {
     using CH = HeadChunks<HD>;
-    constexpr int TILE_BYTES = CH::TILE_BYTES;
-    constexpr int QDO_STAGES = 2;
-    constexpr uint32_t ST_COL = 0, DP_COL = 128, DV_COL = 256, DK_COL = 256 + HD;
-    constexpr bool DQ_SEPARATE = (256 + 3 * HD) <= 512;
-    static_assert(DQ_SEPARATE || CH::NCHUNK <= 2, "dQ aliasing needs at most two chunks");
-    // dQ tiles leave through shared memory + TMA tile reduce-add (one operation per warp and 32 columns, the add is done by
-    // the L2) instead of 32 per-thread red.global.add.v4.f32 per row: the per-thread atomics were 26 % of the pipelined
-    // kernel before it got the same treatment (DESIGN section 7).  The staging slabs are the warp's own rows of the dS^T
-    // tile, which the dQ MMA has finished reading by the time the accumulator is drained.
-    constexpr bool DQ_TMA = (HD % 32 == 0);
+    constexpr int KV_BYTES = CH::tile_bytes(ATT_TILE);
+    constexpr int QT_BYTES = CH::tile_bytes(BWD_QT);
 
     int cta_tile, group;  // key tiles of a document in natural order = longest first
     attn_cta_order(p.head_chunk, p.n_tile_slots, cta_tile, group);
     const TileLoc loc = locate_tile(p.cu_seqlens, p.n_docs, cta_tile);
     if (!loc.valid) return;
-    const int j = loc.tile;                                      // kv tile
-    const int n_q_tiles = (loc.doc_len + ATT_TILE - 1) / ATT_TILE;
-    const int n_i = n_q_tiles - j;                               // q tiles j .. n_q_tiles-1
-    const int n_it = n_i * p.q_per_group;
+    const int k0 = loc.tile * ATT_TILE;             // first key (doc-relative) of this tile
+    const int i0 = k0 / BWD_QT;                     // first query tile that sees a key of the tile
+    const int n_qt = (loc.doc_len + BWD_QT - 1) / BWD_QT;
+    const int n_i = n_qt - i0;
+    const int n_steps = n_i * p.q_per_group;
     const int k_col = (group * (p.q_per_group + 2) + p.q_per_group) * HD;
     const int v_col = k_col + HD;
-    const int kv_row = loc.doc_start + j * ATT_TILE;
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_align_1024(smem_raw);
     uint8_t* sK = smem;
-    uint8_t* sV = sK + TILE_BYTES;
-    uint8_t* sQ = sV + TILE_BYTES;                    // [QDO_STAGES]
-    uint8_t* sDO = sQ + QDO_STAGES * TILE_BYTES;      // [QDO_STAGES]
-    uint8_t* sDS = sDO + QDO_STAGES * TILE_BYTES;     // 128 keys x 128 queries bf16, MN-major SW128 (2 x 16 KB)
-    float* sLSE = reinterpret_cast<float*>(sDS + 2 * ATT_TILE * 128);  // [128] (log2 units)
-    float* sDelta = sLSE + ATT_TILE;                                  // [128]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sDelta + ATT_TILE);
-    uint64_t* kv_full = bars;              // 1
-    uint64_t* qdo_full = bars + 1;         // [2]
-    uint64_t* qdo_empty = bars + 3;        // [2]
-    uint64_t* sdp_full = bars + 5;         // S^T and dP^T ready
-    uint64_t* pds_ready = bars + 6;        // 128 arrivals: P^T / dS^T written
-    uint64_t* dq_full = bars + 7;          // dQ tile (and dV/dK updates) complete
-    uint64_t* dq_done = bars + 8;          // 128 arrivals: dQ tile drained from TMEM
-    uint64_t* dkv_full = bars + 9;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 10);
+    uint8_t* sV = sK + KV_BYTES;
+    uint8_t* sQ = sV + KV_BYTES;                // [QDO_STAGES]
+    uint8_t* sO = sQ + QDO_STAGES * QT_BYTES;   // [QDO_STAGES] dO
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sO + QDO_STAGES * QT_BYTES);
+    uint64_t* kv_full = bars;       // 1
+    uint64_t* qd_full = bars + 1;   // [QDO_STAGES]
+    uint64_t* qd_empty = bars + 3;  // [QDO_STAGES], one arrive per warp
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-    if (warp == 0 && lane == 0) {
+    auto load_step = [&](int n, int s) {
+        const int hl = n / n_i, qi = i0 + n % n_i;
+        const int head = group * p.q_per_group + hl;
+        const int q_col = (group * (p.q_per_group + 2) + hl) * HD;
+        mbar_expect_tx(&qd_full[s], 2 * QT_BYTES);
+        tma_load_chunked<HD, BWD_QT>(sQ + s * QT_BYTES, &tq64, &tqR, &qd_full[s], q_col, loc.doc_start + qi * BWD_QT);
+        tma_load_chunked<HD, BWD_QT>(sO + s * QT_BYTES, &to64, &toR, &qd_full[s], head * HD, loc.doc_start + qi * BWD_QT);
+    };
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tq64);
         tma_prefetch_desc(&to64);
-        mbar_init(kv_full, 1);
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&qdo_full[i], 1);
-            mbar_init(&qdo_empty[i], 1);
+        if (CH::REM > 0) {
+            tma_prefetch_desc(&tqR);
+            tma_prefetch_desc(&toR);
         }
-        mbar_init(sdp_full, 1);
-        mbar_init(pds_ready, 128);
-        mbar_init(dq_full, 1);
-        mbar_init(dq_done, 128);
-        mbar_init(dkv_full, 1);
+        mbar_init(kv_full, 1);
+        for (int i = 0; i < QDO_STAGES; ++i) {
+            mbar_init(&qd_full[i], 1);
+            mbar_init(&qd_empty[i], BWD_THREADS / 32);
+        }
         mbar_fence_init();
+        mbar_expect_tx(kv_full, 2 * KV_BYTES);
+        tma_load_chunked<HD, ATT_TILE>(sK, &tq64, &tqR, kv_full, k_col, loc.doc_start + k0);
+        tma_load_chunked<HD, ATT_TILE>(sV, &tq64, &tqR, kv_full, v_col, loc.doc_start + k0);
+        for (int n = 0; n < QDO_STAGES && n < n_steps; ++n) load_step(n, n);
     }
-    if (warp == 1) tmem_alloc<512>(tmem_slot);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    auto load_tile = [&](uint8_t* dst, uint64_t* bar, const CUtensorMap* m64, const CUtensorMap* mR, int col, int row) {
+    const int wr = (warp & 3) * 16 + (lane >> 2);  // first of the two accumulator rows of this thread (and wr + 8)
+    const int wc = 2 * (lane & 3);                 // first accumulator column inside each n8 block
+    const int kr[2] = {k0 + wg * 64 + wr, k0 + wg * 64 + wr + 8};  // doc-relative keys of the two rows
+    const bool drop = p.drop.threshold != 0;
+    const float log2e = 1.4426950408889634f;
+    const uint32_t sk = smem_u32(sK) , sv = smem_u32(sV);
+
+    float dv[HD / 2], dk[HD / 2];
+#pragma unroll
+    for (int i = 0; i < HD / 2; ++i) dv[i] = dk[i] = 0.f;
+
+    mbar_wait(kv_full, 0, 30);
+    for (int n = 0; n < n_steps; ++n) {
+        const int s = n & (QDO_STAGES - 1);
+        const int hl = n / n_i, qi = i0 + n % n_i;
+        const int head = group * p.q_per_group + hl;
+        const int q0 = qi * BWD_QT;
+        const uint32_t head_key = dropout_head_key(uint32_t(head), p.drop.key0, p.drop.key1);
+        // LSE / Delta of this thread's 16 query columns
+        float lse_c[BWD_QT / 8][2], del_c[BWD_QT / 8][2];
+#pragma unroll
+        for (int b = 0; b < BWD_QT / 8; ++b)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int q = q0 + 8 * b + wc + e;
+                const int64_t idx = int64_t(head) * p.T + loc.doc_start + q;
+                lse_c[b][e] = q < loc.doc_len ? __ldg(p.lse + idx) * log2e : 0.f;
+                del_c[b][e] = q < loc.doc_len ? __ldg(p.delta + idx) : 0.f;
+            }
+        mbar_wait(&qd_full[s], (n / QDO_STAGES) & 1, 31);
+        const uint32_t sq = smem_u32(sQ + s * QT_BYTES), so = smem_u32(sO + s * QT_BYTES);
+
+        float st[BWD_QT / 2], dpt[BWD_QT / 2];
+        wgmma_fence();
 #pragma unroll
         for (int c = 0; c < CH::NCHUNK; ++c) {
-            const CUtensorMap* m = (c < CH::NC64) ? m64 : mR;
-            tma_load_2d(dst + CH::offset(c), m, bar, col + CH::col(c), row);
-        }
-    };
-    auto dq_col = [&](int c) -> uint32_t {
-        return DQ_SEPARATE ? uint32_t(256 + 2 * HD + CH::col(c)) : (c == 0 ? 64u : 192u);
-    };
-
-    if (warp == 0) {
-        if (elect_one()) {
-            mbar_expect_tx(kv_full, 2 * TILE_BYTES);
-            load_tile(sK, kv_full, &tq64, &tqR, k_col, kv_row);
-            load_tile(sV, kv_full, &tq64, &tqR, v_col, kv_row);
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int it = 0; it < n_it; ++it) {
-                const int s = it / n_i, i = j + (it - s * n_i);
-                const int head = group * p.q_per_group + s;
-                const int q_col = (group * (p.q_per_group + 2) + s) * HD;
-                const int q_row = loc.doc_start + i * ATT_TILE;
-                mbar_wait(&qdo_empty[stage], phase ^ 1, 20);
-                mbar_expect_tx(&qdo_full[stage], 2 * TILE_BYTES);
-                load_tile(sQ + stage * TILE_BYTES, &qdo_full[stage], &tq64, &tqR, q_col, q_row);
-                load_tile(sDO + stage * TILE_BYTES, &qdo_full[stage], &to64, &toR, head * HD, q_row);
-                if (++stage == QDO_STAGES) { stage = 0; phase ^= 1; }
+            const int w = CH::width(c);
+            const uint32_t krow = CH::offset(c, ATT_TILE) + wg * 64 * 2 * w;  // this warpgroup's 64 key rows of the chunk
+#pragma unroll
+            for (int k = 0; k < w / 16; ++k) {
+                wgmma_ss<BWD_QT, 0, 0>(st, chunk_desc_kmajor(sk + krow, w, k), chunk_desc_kmajor(sq + CH::offset(c, BWD_QT), w, k),
+                                       (c != 0 || k != 0) ? 1u : 0u);
+                wgmma_ss<BWD_QT, 0, 0>(dpt, chunk_desc_kmajor(sv + krow, w, k), chunk_desc_kmajor(so + CH::offset(c, BWD_QT), w, k),
+                                       (c != 0 || k != 0) ? 1u : 0u);
             }
         }
-    } else if (warp == 1) {
-        if (elect_one()) {
-            constexpr uint32_t idesc_s = umma_idesc_bf16(128, 128, false, false);
-            mbar_wait(kv_full, 0, 21);
-            const uint32_t k_s = smem_u32(sK), v_s = smem_u32(sV), ds_s = smem_u32(sDS);
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int it = 0; it < n_it; ++it) {
-                mbar_wait(&qdo_full[stage], phase, 22);
-                if (it > 0) mbar_wait(dq_done, uint32_t((it - 1) & 1), 23);  // dQ columns (may alias S/dP) drained
-                tc_fence_after();
-                const uint32_t q_s = smem_u32(sQ + stage * TILE_BYTES);
-                const uint32_t do_s = smem_u32(sDO + stage * TILE_BYTES);
-                bool first = true;
+        wgmma_commit();
+        wgmma_wait<0>();
+        reg_fence<BWD_QT / 2>(st);
+        reg_fence<BWD_QT / 2>(dpt);
+
+        // ---------------- P^T, dS^T ----------------
 #pragma unroll
-                for (int c = 0; c < CH::NCHUNK; ++c) {
-                    const int w = CH::width(c);
+        for (int h = 0; h < 2; ++h)
 #pragma unroll
-                    for (int k = 0; k < w / 16; ++k) {
-                        umma_ss(tmem_base + ST_COL, chunk_desc_kmajor(k_s + CH::offset(c), w, k),
-                                chunk_desc_kmajor(q_s + CH::offset(c), w, k), idesc_s, first ? 0u : 1u);
-                        first = false;
+            for (int b = 0; b < BWD_QT / 8; ++b)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int q = q0 + 8 * b + wc + e;
+                    const int i = 4 * b + 2 * h + e;
+                    const bool ok = q >= kr[h] && q < loc.doc_len;  // causal, and a real query of the document
+                    float pr = ok ? fast_exp2(fmaf(st[i], p.scale_log2, -lse_c[b][e])) : 0.f;
+                    float dp = dpt[i];
+                    if (drop) {
+                        const float z = attn_drop_scale(p.drop, head_key, loc.doc_start + q, loc.doc_start + kr[h]);
+                        dp *= z;
+                        st[i] = pr * z;  // dropped-and-rescaled probabilities: what dV sees
+                    } else {
+                        st[i] = pr;
                     }
+                    dpt[i] = p.scale * pr * (dp - del_c[b][e]);
                 }
-                first = true;
+        uint32_t pa[BWD_QT / 16][4], da[BWD_QT / 16][4];
 #pragma unroll
-                for (int c = 0; c < CH::NCHUNK; ++c) {
-                    const int w = CH::width(c);
+        for (int kk = 0; kk < BWD_QT / 16; ++kk) {
+            acc_to_a_frag(st, kk, pa[kk]);
+            acc_to_a_frag(dpt, kk, da[kk]);
+        }
+
+        // ---------------- dV += P^T dO,  dK += dS^T Q ----------------
+        wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < w / 16; ++k) {
-                        umma_ss(tmem_base + DP_COL, chunk_desc_kmajor(v_s + CH::offset(c), w, k),
-                                chunk_desc_kmajor(do_s + CH::offset(c), w, k), idesc_s, first ? 0u : 1u);
-                        first = false;
-                    }
+        for (int c = 0; c < CH::NCHUNK; ++c) {
+#pragma unroll
+            for (int kk = 0; kk < BWD_QT / 16; ++kk) {
+                if (CH::width(c) == 64) {
+                    wgmma_rs<64, 1>(dv + CH::col(c) / 2, pa[kk], chunk_desc_mnmajor(so + CH::offset(c, BWD_QT), 64, kk), 1u);
+                    wgmma_rs<64, 1>(dk + CH::col(c) / 2, da[kk], chunk_desc_mnmajor(sq + CH::offset(c, BWD_QT), 64, kk), 1u);
+                } else {
+                    constexpr int R = CH::REM ? CH::REM : 16;
+                    wgmma_rs<R, 1>(dv + CH::col(c) / 2, pa[kk], chunk_desc_mnmajor(so + CH::offset(c, BWD_QT), R, kk), 1u);
+                    wgmma_rs<R, 1>(dk + CH::col(c) / 2, da[kk], chunk_desc_mnmajor(sq + CH::offset(c, BWD_QT), R, kk), 1u);
                 }
-                umma_commit(sdp_full);
-                mbar_wait(pds_ready, uint32_t(it & 1), 24);
-                tc_fence_after();
-#pragma unroll
-                for (int c = 0; c < CH::NCHUNK; ++c) {
-                    const int w = CH::width(c);
-                    const uint32_t idesc_ts = umma_idesc_bf16(128, w, false, true);
-                    const uint32_t idesc_dq = umma_idesc_bf16(128, w, true, true);
-#pragma unroll
-                    for (int k = 0; k < ATT_TILE / 16; ++k) {
-                        // dV += P^T dO
-                        umma_ts(tmem_base + DV_COL + CH::col(c), tmem_base + ST_COL + k * 8,
-                                chunk_desc_mnmajor(do_s + CH::offset(c), w, k), idesc_ts, (it > 0 || k > 0) ? 1u : 0u);
-                    }
-#pragma unroll
-                    for (int k = 0; k < ATT_TILE / 16; ++k) {
-                        // dK += dS^T Q
-                        umma_ts(tmem_base + DK_COL + CH::col(c), tmem_base + DP_COL + k * 8,
-                                chunk_desc_mnmajor(q_s + CH::offset(c), w, k), idesc_ts, (it > 0 || k > 0) ? 1u : 0u);
-                    }
-#pragma unroll
-                    for (int k = 0; k < ATT_TILE / 16; ++k) {
-                        // dQ = dS K   (A = dS^T rows in smem read as MN-major [queries x keys])
-                        umma_ss(tmem_base + dq_col(c), umma_smem_desc(ds_s + k * 2048, ATT_TILE * 128, 1024, 2),
-                                chunk_desc_mnmajor(k_s + CH::offset(c), w, k), idesc_dq, k > 0 ? 1u : 0u);
-                    }
-                }
-                umma_commit(&qdo_empty[stage]);
-                umma_commit(dq_full);
-                if (it == n_it - 1) umma_commit(dkv_full);
-                if (++stage == QDO_STAGES) { stage = 0; phase ^= 1; }
             }
         }
-    } else {
-        const int sub = warp & 3;
-        const int r = sub * 32 + lane;  // key row in tile == TMEM lane; also the query row when draining dQ
-        const int et = r;
-        const uint32_t t_lane = tmem_base + (uint32_t(sub * 32) << 16);
-        const int kj = j * ATT_TILE + r;  // doc-relative key index
-        const bool key_ok = kj < loc.doc_len;
-        const float LOG2E = 1.4426950408889634f;
-        for (int it = 0; it < n_it; ++it) {
-            const int s = it / n_i, i = j + (it - s * n_i);
-            const int head = group * p.q_per_group + s;
-            // stage LSE (log2 units) and Delta of query tile i; out-of-document queries get lse = +inf (p = 0)
-            {
-                const int qi = i * ATT_TILE + et;
-                float l = INFINITY, d = 0.f;
-                if (qi < loc.doc_len) {
-                    const int64_t idx = int64_t(head) * p.T + loc.doc_start + qi;
-                    l = p.lse[idx] * LOG2E;
-                    d = p.delta[idx];
-                }
-                sLSE[et] = l;
-                sDelta[et] = d;
-            }
-            named_bar_sync(2, 128);
-            if (DQ_TMA && it > 0) {  // this warp's dS^T rows double as dQ staging slabs: the last reduces must have read them
-                if (lane == 0) tma_store_wait_read<0>();
-                __syncwarp();
-            }
-            mbar_wait(sdp_full, uint32_t(it & 1), 25);
-            tc_fence_after();
-            const bool diag = (i == j);
-            const bool drop = p.drop.threshold != 0;
-            const uint32_t head_key = dropout_head_key(uint32_t(head), p.drop.key0, p.drop.key1);
-#pragma unroll 1
-            for (int ch = 0; ch < 4; ++ch) {
-                uint32_t sv[32], dv[32];
-                tmem_ld32(t_lane + ST_COL + ch * 32, sv);
-                tmem_ld32(t_lane + DP_COL + ch * 32, dv);
-                tmem_ld_wait();
-                uint32_t pp[16], dd[16];
-#pragma unroll
-                for (int c2 = 0; c2 < 32; c2 += 2) {
-                    float pv[2], dsv[2];
-#pragma unroll
-                    for (int u = 0; u < 2; ++u) {
-                        const int c = ch * 32 + c2 + u;  // query column
-                        float pe = fast_exp2(__uint_as_float(sv[c2 + u]) * p.scale_log2 - sLSE[c]);
-                        if (!key_ok || (diag && r > c)) pe = 0.f;
-                        float dpe = __uint_as_float(dv[c2 + u]);
-                        pv[u] = pe;
-                        if (drop) {  // dV takes the dropped probabilities, dP passes through the same mask; dS uses the undropped P
-                            const float ms = attn_drop_scale(p.drop, head_key, loc.doc_start + i * ATT_TILE + c, loc.doc_start + kj);
-                            pv[u] = pe * ms;
-                            dpe *= ms;
-                        }
-                        dsv[u] = pe * (dpe - sDelta[c]) * p.scale;
-                    }
-                    pp[c2 >> 1] = pack_bf16(pv[0], pv[1]);
-                    dd[c2 >> 1] = pack_bf16(dsv[0], dsv[1]);
-                }
-                tmem_st16(t_lane + ST_COL + ch * 16, pp);
-                tmem_st16(t_lane + DP_COL + ch * 16, dd);
-                // dS^T row -> smem (MN-major A operand of the dQ MMA): 4 x 16-byte pieces of this 32-query chunk
-                uint8_t* rowp = sDS + (ch >> 1) * (ATT_TILE * 128) + r * 128;
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const int piece = (ch & 1) * 4 + q;  // 16-byte piece index within the 128-byte row
-                    uint4 v = make_uint4(dd[q * 4], dd[q * 4 + 1], dd[q * 4 + 2], dd[q * 4 + 3]);
-                    *reinterpret_cast<uint4*>(rowp + ((piece ^ (r & 7)) << 4)) = v;
-                }
-            }
-            tmem_st_wait();
-            tc_fence_before();
-            fence_proxy_async_smem();
-            mbar_arrive(pds_ready);
-            // drain dQ_i: TMEM lane r == query row r of tile i
-            mbar_wait(dq_full, uint32_t(it & 1), 26);
-            tc_fence_after();
-            if constexpr (DQ_TMA) {
-                // rows past the document add zeros (their dS is zero), rows past the tensor are clipped by the TMA unit
-                const int row0 = int(int64_t(head) * p.T + loc.doc_start + i * ATT_TILE + sub * 32);
-#pragma unroll
-                for (int c = 0; c < CH::NCHUNK; ++c) {
-                    const int w = CH::width(c);
-#pragma unroll 1
-                    for (int c0 = 0; c0 < w; c0 += 32) {
-                        const int slab = ((CH::col(c) + c0) >> 5) & 1;
-                        uint8_t* buf = sDS + slab * (ATT_TILE * 128) + sub * 4096;  // this warp's 32 rows of one dS^T half
-                        if (lane == 0) tma_store_wait_read<1>();  // the reduce issued from this slab two chunks ago has read it
-                        __syncwarp();
-                        uint32_t o[32];
-                        tmem_ld32(t_lane + dq_col(c) + c0, o);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int q = 0; q < 8; ++q)
-                            *reinterpret_cast<uint4*>(buf + lane * 128 + ((q ^ (lane & 7)) << 4)) =
-                                make_uint4(o[q * 4], o[q * 4 + 1], o[q * 4 + 2], o[q * 4 + 3]);
-                        fence_proxy_async_smem();
-                        __syncwarp();
-                        if (lane == 0) {
-                            tma_reduce_add_2d(&tdq, buf, CH::col(c) + c0, row0);
-                            tma_store_commit();
-                        }
-                    }
-                }
-            } else {
-                const int qi = i * ATT_TILE + r;
-                const bool q_ok = qi < loc.doc_len;
-                float* dst = p.dq_accum + (int64_t(head) * p.T + loc.doc_start + qi) * HD;
-#pragma unroll
-                for (int c = 0; c < CH::NCHUNK; ++c) {
-                    const int w = CH::width(c);
-#pragma unroll 1
-                    for (int c0 = 0; c0 < w; c0 += 16) {
-                        uint32_t o[16];
-                        tmem_ld16(t_lane + dq_col(c) + c0, o);
-                        tmem_ld_wait();
-                        if (q_ok) {
-#pragma unroll
-                            for (int q = 0; q < 4; ++q)
-                                red_add_v4(dst + CH::col(c) + c0 + q * 4, __uint_as_float(o[q * 4]),
-                                           __uint_as_float(o[q * 4 + 1]), __uint_as_float(o[q * 4 + 2]),
-                                           __uint_as_float(o[q * 4 + 3]));
-                        }
-                    }
-                }
-            }
-            tc_fence_before();
-            mbar_arrive(dq_done);
+        wgmma_commit();
+
+        wgmma_wait<0>();
+        reg_fence<HD / 2>(dv);
+        reg_fence<HD / 2>(dk);
+        if (lane == 0) mbar_arrive(&qd_empty[s]);  // Q_i / dO_i of this warp's MMAs are read
+        if (threadIdx.x == 0 && n + QDO_STAGES < n_steps) {
+            mbar_wait(&qd_empty[s], (n / QDO_STAGES) & 1, 32);
+            load_step(n + QDO_STAGES, s);
         }
-        // ---------------- dK_j, dV_j epilogue ----------------
-        mbar_wait(dkv_full, 0, 27);
-        tc_fence_after();
-        if (DQ_TMA && lane == 0) tma_store_wait_all<0>();  // shared memory must outlive the last dQ reduce
-        __nv_bfloat16* krow = p.dqkv + int64_t(kv_row + r) * p.row_stride + k_col;
-        __nv_bfloat16* vrow = p.dqkv + int64_t(kv_row + r) * p.row_stride + v_col;
-#pragma unroll 1
-        for (int c0 = 0; c0 < HD; c0 += 16) {
-            uint32_t a[16], b[16];
-            tmem_ld16(t_lane + DK_COL + c0, a);
-            tmem_ld16(t_lane + DV_COL + c0, b);
-            tmem_ld_wait();
-            if (key_ok) {
-                uint4 x, y;
-                x.x = pack_bf16(__uint_as_float(a[0]), __uint_as_float(a[1]));
-                x.y = pack_bf16(__uint_as_float(a[2]), __uint_as_float(a[3]));
-                x.z = pack_bf16(__uint_as_float(a[4]), __uint_as_float(a[5]));
-                x.w = pack_bf16(__uint_as_float(a[6]), __uint_as_float(a[7]));
-                y.x = pack_bf16(__uint_as_float(a[8]), __uint_as_float(a[9]));
-                y.y = pack_bf16(__uint_as_float(a[10]), __uint_as_float(a[11]));
-                y.z = pack_bf16(__uint_as_float(a[12]), __uint_as_float(a[13]));
-                y.w = pack_bf16(__uint_as_float(a[14]), __uint_as_float(a[15]));
-                *reinterpret_cast<uint4*>(krow + c0) = x;
-                *reinterpret_cast<uint4*>(krow + c0 + 8) = y;
-                x.x = pack_bf16(__uint_as_float(b[0]), __uint_as_float(b[1]));
-                x.y = pack_bf16(__uint_as_float(b[2]), __uint_as_float(b[3]));
-                x.z = pack_bf16(__uint_as_float(b[4]), __uint_as_float(b[5]));
-                x.w = pack_bf16(__uint_as_float(b[6]), __uint_as_float(b[7]));
-                y.x = pack_bf16(__uint_as_float(b[8]), __uint_as_float(b[9]));
-                y.y = pack_bf16(__uint_as_float(b[10]), __uint_as_float(b[11]));
-                y.z = pack_bf16(__uint_as_float(b[12]), __uint_as_float(b[13]));
-                y.w = pack_bf16(__uint_as_float(b[14]), __uint_as_float(b[15]));
-                *reinterpret_cast<uint4*>(vrow + c0) = x;
-                *reinterpret_cast<uint4*>(vrow + c0 + 8) = y;
-            }
+        __syncwarp();
+    }
+
+    // ---------------- dK_j, dV_j -> the k / v slots of dqkv ----------------
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        if (kr[h] >= loc.doc_len) continue;
+        __nv_bfloat16* row = p.dqkv + (loc.doc_start + int64_t(kr[h])) * p.row_stride;
+#pragma unroll
+        for (int b = 0; b < HD / 8; ++b) {
+            *reinterpret_cast<uint32_t*>(row + k_col + 8 * b + wc) = pack_bf16(dk[4 * b + 2 * h], dk[4 * b + 2 * h + 1]);
+            *reinterpret_cast<uint32_t*>(row + v_col + 8 * b + wc) = pack_bf16(dv[4 * b + 2 * h], dv[4 * b + 2 * h + 1]);
         }
     }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc<512>(tmem_base);
-    }
-}
-
-template <int HD>
-int make_maps(const void* base, int64_t ld, int64_t rows, CUtensorMap* m64, CUtensorMap* mR) {
-    using CH = HeadChunks<HD>;
-    uint64_t dims[2] = {uint64_t(ld), uint64_t(rows)};
-    uint64_t strides[2] = {2, uint64_t(ld) * 2};
-    uint32_t box[2] = {64, ATT_TILE};
-    int rc;
-    if (CH::NC64 > 0) {
-        rc = dolo_make_tmap(m64, base, 2, 2, dims, strides, box, DOLO_SW_128);
-        if (rc) return rc;
-    }
-    if (CH::REM > 0) {
-        box[0] = CH::REM;
-        rc = dolo_make_tmap(mR, base, 2, 2, dims, strides, box, CH::REM == 32 ? DOLO_SW_64 : DOLO_SW_32);
-        if (rc) return rc;
-    }
-    if (CH::NC64 == 0) *m64 = *mR;
-    if (CH::REM == 0) *mR = *m64;
-    return DOLO_OK;
-}
-
-#include "attention_bwd_v3.cuh"
-
-// head_dim <= 80: pipelined kernel (two softmax warp groups); larger head dims: serial kernel below
-template <int HD>
-int launch_bwd_pipelined(const void* dout, const void* qkv, int64_t row_stride, const BwdParams& p, cudaStream_t st,
-                         int variant) {
-    if (variant == 0) return launch_bwd_v3<HD, 2, false, false>(dout, qkv, row_stride, p, st);
-    if constexpr (HD % 64 != 0) {
-        if (variant == 2) return launch_bwd_v3<HD, 2, true, true>(dout, qkv, row_stride, p, st);
-    }
-    return launch_bwd_v3<HD, 2, true, false>(dout, qkv, row_stride, p, st);
 }
 
 template <int HD>
 int launch_bwd(const void* dout, const void* qkv, int64_t row_stride, const BwdParams& p, cudaStream_t st) {
     using CH = HeadChunks<HD>;
-    constexpr int QDO_STAGES = 2;
     CUtensorMap tq64, tqR, to64, toR;
-    int rc = make_maps<HD>(qkv, row_stride, p.T, &tq64, &tqR);
+    int rc = attn_make_maps<HD>(qkv, row_stride, p.T, &tq64, &tqR);
     if (rc) return rc;
-    rc = make_maps<HD>(dout, int64_t(p.n_heads) * HD, p.T, &to64, &toR);
+    rc = attn_make_maps<HD>(dout, int64_t(p.n_heads) * HD, p.T, &to64, &toR);
     if (rc) return rc;
-    constexpr int smem_bytes =
-        1024 + (2 + 2 * QDO_STAGES) * CH::TILE_BYTES + 2 * ATT_TILE * 128 + 2 * ATT_TILE * 4 + 128;
+    constexpr int smem_bytes = 1024 + 2 * CH::tile_bytes(ATT_TILE) + 2 * QDO_STAGES * CH::tile_bytes(BWD_QT) + 128;
     static_assert(smem_bytes <= 232448, "attention backward shared memory budget exceeded");
-    CUtensorMap tdq;
-    {
-        // dq_accum as [heads * T rows, HD columns] fp32; box = 32 columns x 32 rows (the staging slab of one warp)
-        uint64_t dims[2] = {uint64_t(HD), uint64_t(p.n_heads) * uint64_t(p.T)};
-        uint64_t strides[2] = {4, uint64_t(HD) * 4};
-        uint32_t box[2] = {HD >= 32 ? 32u : uint32_t(HD), 32};
-        rc = dolo_make_tmap(&tdq, p.dq_accum, 4, 2, dims, strides, box, HD >= 32 ? DOLO_SW_128 : DOLO_SW_64);
-        if (rc) return rc;
-    }
     auto kern = attn_bwd_kernel<HD>;
     static bool attr_set = false;
     if (!attr_set) {
@@ -510,8 +275,195 @@ int launch_bwd(const void* dout, const void* qkv, int64_t row_stride, const BwdP
     const int64_t max_tiles = (p.T + ATT_TILE - 1) / ATT_TILE + p.n_docs;
     DOLO_REQUIRE(max_tiles == p.n_tile_slots && max_tiles * p.n_groups < (1ll << 31), "attn_bwd: grid too large");
     dim3 grid((unsigned)(max_tiles * p.n_groups));
-    kern<<<grid, BWD_THREADS, smem_bytes, st>>>(tq64, tqR, to64, toR, tdq, p);
+    kern<<<grid, BWD_THREADS, smem_bytes, st>>>(tq64, tqR, to64, toR, p);
     DOLO_LAUNCH_OK("attn_varlen_bwd");
+    return DOLO_OK;
+}
+
+// dQ of the backward: one CTA = one 128-row query tile of one head of one document, two warpgroups of 64 queries each,
+// looping over the 64-row key tiles the queries see, in order.  Per key tile every warpgroup recomputes
+//     S  = Q_i K_j^T ,  dP = dO_i V_j^T           (SS)
+//     dS = scale * P o (dP - Delta_i)             (registers, P = exp2(S*scale - LSE_i))
+//     dQ_i += dS K_j                              (RS, B = K MN-major)
+// and finally writes dQ_i (bf16) into the q slots of dqkv.  Thread 0 issues the TMA loads: Q_i and dO_i once, (K_j, V_j)
+// through a 2-stage ring.
+constexpr int DQ_THREADS = 256;
+constexpr int DQ_KT = 64;  // keys per step
+
+template <int HD>
+__global__ void __launch_bounds__(DQ_THREADS, 1)
+    attn_dq_kernel(const __grid_constant__ CUtensorMap tq64, const __grid_constant__ CUtensorMap tqR,
+                   const __grid_constant__ CUtensorMap to64, const __grid_constant__ CUtensorMap toR, const BwdParams p) {
+    using CH = HeadChunks<HD>;
+    constexpr int Q_BYTES = CH::tile_bytes(ATT_TILE);
+    constexpr int KT_BYTES = CH::tile_bytes(DQ_KT);
+
+    int ti, head;
+    attn_cta_order(p.head_chunk_q, p.n_tile_slots, ti, head);
+    ti = p.n_tile_slots - 1 - ti;  // long (late) tiles first
+    const TileLoc loc = locate_tile(p.cu_seqlens, p.n_docs, ti);
+    if (!loc.valid) return;
+    const int group = head / p.q_per_group, slot = head % p.q_per_group;
+    const int q_col = (group * (p.q_per_group + 2) + slot) * HD;
+    const int k_col = (group * (p.q_per_group + 2) + p.q_per_group) * HD;
+    const int v_col = k_col + HD;
+    const int q0 = loc.tile * ATT_TILE;
+    const int k_end = min(q0 + ATT_TILE, loc.doc_len);  // causal: keys [0, k_end) are seen by some query of the tile
+    const int n_kt = (k_end + DQ_KT - 1) / DQ_KT;
+
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_align_1024(smem_raw);
+    uint8_t* sQ = smem;
+    uint8_t* sO = sQ + Q_BYTES;       // dO
+    uint8_t* sK = sO + Q_BYTES;       // [2]
+    uint8_t* sV = sK + 2 * KT_BYTES;  // [2]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sV + 2 * KT_BYTES);
+    uint64_t* q_full = bars;        // 1
+    uint64_t* kv_full = bars + 1;   // [2]
+    uint64_t* kv_empty = bars + 3;  // [2], one arrive per warp
+
+    const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    auto load_kv = [&](int j, int s) {
+        mbar_expect_tx(&kv_full[s], 2 * KT_BYTES);
+        tma_load_chunked<HD, DQ_KT>(sK + s * KT_BYTES, &tq64, &tqR, &kv_full[s], k_col, loc.doc_start + j * DQ_KT);
+        tma_load_chunked<HD, DQ_KT>(sV + s * KT_BYTES, &tq64, &tqR, &kv_full[s], v_col, loc.doc_start + j * DQ_KT);
+    };
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(&tq64);
+        tma_prefetch_desc(&to64);
+        if (CH::REM > 0) {
+            tma_prefetch_desc(&tqR);
+            tma_prefetch_desc(&toR);
+        }
+        mbar_init(q_full, 1);
+        for (int i = 0; i < 2; ++i) {
+            mbar_init(&kv_full[i], 1);
+            mbar_init(&kv_empty[i], DQ_THREADS / 32);
+        }
+        mbar_fence_init();
+        mbar_expect_tx(q_full, 2 * Q_BYTES);
+        tma_load_chunked<HD, ATT_TILE>(sQ, &tq64, &tqR, q_full, q_col, loc.doc_start + q0);
+        tma_load_chunked<HD, ATT_TILE>(sO, &to64, &toR, q_full, head * HD, loc.doc_start + q0);
+        for (int j = 0; j < 2 && j < n_kt; ++j) load_kv(j, j);
+    }
+    __syncthreads();
+
+    const int wr = (warp & 3) * 16 + (lane >> 2);
+    const int wc = 2 * (lane & 3);
+    const int qr[2] = {q0 + wg * 64 + wr, q0 + wg * 64 + wr + 8};  // doc-relative queries of the two rows
+    const bool drop = p.drop.threshold != 0;
+    const uint32_t head_key = dropout_head_key(uint32_t(head), p.drop.key0, p.drop.key1);
+    const float log2e = 1.4426950408889634f;
+    float lse_r[2], del_r[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const bool ok = qr[h] < loc.doc_len;
+        const int64_t idx = int64_t(head) * p.T + loc.doc_start + qr[h];
+        lse_r[h] = ok ? __ldg(p.lse + idx) * log2e : 0.f;
+        del_r[h] = ok ? __ldg(p.delta + idx) : 0.f;
+    }
+    const uint32_t sq = smem_u32(sQ), so = smem_u32(sO);
+    float dq[HD / 2];
+#pragma unroll
+    for (int i = 0; i < HD / 2; ++i) dq[i] = 0.f;
+
+    mbar_wait(q_full, 0, 40);
+    for (int j = 0; j < n_kt; ++j) {
+        const int s = j & 1;
+        mbar_wait(&kv_full[s], (j >> 1) & 1, 41);
+        const uint32_t sk = smem_u32(sK + s * KT_BYTES), sv = smem_u32(sV + s * KT_BYTES);
+        float sc[DQ_KT / 2], dp[DQ_KT / 2];
+        wgmma_fence();
+#pragma unroll
+        for (int c = 0; c < CH::NCHUNK; ++c) {
+            const int w = CH::width(c);
+            const uint32_t qrow = CH::offset(c, ATT_TILE) + wg * 64 * 2 * w;  // this warpgroup's 64 query rows of the chunk
+#pragma unroll
+            for (int k = 0; k < w / 16; ++k) {
+                wgmma_ss<DQ_KT, 0, 0>(sc, chunk_desc_kmajor(sq + qrow, w, k), chunk_desc_kmajor(sk + CH::offset(c, DQ_KT), w, k),
+                                      (c != 0 || k != 0) ? 1u : 0u);
+                wgmma_ss<DQ_KT, 0, 0>(dp, chunk_desc_kmajor(so + qrow, w, k), chunk_desc_kmajor(sv + CH::offset(c, DQ_KT), w, k),
+                                      (c != 0 || k != 0) ? 1u : 0u);
+            }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        reg_fence<DQ_KT / 2>(sc);
+        reg_fence<DQ_KT / 2>(dp);
+
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int b = 0; b < DQ_KT / 8; ++b)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int k = j * DQ_KT + 8 * b + wc + e;
+                    const int i = 4 * b + 2 * h + e;
+                    const bool ok = k <= qr[h] && qr[h] < loc.doc_len;  // causal, and a real query of the document
+                    const float pr = ok ? fast_exp2(fmaf(sc[i], p.scale_log2, -lse_r[h])) : 0.f;
+                    float d = dp[i];
+                    if (drop) d *= attn_drop_scale(p.drop, head_key, loc.doc_start + qr[h], loc.doc_start + k);
+                    sc[i] = p.scale * pr * (d - del_r[h]);
+                }
+        uint32_t da[DQ_KT / 16][4];
+#pragma unroll
+        for (int kk = 0; kk < DQ_KT / 16; ++kk) acc_to_a_frag(sc, kk, da[kk]);
+
+        wgmma_fence();
+#pragma unroll
+        for (int c = 0; c < CH::NCHUNK; ++c) {
+#pragma unroll
+            for (int kk = 0; kk < DQ_KT / 16; ++kk) {
+                if (CH::width(c) == 64) {
+                    wgmma_rs<64, 1>(dq + CH::col(c) / 2, da[kk], chunk_desc_mnmajor(sk + CH::offset(c, DQ_KT), 64, kk), 1u);
+                } else {
+                    constexpr int R = CH::REM ? CH::REM : 16;
+                    wgmma_rs<R, 1>(dq + CH::col(c) / 2, da[kk], chunk_desc_mnmajor(sk + CH::offset(c, DQ_KT), R, kk), 1u);
+                }
+            }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        reg_fence<HD / 2>(dq);
+        if (lane == 0) mbar_arrive(&kv_empty[s]);
+        if (threadIdx.x == 0 && j + 2 < n_kt) {
+            mbar_wait(&kv_empty[s], (j >> 1) & 1, 42);  // both warpgroups are done with key tile j
+            load_kv(j + 2, s);
+        }
+        __syncwarp();
+    }
+
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        if (qr[h] >= loc.doc_len) continue;
+        __nv_bfloat16* row = p.dqkv + (loc.doc_start + int64_t(qr[h])) * p.row_stride + q_col + wc;
+#pragma unroll
+        for (int b = 0; b < HD / 8; ++b)
+            *reinterpret_cast<uint32_t*>(row + 8 * b) = pack_bf16(dq[4 * b + 2 * h], dq[4 * b + 2 * h + 1]);
+    }
+}
+
+template <int HD>
+int launch_dq(const void* dout, const void* qkv, int64_t row_stride, const BwdParams& p, cudaStream_t st) {
+    using CH = HeadChunks<HD>;
+    CUtensorMap tq64, tqR, to64, toR;
+    int rc = attn_make_maps<HD>(qkv, row_stride, p.T, &tq64, &tqR);
+    if (rc) return rc;
+    rc = attn_make_maps<HD>(dout, int64_t(p.n_heads) * HD, p.T, &to64, &toR);
+    if (rc) return rc;
+    constexpr int smem_bytes = 1024 + 2 * CH::tile_bytes(ATT_TILE) + 4 * CH::tile_bytes(DQ_KT) + 128;
+    static_assert(smem_bytes <= 232448, "attention dQ shared memory budget exceeded");
+    auto kern = attn_dq_kernel<HD>;
+    static bool attr_set = false;
+    if (!attr_set) {
+        DOLO_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+        attr_set = true;
+    }
+    const int64_t max_tiles = (p.T + ATT_TILE - 1) / ATT_TILE + p.n_docs;
+    DOLO_REQUIRE(max_tiles == p.n_tile_slots && max_tiles * p.n_heads < (1ll << 31), "attn_bwd: grid too large");
+    dim3 grid((unsigned)(max_tiles * p.n_heads));
+    kern<<<grid, DQ_THREADS, smem_bytes, st>>>(tq64, tqR, to64, toR, p);
+    DOLO_LAUNCH_OK("attn_varlen_bwd_dq");
     return DOLO_OK;
 }
 
@@ -519,20 +471,11 @@ inline int64_t align256(int64_t x) { return (x + 255) & ~int64_t(255); }
 
 }  // namespace
 
-static unsigned long long* g_bwd_trace = nullptr;
-static int g_bwd_trace_cta = 0;
-// DEBUG (not part of the ABI header): device buffer of 5 x 2048 uint64 that one CTA of the pipelined backward fills with
-// (event id << 56 | clock64) stamps; nullptr switches tracing off.
-extern "C" int dolomite_b200_debug_attn_bwd_trace(void* buf, int cta) {
-    g_bwd_trace = static_cast<unsigned long long*>(buf);
-    g_bwd_trace_cta = cta;
-    return DOLO_OK;
-}
-
 extern "C" int64_t dolomite_b200_attn_varlen_bwd_workspace_bytes(int64_t T, int n_groups, int q_per_group,
                                                                  int head_dim) {
     const int64_t nh = int64_t(n_groups) * q_per_group;
-    return align256(nh * T * 4) + align256(T * nh * head_dim * 4) + 256;
+    (void)head_dim;
+    return align256(nh * T * 4) + 256;  // Delta
 }
 
 uint32_t dolo_dropout_threshold(float p);  // dropout.cu
@@ -563,8 +506,6 @@ extern "C" int dolomite_b200_attn_varlen_bwd_dropout(const void* dout, const voi
     DOLO_REQUIRE(int64_t(nh) * T < (1ll << 31), "attn_bwd: heads * T too large for the dQ tile reduce");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     float* delta = static_cast<float*>(workspace);
-    float* dq_accum = reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) + align256(int64_t(nh) * T * 4));
-    DOLO_CUDA_OK(cudaMemsetAsync(dq_accum, 0, size_t(T) * nh * head_dim * 4, st));
     {
         const int64_t blocks = (T + DELTA_TOK - 1) / DELTA_TOK;
         attn_delta_kernel<<<(unsigned)blocks, 256, size_t(nh) * (head_dim / 8) * DELTA_TOK * sizeof(float), st>>>(
@@ -574,7 +515,6 @@ extern "C" int dolomite_b200_attn_varlen_bwd_dropout(const void* dout, const voi
     BwdParams p;
     p.lse = lse;
     p.delta = delta;
-    p.dq_accum = dq_accum;
     p.dqkv = static_cast<__nv_bfloat16*>(dqkv);
     p.row_stride = row_stride;
     p.cu_seqlens = cu_seqlens;
@@ -587,36 +527,21 @@ extern "C" int dolomite_b200_attn_varlen_bwd_dropout(const void* dout, const voi
     p.scale_log2 = softmax_scale * 1.4426950408889634f;
     p.n_tile_slots = int((T + ATT_TILE - 1) / ATT_TILE + n_docs);
     p.head_chunk = attn_head_chunk(dolo_option_attn_head_fastest(), n_groups, 1);
+    p.head_chunk_q = attn_head_chunk(dolo_option_attn_head_fastest(), nh, q_per_group);
     p.drop.threshold = dolo_dropout_threshold(dropout_p);
     p.drop.keep_scale = 1.f / (1.f - dropout_p);
     p.drop.key0 = key0;
     p.drop.key1 = key1;
-    p.ablate = dolo_option_attn_bwd_ablate();
-    p.trace = g_bwd_trace;
-    p.trace_cta = g_bwd_trace_cta;
     int rc;
-    // dropout lives in the round-1 softmax warps of the pipelined kernel only (the lean variants have no registers to spare)
-    const int variant = p.drop.threshold != 0 ? 0 : dolo_option_attn_bwd_variant();
-    const bool pipelined = head_dim == 64 || head_dim == 80;
-    const float dq_scale = (pipelined && variant != 0) ? softmax_scale : 1.f;
     switch (head_dim) {
-        case 16: rc = launch_bwd<16>(dout, qkv, row_stride, p, st); break;
-        case 32: rc = launch_bwd<32>(dout, qkv, row_stride, p, st); break;
-        case 64: rc = launch_bwd_pipelined<64>(dout, qkv, row_stride, p, st, variant); break;
-        case 80: rc = launch_bwd_pipelined<80>(dout, qkv, row_stride, p, st, variant); break;
-        case 96: rc = launch_bwd<96>(dout, qkv, row_stride, p, st); break;
-        case 128: rc = launch_bwd<128>(dout, qkv, row_stride, p, st); break;
+        case 16: rc = launch_bwd<16>(dout, qkv, row_stride, p, st); if (!rc) rc = launch_dq<16>(dout, qkv, row_stride, p, st); break;
+        case 32: rc = launch_bwd<32>(dout, qkv, row_stride, p, st); if (!rc) rc = launch_dq<32>(dout, qkv, row_stride, p, st); break;
+        case 64: rc = launch_bwd<64>(dout, qkv, row_stride, p, st); if (!rc) rc = launch_dq<64>(dout, qkv, row_stride, p, st); break;
+        case 80: rc = launch_bwd<80>(dout, qkv, row_stride, p, st); if (!rc) rc = launch_dq<80>(dout, qkv, row_stride, p, st); break;
+        case 96: rc = launch_bwd<96>(dout, qkv, row_stride, p, st); if (!rc) rc = launch_dq<96>(dout, qkv, row_stride, p, st); break;
+        case 128: rc = launch_bwd<128>(dout, qkv, row_stride, p, st); if (!rc) rc = launch_dq<128>(dout, qkv, row_stride, p, st); break;
         default: return dolo_set_error("attn_bwd: unsupported head_dim %d (supported: 16,32,64,80,96,128)", head_dim);
     }
     if (rc) return rc;
-    {
-        const int64_t total = T * nh * head_dim / 4;
-        int64_t blocks = (total + 255) / 256;
-        const int64_t cap = int64_t(dolo_num_sms()) * 16;
-        if (blocks > cap) blocks = cap;
-        attn_dq_finalize_kernel<<<(unsigned)blocks, 256, 0, st>>>(dq_accum, static_cast<__nv_bfloat16*>(dqkv), row_stride,
-                                                                  T, n_groups, q_per_group, head_dim, dq_scale);
-        DOLO_LAUNCH_OK("attn_dq_finalize");
-    }
     return DOLO_OK;
 }

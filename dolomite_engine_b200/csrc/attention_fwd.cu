@@ -1,12 +1,12 @@
-// Packed var-len causal attention forward on tcgen05 (replaces flash_attn_varlen_func at
+// Packed var-len causal attention forward on wgmma (replaces flash_attn_varlen_func at
 // attention/padding_free.py:51-62).
 //
-// One CTA = one 128-row query tile of one head of one document.  Warp roles:
-//   warp 0   TMA producer: Q tile once, then (K_j, V_j) tiles through a 2-stage ring
-//   warp 1   MMA issuer:   S = Q K_j^T  (SS, fp32 in TMEM)  and  O += P_j V_j  (A = P from TMEM, B = V MN-major)
-//   warps 2-5 softmax:     one query row per thread (TMEM lane == row): online max / exp2 / sum, P -> TMEM as bf16
-//                          (aliasing the S columns), O rescale in TMEM, final O / l and LSE store.
-// TMEM: S/P 128 columns + O head_dim columns  (<= 256 -> two CTAs per SM overlap each other's softmax and MMA).
+// One CTA = one 128-row query tile of one head of one document, two warpgroups of 64 query rows each.  Thread 0 also
+// issues the TMA loads: the Q tile once, then (K_j, V_j) tiles through a 2-stage ring.  Per key tile every warpgroup runs
+//     S = Q K_j^T        (wgmma SS, fp32 scores in registers, 64 x 128 per warpgroup)
+//     online softmax     (each thread holds two query rows x 32 keys; row max / sum over the quad of a row)
+//     O += P V_j         (wgmma RS: P as the bf16 register A operand, V MN-major from shared memory)
+// and finally writes O / l and the natural-log LSE.
 #include "attention_common.cuh"
 #include "../../include/dolomite_b200.h"
 
@@ -14,7 +14,7 @@ using namespace dolo;
 
 namespace {
 
-constexpr int FWD_THREADS = 192;
+constexpr int FWD_THREADS = 256;
 constexpr int KV_STAGES = 2;
 
 struct FwdParams {
@@ -28,18 +28,16 @@ struct FwdParams {
     float scale_log2;  // softmax_scale * log2(e)
     float scale;
     AttnDropout drop;  // threshold 0: none
-    int head_chunk;    // CTA order (attention_common.cuh: attn_cta_order): heads per chunk, 0 = tiles fastest (round 1)
+    int head_chunk;    // CTA order (attention_common.cuh: attn_cta_order): heads per chunk, 0 = tiles fastest
     int n_tile_slots;  // upper bound of the number of query tiles (the grid has n_tile_slots x n_heads CTAs)
 };
 
 template <int HD>
-__global__ void __launch_bounds__(FWD_THREADS)
+__global__ void __launch_bounds__(FWD_THREADS, 1)
     attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap64, const __grid_constant__ CUtensorMap tmapR,
                     const FwdParams p) {
     using CH = HeadChunks<HD>;
-    constexpr int TILE_BYTES = CH::TILE_BYTES;
-    constexpr int TMEM_COLS = (128 + HD) <= 256 ? 256 : 512;
-    constexpr uint32_t O_COL = 128;
+    constexpr int TILE_BYTES = CH::tile_bytes(ATT_TILE);
 
     int ti, head;
     attn_cta_order(p.head_chunk, p.n_tile_slots, ti, head);
@@ -50,680 +48,164 @@ __global__ void __launch_bounds__(FWD_THREADS)
     const int q_col = (group * (p.q_per_group + 2) + slot) * HD;
     const int k_col = (group * (p.q_per_group + 2) + p.q_per_group) * HD;
     const int v_col = k_col + HD;
-    const int q0 = loc.tile * ATT_TILE;                       // first query (doc-relative) of this tile
-    const int n_kv = loc.tile + 1;                            // causal: key tiles 0 .. tile
-    const int row_base = loc.doc_start + q0;                  // global token row of query 0
+    const int q0 = loc.tile * ATT_TILE;  // first query (doc-relative) of this tile
+    const int n_kv = loc.tile + 1;       // causal: key tiles 0 .. tile
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_align_1024(smem_raw);
     uint8_t* sQ = smem;
-    uint8_t* sK = sQ + TILE_BYTES;                 // [KV_STAGES]
-    uint8_t* sV = sK + KV_STAGES * TILE_BYTES;     // [KV_STAGES]
+    uint8_t* sK = sQ + TILE_BYTES;              // [KV_STAGES]
+    uint8_t* sV = sK + KV_STAGES * TILE_BYTES;  // [KV_STAGES]
     uint64_t* bars = reinterpret_cast<uint64_t*>(sV + KV_STAGES * TILE_BYTES);
-    uint64_t* q_full = bars;            // 1
-    uint64_t* kv_full = bars + 1;       // [KV_STAGES]
-    uint64_t* kv_empty = bars + 3;      // [KV_STAGES]
-    uint64_t* s_full = bars + 5;        // 1
-    uint64_t* p_ready = bars + 6;       // 1 (128 arrivals)
-    uint64_t* o_full = bars + 7;        // 1
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
+    uint64_t* q_full = bars;        // 1
+    uint64_t* kv_full = bars + 1;   // [KV_STAGES]
+    uint64_t* kv_empty = bars + 3;  // [KV_STAGES], one arrive per warp
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-    if (warp == 0 && lane == 0) {
+    auto load_kv = [&](int j, int s) {
+        mbar_expect_tx(&kv_full[s], 2 * TILE_BYTES);
+        tma_load_chunked<HD, ATT_TILE>(sK + s * TILE_BYTES, &tmap64, &tmapR, &kv_full[s], k_col, loc.doc_start + j * ATT_TILE);
+        tma_load_chunked<HD, ATT_TILE>(sV + s * TILE_BYTES, &tmap64, &tmapR, &kv_full[s], v_col, loc.doc_start + j * ATT_TILE);
+    };
+    if (threadIdx.x == 0) {
         if (CH::NC64 > 0) tma_prefetch_desc(&tmap64);
         if (CH::REM > 0) tma_prefetch_desc(&tmapR);
         mbar_init(q_full, 1);
         for (int i = 0; i < KV_STAGES; ++i) {
             mbar_init(&kv_full[i], 1);
-            mbar_init(&kv_empty[i], 1);
+            mbar_init(&kv_empty[i], FWD_THREADS / 32);
         }
-        mbar_init(s_full, 1);
-        mbar_init(p_ready, 128);
-        mbar_init(o_full, 1);
         mbar_fence_init();
+        mbar_expect_tx(q_full, TILE_BYTES);
+        tma_load_chunked<HD, ATT_TILE>(sQ, &tmap64, &tmapR, q_full, q_col, loc.doc_start + q0);
+        for (int j = 0; j < KV_STAGES && j < n_kv; ++j) load_kv(j, j);
     }
-    if (warp == 1) tmem_alloc<TMEM_COLS>(tmem_slot);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    auto load_tile = [&](uint8_t* dst, uint64_t* bar, int col, int row) {
+    const int wr = (warp & 3) * 16 + (lane >> 2);  // first of the two accumulator rows of this thread (and wr + 8)
+    const int wc = 2 * (lane & 3);                 // first accumulator column inside each n8 block
+    const int qr[2] = {q0 + wg * 64 + wr, q0 + wg * 64 + wr + 8};  // doc-relative queries of the two rows
+    const bool drop = p.drop.threshold != 0;
+    const uint32_t head_key = dropout_head_key(uint32_t(head), p.drop.key0, p.drop.key1);
+    const uint32_t sq = smem_u32(sQ);
+
+    float o[HD / 2];
+#pragma unroll
+    for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};  // raw-score row max, thread-partial row sum
+
+    mbar_wait(q_full, 0, 10);
+    for (int j = 0; j < n_kv; ++j) {
+        const int s = j & (KV_STAGES - 1);
+        mbar_wait(&kv_full[s], (j / KV_STAGES) & 1, 11);
+        const uint32_t sk = smem_u32(sK + s * TILE_BYTES), sv = smem_u32(sV + s * TILE_BYTES);
+        float sc[ATT_TILE / 2];
+        wgmma_fence();
 #pragma unroll
         for (int c = 0; c < CH::NCHUNK; ++c) {
-            const CUtensorMap* m = (c < CH::NC64) ? &tmap64 : &tmapR;
-            tma_load_2d(dst + CH::offset(c), m, bar, col + CH::col(c), row);
+            const int w = CH::width(c);
+#pragma unroll
+            for (int k = 0; k < w / 16; ++k)
+                wgmma_ss<ATT_TILE, 0, 0>(sc, chunk_desc_kmajor(sq + CH::offset(c, ATT_TILE) + wg * 64 * 2 * w, w, k),
+                                         chunk_desc_kmajor(sk + CH::offset(c, ATT_TILE), w, k), (c != 0 || k != 0) ? 1u : 0u);
         }
-    };
+        wgmma_commit();
+        wgmma_wait<0>();
+        reg_fence<ATT_TILE / 2>(sc);
 
-    if (warp == 0) {
-        if (elect_one()) {
-            mbar_expect_tx(q_full, TILE_BYTES);
-            load_tile(sQ, q_full, q_col, row_base);
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int j = 0; j < n_kv; ++j) {
-                mbar_wait(&kv_empty[stage], phase ^ 1, 10);
-                mbar_expect_tx(&kv_full[stage], 2 * TILE_BYTES);
-                const int krow = loc.doc_start + j * ATT_TILE;
-                load_tile(sK + stage * TILE_BYTES, &kv_full[stage], k_col, krow);
-                load_tile(sV + stage * TILE_BYTES, &kv_full[stage], v_col, krow);
-                if (++stage == KV_STAGES) { stage = 0; phase ^= 1; }
+        // ---------------- online softmax over this key tile ----------------
+        const bool diag = j == loc.tile;  // only the diagonal tile has keys past a query of the tile
+        const int kbase = j * ATT_TILE + wc;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            float mx = m_run[h];
+#pragma unroll
+            for (int b = 0; b < ATT_TILE / 8; ++b)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    float& x = sc[4 * b + 2 * h + e];
+                    if (diag && kbase + 8 * b + e > qr[h]) x = -INFINITY;
+                    mx = fmaxf(mx, x);
+                }
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+            // key 0 of every tile j <= tile precedes every query of the tile: the row max is finite from tile 0 on
+            const float corr = fast_exp2((m_run[h] - mx) * p.scale_log2);
+            const float neg_m = -mx * p.scale_log2;
+            float lsum = 0.f;
+#pragma unroll
+            for (int b = 0; b < ATT_TILE / 8; ++b)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    float& x = sc[4 * b + 2 * h + e];
+                    float pr = fast_exp2(fmaf(x, p.scale_log2, neg_m));  // exp2(-inf) = 0 for masked keys
+                    lsum += pr;
+                    if (drop)  // the row sum above is that of the undropped probabilities
+                        pr *= attn_drop_scale(p.drop, head_key, loc.doc_start + qr[h], loc.doc_start + kbase + 8 * b + e);
+                    x = pr;
+                }
+            l_run[h] = l_run[h] * corr + lsum;
+            m_run[h] = mx;
+#pragma unroll
+            for (int b = 0; b < HD / 8; ++b) {
+                o[4 * b + 2 * h] *= corr;
+                o[4 * b + 2 * h + 1] *= corr;
             }
         }
-    } else if (warp == 1) {
-        if (elect_one()) {  // uniform single-thread region: no per-MMA R2UR waterfall loops
-            constexpr uint32_t idesc_qk = umma_idesc_bf16(128, 128, false, false);
-            mbar_wait(q_full, 0, 11);
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int j = 0; j < n_kv; ++j) {
-                mbar_wait(&kv_full[stage], phase, 12);
-                tc_fence_after();
-                const uint32_t q_s = smem_u32(sQ);
-                const uint32_t k_s = smem_u32(sK + stage * TILE_BYTES);
-                const uint32_t v_s = smem_u32(sV + stage * TILE_BYTES);
-                // S = Q K^T  (contraction over head_dim, chunk by chunk)
-                bool first = true;
+        uint32_t pa[ATT_TILE / 16][4];
 #pragma unroll
-                for (int c = 0; c < CH::NCHUNK; ++c) {
-                    const int w = CH::width(c);
+        for (int kk = 0; kk < ATT_TILE / 16; ++kk) acc_to_a_frag(sc, kk, pa[kk]);
+
+        // ---------------- O += P V_j ----------------
+        wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < w / 16; ++k) {
-                        umma_ss(tmem_base, chunk_desc_kmajor(q_s + CH::offset(c), w, k),
-                                chunk_desc_kmajor(k_s + CH::offset(c), w, k), idesc_qk, first ? 0u : 1u);
-                        first = false;
-                    }
-                }
-                umma_commit(s_full);
-                // wait for P_j (bf16, TMEM columns [0,64)) and the rescaled O
-                mbar_wait(p_ready, uint32_t(j & 1), 13);
-                tc_fence_after();
+        for (int c = 0; c < CH::NCHUNK; ++c) {
 #pragma unroll
-                for (int c = 0; c < CH::NCHUNK; ++c) {
-                    const int w = CH::width(c);
-                    const uint32_t idesc_pv = umma_idesc_bf16(128, w, false, true);
-#pragma unroll
-                    for (int k = 0; k < ATT_TILE / 16; ++k) {
-                        umma_ts(tmem_base + O_COL + CH::col(c), tmem_base + k * 8,
-                                chunk_desc_mnmajor(v_s + CH::offset(c), w, k), idesc_pv, (j > 0 || k > 0) ? 1u : 0u);
-                    }
-                }
-                umma_commit(&kv_empty[stage]);
-                if (j == n_kv - 1) umma_commit(o_full);
-                if (++stage == KV_STAGES) { stage = 0; phase ^= 1; }
+            for (int kk = 0; kk < ATT_TILE / 16; ++kk) {
+                if (CH::width(c) == 64)
+                    wgmma_rs<64, 1>(o + CH::col(c) / 2, pa[kk], chunk_desc_mnmajor(sv + CH::offset(c, ATT_TILE), 64, kk), 1u);
+                else
+                    wgmma_rs<(CH::REM ? CH::REM : 16), 1>(o + CH::col(c) / 2, pa[kk],
+                                                          chunk_desc_mnmajor(sv + CH::offset(c, ATT_TILE), CH::REM, kk), 1u);
             }
         }
-    } else {
-        // ---------------- softmax / correction / epilogue: one query row per thread ----------------
-        const int sub = warp & 3;
-        const int r = sub * 32 + lane;                 // row in tile == TMEM lane
-        const uint32_t t_lane = tmem_base + (uint32_t(sub * 32) << 16);
-        const int qi = q0 + r;                         // doc-relative query index
-        float m_run = -INFINITY, l_run = 0.f;
-        const bool drop = p.drop.threshold != 0;  // dropout: every tile takes the per-element path below
-        const uint32_t head_key = dropout_head_key(uint32_t(head), p.drop.key0, p.drop.key1);
-        for (int j = 0; j < n_kv; ++j) {
-            mbar_wait(s_full, uint32_t(j & 1), 14);
-            tc_fence_after();
-            const bool diag = (j == n_kv - 1);
-            const int kbase = j * ATT_TILE;
-            // pass 1: row max.  Only the diagonal tile needs the causal mask; interior tiles take the mask-free path
-            // (ncu on the first version: 13.7 instructions per score, most of them per-element mask selects).
-            float mx = m_run;
-            if (!diag) {
-                // software-pipelined TMEM reads: chunk ch+1 is in flight while chunk ch is reduced (the exposed
-                // tcgen05.ld latency, not issue slots, bounded the first version: ncu issue-active 37 %)
-                float mx1 = -INFINITY, mx2 = -INFINITY, mx3 = -INFINITY;
-                uint32_t va[32], vb[32];
-                auto fold = [&](const uint32_t (&v)[32]) {  // 3-input FMNMX3: half the instructions of a max chain
-#pragma unroll
-                    for (int i = 0; i < 32; i += 8) {
-                        mx = fmax3(mx, __uint_as_float(v[i]), __uint_as_float(v[i + 1]));
-                        mx1 = fmax3(mx1, __uint_as_float(v[i + 2]), __uint_as_float(v[i + 3]));
-                        mx2 = fmax3(mx2, __uint_as_float(v[i + 4]), __uint_as_float(v[i + 5]));
-                        mx3 = fmax3(mx3, __uint_as_float(v[i + 6]), __uint_as_float(v[i + 7]));
-                    }
-                };
-                tmem_ld32(t_lane, va);
-                tmem_ld_wait();
-                reg_fence32(va);
-                tmem_ld32(t_lane + 32, vb);
-                fold(va);
-                tmem_ld_wait();
-                reg_fence32(vb);
-                tmem_ld32(t_lane + 64, va);
-                fold(vb);
-                tmem_ld_wait();
-                reg_fence32(va);
-                tmem_ld32(t_lane + 96, vb);
-                fold(va);
-                tmem_ld_wait();
-                reg_fence32(vb);
-                fold(vb);
-                mx = fmaxf(fmaxf(mx, mx1), fmaxf(mx2, mx3));
-            } else {
-#pragma unroll 1
-                for (int ch = 0; ch < 4; ++ch) {
-                    uint32_t v[32];
-                    tmem_ld32(t_lane + ch * 32, v);
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) {
-                        float s = __uint_as_float(v[i]);
-                        if (kbase + ch * 32 + i > qi) s = -INFINITY;
-                        mx = fmaxf(mx, s);
-                    }
-                }
-            }
-            // Lazy reference maximum: the exponent reference of a row only moves when the tile's maximum exceeds it by more
-            // than 2^8 (FlashAttention-4's thresholded rescale).  P then stays <= 256 (exact in bf16's exponent range, fp32
-            // sums), O and l are rescaled a handful of times per row instead of once per tile for most warps -- with random
-            // scores some row of a warp sets a new maximum in ~90 % of the tiles, so the "all alpha == 1" skip below almost
-            // never fired (ncu: the O rescale was 14 % of the softmax warps' samples).  mx is finite for every valid row.
-            const bool move_ref = (m_run == -INFINITY) || (mx * p.scale_log2 > m_run * p.scale_log2 + 8.f);
-            const float m_new = move_ref ? mx : m_run;
-            const float m_scaled = (m_new == -INFINITY) ? 0.f : m_new * p.scale_log2;
-            // (alpha must be EXACTLY 1 when the reference stays: `m_run * scale - m_scaled` contracts to an FMA whose result is the
-            //  rounding error of the product, not 0 -- the ncu capture of call 73 showed the "skipped" rescale running on 93 %
-            //  of the tiles for that reason)
-            const float alpha = !move_ref ? 1.f : ((m_run == -INFINITY) ? 0.f : fast_exp2(m_run * p.scale_log2 - m_scaled));
-            // rescale O (previous PV has completed: s_full is committed after it); skipped when no row of this
-            // warp raised its running max (alpha == 1 everywhere), which is the common case after the first tiles
-            if (j > 0 && !__all_sync(0xffffffffu, alpha == 1.f)) {
-#pragma unroll 1
-                for (int c0 = 0; c0 < HD; c0 += 16) {
-                    uint32_t o[16];
-                    tmem_ld16(t_lane + O_COL + c0, o);
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-                    tmem_st16(t_lane + O_COL + c0, o);
-                }
-            }
-            // pass 2: P = exp2(s*scale - m), row sum; P (bf16) overwrites the already-consumed S columns
-            float lsum = 0.f, lsum1 = 0.f;
-            const float neg_m = -m_scaled;
-            if (!diag && !drop) {
-                uint32_t va[32], vb[32];
-                auto expo = [&](const uint32_t (&v)[32], int ch) {
-                    uint32_t pk[16];
-#pragma unroll
-                    for (int i = 0; i < 32; i += 2) {  // packed fp32 pipes: FFMA2 for scale/shift, FADD2 for the row sums
-                        float x0, x1;
-                        ffma2_bcast(x0, x1, __uint_as_float(v[i]), __uint_as_float(v[i + 1]), p.scale_log2, neg_m);
-                        const float p0 = fast_exp2(x0), p1 = fast_exp2(x1);
-                        fadd2(lsum, lsum1, p0, p1);
-                        pk[i >> 1] = pack_bf16(p0, p1);
-                    }
-                    tmem_st16(t_lane + ch * 16, pk);  // bf16 P chunk ch aliases fp32 S columns [16ch, 16ch+16): consumed
-                };
-                tmem_ld32(t_lane, va);
-                tmem_ld_wait();
-                reg_fence32(va);
-                tmem_ld32(t_lane + 32, vb);
-                expo(va, 0);
-                tmem_ld_wait();
-                reg_fence32(vb);
-                tmem_ld32(t_lane + 64, va);
-                expo(vb, 1);
-                tmem_ld_wait();
-                reg_fence32(va);
-                tmem_ld32(t_lane + 96, vb);
-                expo(va, 2);
-                tmem_ld_wait();
-                reg_fence32(vb);
-                expo(vb, 3);
-            } else {
-#pragma unroll 1
-                for (int ch = 0; ch < 4; ++ch) {
-                    uint32_t v[32];
-                    tmem_ld32(t_lane + ch * 32, v);
-                    tmem_ld_wait();
-                    uint32_t pk[16];
-#pragma unroll
-                    for (int i = 0; i < 32; i += 2) {
-                        float p0 = fast_exp2(fmaf(__uint_as_float(v[i]), p.scale_log2, neg_m));
-                        float p1 = fast_exp2(fmaf(__uint_as_float(v[i + 1]), p.scale_log2, neg_m));
-                        if (kbase + ch * 32 + i > qi) p0 = 0.f;  // (never true off the diagonal tile)
-                        if (kbase + ch * 32 + i + 1 > qi) p1 = 0.f;
-                        lsum += p0;
-                        lsum1 += p1;
-                        if (drop) {  // the row sum above is that of the undropped probabilities
-                            const int kt = loc.doc_start + kbase + ch * 32 + i;
-                            p0 *= attn_drop_scale(p.drop, head_key, row_base + r, kt);
-                            p1 *= attn_drop_scale(p.drop, head_key, row_base + r, kt + 1);
-                        }
-                        pk[i >> 1] = pack_bf16(p0, p1);
-                    }
-                    tmem_st16(t_lane + ch * 16, pk);
-                }
-            }
-            lsum += lsum1;
-            l_run = l_run * alpha + lsum;
-            m_run = m_new;
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive(p_ready);
+        wgmma_commit();
+        wgmma_wait<0>();
+        reg_fence<HD / 2>(o);
+        if (lane == 0) mbar_arrive(&kv_empty[s]);
+        if (threadIdx.x == 0 && j + KV_STAGES < n_kv) {
+            mbar_wait(&kv_empty[s], (j / KV_STAGES) & 1, 12);  // both warpgroups are done with tile j
+            load_kv(j + KV_STAGES, s);
         }
-        // ---------------- epilogue ----------------
-        mbar_wait(o_full, 0, 15);
-        tc_fence_after();
-        const bool row_ok = qi < loc.doc_len;
-        const float inv_l = l_run > 0.f ? 1.f / l_run : 0.f;
-        __nv_bfloat16* orow = p.out + int64_t(row_base + r) * (int64_t(p.n_heads) * HD) + int64_t(head) * HD;
-#pragma unroll 1
-        for (int c0 = 0; c0 < HD; c0 += 16) {
-            uint32_t o[16];
-            tmem_ld16(t_lane + O_COL + c0, o);
-            tmem_ld_wait();
-            if (row_ok) {
-                uint4 a, b;
-                a.x = pack_bf16(__uint_as_float(o[0]) * inv_l, __uint_as_float(o[1]) * inv_l);
-                a.y = pack_bf16(__uint_as_float(o[2]) * inv_l, __uint_as_float(o[3]) * inv_l);
-                a.z = pack_bf16(__uint_as_float(o[4]) * inv_l, __uint_as_float(o[5]) * inv_l);
-                a.w = pack_bf16(__uint_as_float(o[6]) * inv_l, __uint_as_float(o[7]) * inv_l);
-                b.x = pack_bf16(__uint_as_float(o[8]) * inv_l, __uint_as_float(o[9]) * inv_l);
-                b.y = pack_bf16(__uint_as_float(o[10]) * inv_l, __uint_as_float(o[11]) * inv_l);
-                b.z = pack_bf16(__uint_as_float(o[12]) * inv_l, __uint_as_float(o[13]) * inv_l);
-                b.w = pack_bf16(__uint_as_float(o[14]) * inv_l, __uint_as_float(o[15]) * inv_l);
-                *reinterpret_cast<uint4*>(orow + c0) = a;
-                *reinterpret_cast<uint4*>(orow + c0 + 8) = b;
-            }
-        }
-        if (row_ok) p.lse[int64_t(head) * p.T + row_base + r] = m_run * p.scale + logf(l_run);
+        __syncwarp();
     }
 
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc<TMEM_COLS>(tmem_base);
+    // ---------------- epilogue: O / l, LSE ----------------
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        float l = l_run[h];
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        if (qr[h] >= loc.doc_len) continue;
+        const float inv_l = l > 0.f ? 1.f / l : 0.f;
+        const int64_t row = loc.doc_start + qr[h];
+        __nv_bfloat16* orow = p.out + row * (int64_t(p.n_heads) * HD) + int64_t(head) * HD + wc;
+#pragma unroll
+        for (int b = 0; b < HD / 8; ++b)
+            *reinterpret_cast<uint32_t*>(orow + 8 * b) = pack_bf16(o[4 * b + 2 * h] * inv_l, o[4 * b + 2 * h + 1] * inv_l);
+        if ((lane & 3) == 0) p.lse[int64_t(head) * p.T + row] = m_run[h] * p.scale + logf(l);
     }
-}
-
-// ------------------------------------------------------------------------------------------------------------------------
-// Split-softmax forward (head_dim >= 64).  ncu of the kernel above (profiles/r02_ncu_kernels_hd80_call70.txt): tensor pipe
-// 25 %, issue slots 36 %, the four softmax warps stalled on the dependent chain  S MMA -> TMEM load -> max -> exp -> TMEM
-// store -> fence -> arrive -> PV MMA -> S MMA of the next tile  (~5600 cycles per tile and CTA, hidden only by a second CTA
-// on the SM).  This kernel breaks the chain inside ONE CTA per SM:
-//   * S is double buffered in TMEM (columns 0-127 / 128-255, O behind them): the MMA warp issues S(j+1) = Q K_{j+1}^T BEFORE
-//     it waits for P(j), so the tensor pipe computes the next scores while the softmax warps work on the current ones;
-//   * EIGHT softmax warps: two threads per query row (same TMEM lanes, warps w and w+4), each owning 64 of the 128 key
-//     columns -- half the dependent work per thread and two warps per scheduler; the row maximum is exchanged through shared
-//     memory inside the warp pair (64-thread named barrier), row sums are only combined in the epilogue;
-//   * lazy reference maximum (threshold 2^8) so that O in TMEM is rescaled a handful of times per row.
-// P(j) (bf16) overwrites the S columns its own thread has consumed; the PV MMA reads it with one TMEM address per 16-key step.
-// ------------------------------------------------------------------------------------------------------------------------
-// NT = threads per query row (2 or 4): 4 NT softmax warps, thread g of a row owns the 128 / NT key columns [g 128 / NT, ...).
-// NT = 4 halves the dependent chain per thread again and puts four softmax warps on every scheduler.
-template <int NT>
-constexpr int fwd2_threads() {
-    return 64 + 128 * NT;
 }
 
 template <int HD>
-constexpr int fwd2_kv_stages() {
-    return (1024 + (1 + 2 * 3) * HeadChunks<HD>::TILE_BYTES + 8 * ATT_TILE * 4 + 256 <= 232448) ? 3 : 2;
-}
-
-template <int HD, int NT>
-__global__ void __launch_bounds__(fwd2_threads<NT>(), 1)
-    attn_fwd_split_kernel(const __grid_constant__ CUtensorMap tmap64, const __grid_constant__ CUtensorMap tmapR,
-                          const FwdParams p) {
-    static_assert(NT == 2 || NT == 4, "two or four threads per query row");
-    using CH = HeadChunks<HD>;
-    constexpr int TILE_BYTES = CH::TILE_BYTES;
-    constexpr int ST = fwd2_kv_stages<HD>();
-    constexpr int GCOLS = ATT_TILE / NT;  // key columns per thread
-    constexpr int NV = GCOLS / 32;        // 32-column register blocks per thread
-    constexpr uint32_t O_COL = 256;
-    constexpr int NCH16 = HD / 16;               // 16-column chunks of O
-    // O chunks [chunk_lo(g), chunk_lo(g + 1)) belong to column group g (rescale and epilogue)
-    auto chunk_lo = [](int gg) { return (gg * NCH16 + NT - 1) / NT; };
-
-    int ti, head;
-    attn_cta_order(p.head_chunk, p.n_tile_slots, ti, head);
-    ti = p.n_tile_slots - 1 - ti;  // long (late) tiles first
-    const TileLoc loc = locate_tile(p.cu_seqlens, p.n_docs, ti);
-    if (!loc.valid) return;  // uniform for the whole CTA
-    const int group = head / p.q_per_group, slot = head % p.q_per_group;
-    const int q_col = (group * (p.q_per_group + 2) + slot) * HD;
-    const int k_col = (group * (p.q_per_group + 2) + p.q_per_group) * HD;
-    const int v_col = k_col + HD;
-    const int q0 = loc.tile * ATT_TILE;
-    const int n_kv = loc.tile + 1;
-    const int row_base = loc.doc_start + q0;
-
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_align_1024(smem_raw);
-    uint8_t* sQ = smem;
-    uint8_t* sK = sQ + TILE_BYTES;            // [ST]
-    uint8_t* sV = sK + ST * TILE_BYTES;       // [ST]
-    float* xmax = reinterpret_cast<float*>(sV + ST * TILE_BYTES);  // [2 parities][NT groups][128]  row-max exchange
-    uint64_t* bars = reinterpret_cast<uint64_t*>(xmax + 8 * ATT_TILE);
-    uint64_t* q_full = bars;                 // 1
-    uint64_t* kv_full = bars + 1;            // [ST]
-    uint64_t* kv_empty = bars + 1 + ST;      // [ST]
-    uint64_t* s_full = bars + 1 + 2 * ST;    // [2]  S buffer b holds the scores of tile j (b = j & 1)
-    uint64_t* p_ready = s_full + 2;          // [2]  256 arrivals: P written, O rescaled
-    uint64_t* pv_done = p_ready + 2;         // 1    commit after every PV: O is stable again
-    uint64_t* o_full = pv_done + 1;          // 1
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_full + 1);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-    if (warp == 0 && lane == 0) {
-        if (CH::NC64 > 0) tma_prefetch_desc(&tmap64);
-        if (CH::REM > 0) tma_prefetch_desc(&tmapR);
-        mbar_init(q_full, 1);
-        for (int i = 0; i < ST; ++i) {
-            mbar_init(&kv_full[i], 1);
-            mbar_init(&kv_empty[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&s_full[i], 1);
-            mbar_init(&p_ready[i], 128 * NT);
-        }
-        mbar_init(pv_done, 1);
-        mbar_init(o_full, 1);
-        mbar_fence_init();
-    }
-    if (warp == 1) tmem_alloc<512>(tmem_slot);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    auto load_tile = [&](uint8_t* dst, uint64_t* bar, int col, int row) {
-#pragma unroll
-        for (int c = 0; c < CH::NCHUNK; ++c) {
-            const CUtensorMap* m = (c < CH::NC64) ? &tmap64 : &tmapR;
-            tma_load_2d(dst + CH::offset(c), m, bar, col + CH::col(c), row);
-        }
-    };
-
-    if (warp == 0) {
-        if (elect_one()) {
-            mbar_expect_tx(q_full, TILE_BYTES);
-            load_tile(sQ, q_full, q_col, row_base);
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int j = 0; j < n_kv; ++j) {
-                mbar_wait(&kv_empty[stage], phase ^ 1, 50);
-                mbar_expect_tx(&kv_full[stage], 2 * TILE_BYTES);
-                const int krow = loc.doc_start + j * ATT_TILE;
-                load_tile(sK + stage * TILE_BYTES, &kv_full[stage], k_col, krow);
-                load_tile(sV + stage * TILE_BYTES, &kv_full[stage], v_col, krow);
-                if (++stage == ST) { stage = 0; phase ^= 1; }
-            }
-        }
-    } else if (warp == 1) {
-        if (elect_one()) {
-            constexpr uint32_t idesc_qk = umma_idesc_bf16(128, 128, false, false);
-            mbar_wait(q_full, 0, 51);
-            const uint32_t q_s = smem_u32(sQ);
-            // S(jj) = Q K_jj^T into buffer jj & 1; K_jj lives in stage jj % ST (its barrier phase is (jj / ST) & 1)
-            auto issue_S = [&](int jj) {
-                const int stg = jj % ST;
-                mbar_wait(&kv_full[stg], uint32_t(jj / ST) & 1, 52);
-                tc_fence_after();
-                const uint32_t k_s = smem_u32(sK + stg * TILE_BYTES);
-                const uint32_t d = tmem_base + uint32_t(jj & 1) * 128;
-                bool first = true;
-#pragma unroll
-                for (int c = 0; c < CH::NCHUNK; ++c) {
-                    const int w = CH::width(c);
-#pragma unroll
-                    for (int k = 0; k < w / 16; ++k) {
-                        umma_ss(d, chunk_desc_kmajor(q_s + CH::offset(c), w, k), chunk_desc_kmajor(k_s + CH::offset(c), w, k),
-                                idesc_qk, first ? 0u : 1u);
-                        first = false;
-                    }
-                }
-                umma_commit(&s_full[jj & 1]);
-            };
-            issue_S(0);
-            if (n_kv > 1) issue_S(1);
-            for (int j = 0; j < n_kv; ++j) {
-                const int b = j & 1, stg = j % ST;
-                mbar_wait(&p_ready[b], uint32_t(j >> 1) & 1, 53);
-                tc_fence_after();
-                const uint32_t v_s = smem_u32(sV + stg * TILE_BYTES);
-#pragma unroll
-                for (int c = 0; c < CH::NCHUNK; ++c) {
-                    const int w = CH::width(c);
-                    const uint32_t idesc_pv = umma_idesc_bf16(128, w, false, true);
-#pragma unroll
-                    for (int k = 0; k < ATT_TILE / 16; ++k) {
-                        // P of keys [16k, 16k+16): written by the column group that owns them, at the start of its own columns
-                        constexpr int KPG = GCOLS / 16;  // 16-key steps per column group
-                        const uint32_t a_tmem = tmem_base + uint32_t(b) * 128 + uint32_t(k / KPG) * GCOLS + uint32_t(k % KPG) * 8;
-                        umma_ts(tmem_base + O_COL + CH::col(c), a_tmem, chunk_desc_mnmajor(v_s + CH::offset(c), w, k), idesc_pv,
-                                (j > 0 || k > 0) ? 1u : 0u);
-                    }
-                }
-                umma_commit(&kv_empty[stg]);  // K_j (scores done long ago) and V_j are free
-                umma_commit(pv_done);
-                if (j == n_kv - 1) umma_commit(o_full);
-                if (j + 2 < n_kv) issue_S(j + 2);  // reuses buffer b: ordered behind PV(j) on the tensor pipe
-            }
-        }
-    } else {
-        // ---------------- softmax: NT threads per query row, 128 / NT key columns each ----------------
-        const int g = (warp - 2) >> 2;                 // column group
-        const int sub = warp & 3;                      // TMEM sub-partition of this warp (lanes 32 sub .. 32 sub + 31)
-        const int r = sub * 32 + lane;
-        const uint32_t t_lane = tmem_base + (uint32_t(sub * 32) << 16);
-        const int qi = q0 + r;
-        const uint32_t pair_bar = 1 + uint32_t(sub);   // named barrier of the NT warps that share this row block
-        float m_run = -INFINITY, l_run = 0.f;
-        const bool drop = p.drop.threshold != 0;  // dropout: every tile takes the per-element path below
-        const uint32_t head_key = dropout_head_key(uint32_t(head), p.drop.key0, p.drop.key1);
-        for (int j = 0; j < n_kv; ++j) {
-            const int b = j & 1;
-            const uint32_t s_col = t_lane + uint32_t(b) * 128 + uint32_t(g) * GCOLS;
-            mbar_wait(&s_full[b], uint32_t(j >> 1) & 1, 54);
-            tc_fence_after();
-            const bool diag = (j == n_kv - 1);
-            const int kbase = j * ATT_TILE + g * GCOLS;
-            uint32_t v[NV][32];
-#pragma unroll
-            for (int h = 0; h < NV; ++h) tmem_ld32(s_col + h * 32, v[h]);
-            tmem_ld_wait();
-#pragma unroll
-            for (int h = 0; h < NV; ++h) reg_fence32(v[h]);
-            // ---- row maximum over my columns, then over the threads of the row ----
-            float mx = -INFINITY, mx1 = -INFINITY;
-            if (!diag) {
-#pragma unroll
-                for (int h = 0; h < NV; ++h)
-#pragma unroll
-                    for (int i = 0; i < 32; i += 4) {
-                        mx = fmax3(mx, __uint_as_float(v[h][i]), __uint_as_float(v[h][i + 1]));
-                        mx1 = fmax3(mx1, __uint_as_float(v[h][i + 2]), __uint_as_float(v[h][i + 3]));
-                    }
-            } else {
-#pragma unroll
-                for (int h = 0; h < NV; ++h)
-#pragma unroll
-                    for (int i = 0; i < 32; i += 2) {
-                        if (kbase + h * 32 + i <= qi) mx = fmaxf(mx, __uint_as_float(v[h][i]));
-                        if (kbase + h * 32 + i + 1 <= qi) mx1 = fmaxf(mx1, __uint_as_float(v[h][i + 1]));
-                    }
-            }
-            mx = fmaxf(mx, mx1);
-            float* xm = xmax + (b * NT) * ATT_TILE;  // parity-buffered: a partner may still read the previous tile's value
-            xm[g * ATT_TILE + r] = mx;
-            named_bar_sync(pair_bar, 32 * NT);
-#pragma unroll
-            for (int o = 1; o < NT; ++o) mx = fmaxf(mx, xm[((g + o) % NT) * ATT_TILE + r]);
-            mx = fmaxf(mx, m_run);
-            // lazy reference maximum (see attn_fwd_kernel): identical in all threads of the row
-            const bool move_ref = (m_run == -INFINITY) || (mx * p.scale_log2 > m_run * p.scale_log2 + 8.f);
-            const float m_new = move_ref ? mx : m_run;
-            const float m_scaled = (m_new == -INFINITY) ? 0.f : m_new * p.scale_log2;
-            // (alpha must be EXACTLY 1 when the reference stays: `m_run * scale - m_scaled` contracts to an FMA whose result is the
-            //  rounding error of the product, not 0 -- the ncu capture of call 73 showed the "skipped" rescale running on 93 %
-            //  of the tiles for that reason)
-            const float alpha = !move_ref ? 1.f : ((m_run == -INFINITY) ? 0.f : fast_exp2(m_run * p.scale_log2 - m_scaled));
-            if (j > 0) {
-                mbar_wait(pv_done, uint32_t(j - 1) & 1, 55);  // PV(j-1) has retired: O may be rescaled, P(j) may be handed over
-                tc_fence_after();
-                if (!__all_sync(0xffffffffu, alpha == 1.f)) {
-#pragma unroll 1
-                    for (int c = chunk_lo(g); c < chunk_lo(g + 1); ++c) {
-                        uint32_t o[16];
-                        tmem_ld16(t_lane + O_COL + c * 16, o);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-                        tmem_st16(t_lane + O_COL + c * 16, o);
-                    }
-                }
-            }
-            // ---- P = exp2(s * scale - m), row sum over my columns; bf16 P overwrites my own consumed S columns ----
-            float lsum = 0.f, lsum1 = 0.f;
-            const float neg_m = -m_scaled;
-            uint32_t pk[16];
-            if (!diag && !drop) {
-#pragma unroll
-                for (int h = 0; h < NV; ++h) {
-#pragma unroll
-                    for (int i = 0; i < 32; i += 2) {
-                        float x0, x1;
-                        ffma2_bcast(x0, x1, __uint_as_float(v[h][i]), __uint_as_float(v[h][i + 1]), p.scale_log2, neg_m);
-                        const float p0 = fast_exp2(x0), p1 = fast_exp2(x1);
-                        fadd2(lsum, lsum1, p0, p1);
-                        pk[i >> 1] = pack_bf16(p0, p1);
-                    }
-                    tmem_st16(s_col + h * 16, pk);
-                }
-            } else {
-#pragma unroll
-                for (int h = 0; h < NV; ++h) {
-#pragma unroll
-                    for (int i = 0; i < 32; i += 2) {
-                        float p0 = fast_exp2(fmaf(__uint_as_float(v[h][i]), p.scale_log2, neg_m));
-                        float p1 = fast_exp2(fmaf(__uint_as_float(v[h][i + 1]), p.scale_log2, neg_m));
-                        if (kbase + h * 32 + i > qi) p0 = 0.f;  // (never true off the diagonal tile)
-                        if (kbase + h * 32 + i + 1 > qi) p1 = 0.f;
-                        lsum += p0;
-                        lsum1 += p1;
-                        if (drop) {
-                            p0 *= attn_drop_scale(p.drop, head_key, row_base + r, loc.doc_start + kbase + h * 32 + i);
-                            p1 *= attn_drop_scale(p.drop, head_key, row_base + r, loc.doc_start + kbase + h * 32 + i + 1);
-                        }
-                        pk[i >> 1] = pack_bf16(p0, p1);
-                    }
-                    tmem_st16(s_col + h * 16, pk);
-                }
-            }
-            l_run = l_run * alpha + (lsum + lsum1);
-            m_run = m_new;
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive(&p_ready[b]);
-        }
-        // ---------------- epilogue: combine the partial row sums, each thread stores its share of the O columns ----------------
-        mbar_wait(o_full, 0, 56);
-        tc_fence_after();
-        float* xs = xmax + ((n_kv & 1) * NT) * ATT_TILE;  // the parity buffer the last tile did not use
-        xs[g * ATT_TILE + r] = l_run;
-        named_bar_sync(pair_bar, 32 * NT);
-        float l_tot = 0.f;
-#pragma unroll
-        for (int o = 0; o < NT; ++o) l_tot += xs[o * ATT_TILE + r];  // same order in every thread of the row
-        const bool row_ok = qi < loc.doc_len;
-        const float inv_l = l_tot > 0.f ? 1.f / l_tot : 0.f;
-        __nv_bfloat16* orow = p.out + int64_t(row_base + r) * (int64_t(p.n_heads) * HD) + int64_t(head) * HD;
-#pragma unroll 1
-        for (int c = chunk_lo(g); c < chunk_lo(g + 1); ++c) {
-            uint32_t o[16];
-            tmem_ld16(t_lane + O_COL + c * 16, o);
-            tmem_ld_wait();
-            if (row_ok) {
-                uint4 a, b4;
-                a.x = pack_bf16(__uint_as_float(o[0]) * inv_l, __uint_as_float(o[1]) * inv_l);
-                a.y = pack_bf16(__uint_as_float(o[2]) * inv_l, __uint_as_float(o[3]) * inv_l);
-                a.z = pack_bf16(__uint_as_float(o[4]) * inv_l, __uint_as_float(o[5]) * inv_l);
-                a.w = pack_bf16(__uint_as_float(o[6]) * inv_l, __uint_as_float(o[7]) * inv_l);
-                b4.x = pack_bf16(__uint_as_float(o[8]) * inv_l, __uint_as_float(o[9]) * inv_l);
-                b4.y = pack_bf16(__uint_as_float(o[10]) * inv_l, __uint_as_float(o[11]) * inv_l);
-                b4.z = pack_bf16(__uint_as_float(o[12]) * inv_l, __uint_as_float(o[13]) * inv_l);
-                b4.w = pack_bf16(__uint_as_float(o[14]) * inv_l, __uint_as_float(o[15]) * inv_l);
-                *reinterpret_cast<uint4*>(orow + c * 16) = a;
-                *reinterpret_cast<uint4*>(orow + c * 16 + 8) = b4;
-            }
-        }
-        if (g == 0 && row_ok) p.lse[int64_t(head) * p.T + row_base + r] = m_run * p.scale + logf(l_tot);
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc<512>(tmem_base);
-    }
-}
-
-template <int HD, int NT>
-int launch_fwd_split(const void* qkv, int64_t row_stride, const FwdParams& p, cudaStream_t st) {
+int launch_fwd(const void* qkv, int64_t row_stride, const FwdParams& p, cudaStream_t st) {
     using CH = HeadChunks<HD>;
     CUtensorMap t64, tR;
-    uint64_t dims[2] = {uint64_t(row_stride), uint64_t(p.T)};
-    uint64_t strides[2] = {2, uint64_t(row_stride) * 2};
-    uint32_t box[2] = {64, ATT_TILE};
-    int rc;
-    if (CH::NC64 > 0) {
-        rc = dolo_make_tmap(&t64, qkv, 2, 2, dims, strides, box, DOLO_SW_128);
-        if (rc) return rc;
-    }
-    if (CH::REM > 0) {
-        box[0] = CH::REM;
-        rc = dolo_make_tmap(&tR, qkv, 2, 2, dims, strides, box, CH::REM == 32 ? DOLO_SW_64 : DOLO_SW_32);
-        if (rc) return rc;
-    }
-    if (CH::NC64 == 0) t64 = tR;
-    if (CH::REM == 0) tR = t64;
-    constexpr int ST = fwd2_kv_stages<HD>();
-    constexpr int smem_bytes = 1024 + (1 + 2 * ST) * CH::TILE_BYTES + 8 * ATT_TILE * 4 + 256;
-    static_assert(smem_bytes <= 232448, "attention forward (split softmax) shared memory budget exceeded");
-    auto kern = attn_fwd_split_kernel<HD, NT>;
-    static bool attr_set = false;
-    if (!attr_set) {
-        DOLO_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-        attr_set = true;
-    }
-    const int64_t max_tiles = (p.T + ATT_TILE - 1) / ATT_TILE + p.n_docs;
-    DOLO_REQUIRE(max_tiles == p.n_tile_slots && max_tiles * p.n_heads < (1ll << 31), "attn_fwd: grid too large");
-    dim3 grid((unsigned)(max_tiles * p.n_heads));
-    kern<<<grid, fwd2_threads<NT>(), smem_bytes, st>>>(t64, tR, p);
-    DOLO_LAUNCH_OK("attn_varlen_fwd_split");
-    return DOLO_OK;
-}
-
-template <int HD>
-int launch_fwd(const void* qkv, int64_t row_stride, const FwdParams& p, int max_seqlen, cudaStream_t st) {
-    using CH = HeadChunks<HD>;
-    CUtensorMap t64, tR;
-    uint64_t dims[2] = {uint64_t(row_stride), uint64_t(p.T)};
-    uint64_t strides[2] = {2, uint64_t(row_stride) * 2};
-    uint32_t box[2] = {64, ATT_TILE};
-    int rc;
-    if (CH::NC64 > 0) {
-        rc = dolo_make_tmap(&t64, qkv, 2, 2, dims, strides, box, DOLO_SW_128);
-        if (rc) return rc;
-    }
-    if (CH::REM > 0) {
-        box[0] = CH::REM;
-        rc = dolo_make_tmap(&tR, qkv, 2, 2, dims, strides, box, CH::REM == 32 ? DOLO_SW_64 : DOLO_SW_32);
-        if (rc) return rc;
-    }
-    if (CH::NC64 == 0) t64 = tR;
-    if (CH::REM == 0) tR = t64;
-    constexpr int smem_bytes = 1024 + (1 + 2 * KV_STAGES) * CH::TILE_BYTES + 128;
+    int rc = attn_make_maps<HD>(qkv, row_stride, p.T, &t64, &tR);
+    if (rc) return rc;
+    constexpr int smem_bytes = 1024 + (1 + 2 * KV_STAGES) * CH::tile_bytes(ATT_TILE) + 128;
+    static_assert(smem_bytes <= 232448, "attention forward shared memory budget exceeded");
     auto kern = attn_fwd_kernel<HD>;
     static bool attr_set = false;
     if (!attr_set) {
@@ -736,7 +218,6 @@ int launch_fwd(const void* qkv, int64_t row_stride, const FwdParams& p, int max_
     dim3 grid((unsigned)(max_tiles * p.n_heads));
     kern<<<grid, FWD_THREADS, smem_bytes, st>>>(t64, tR, p);
     DOLO_LAUNCH_OK("attn_varlen_fwd");
-    (void)max_seqlen;
     return DOLO_OK;
 }
 
@@ -781,28 +262,17 @@ extern "C" int dolomite_b200_attn_varlen_fwd_dropout(const void* qkv, int64_t ro
     p.n_tile_slots = int((T + ATT_TILE - 1) / ATT_TILE + n_docs);
     p.head_chunk = attn_head_chunk(dolo_option_attn_head_fastest(), p.n_heads, q_per_group);
     // all heads in one chunk when the K / V of the whole batch stay in L2 anyway (GQA / short batches): nothing to lose to
-    // re-reads, and the longest-first order then spans every head (Llama-3-8B shape: 0.707 -> 0.666 ms, call 87)
-    if (p.head_chunk > 0 && T * int64_t(n_groups) * head_dim * 4 <= (64ll << 20)) p.head_chunk = p.n_heads;
+    // re-reads, and the longest-first order then spans every head
+    if (p.head_chunk > 0 && T * int64_t(n_groups) * head_dim * 4 <= (24ll << 20)) p.head_chunk = p.n_heads;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int split = dolo_option_attn_fwd_split();
+    (void)max_seqlen;
     switch (head_dim) {
-        case 16: return launch_fwd<16>(qkv, row_stride, p, max_seqlen, st);
-        case 32: return launch_fwd<32>(qkv, row_stride, p, max_seqlen, st);
-        // head_dim 64 / 80: the single-buffer kernel fits two CTAs per SM, which overlap each other; measured faster than the
-        // split kernel there (call 73: 0.323 vs 0.370 ms at hd 80) unless "attn_fwd_split" is set to 2
-        // (split: 0 never / 1 head_dim >= 96 / 2 also 64, 80 -- two threads per row; 3 = like 2 with FOUR threads per row)
-        case 64:
-            if (split >= 3) return launch_fwd_split<64, 4>(qkv, row_stride, p, st);
-            return split >= 2 ? launch_fwd_split<64, 2>(qkv, row_stride, p, st) : launch_fwd<64>(qkv, row_stride, p, max_seqlen, st);
-        case 80:
-            if (split >= 3) return launch_fwd_split<80, 4>(qkv, row_stride, p, st);
-            return split >= 2 ? launch_fwd_split<80, 2>(qkv, row_stride, p, st) : launch_fwd<80>(qkv, row_stride, p, max_seqlen, st);
-        case 96:
-            if (split >= 3) return launch_fwd_split<96, 4>(qkv, row_stride, p, st);
-            return split ? launch_fwd_split<96, 2>(qkv, row_stride, p, st) : launch_fwd<96>(qkv, row_stride, p, max_seqlen, st);
-        case 128:
-            if (split >= 3) return launch_fwd_split<128, 4>(qkv, row_stride, p, st);
-            return split ? launch_fwd_split<128, 2>(qkv, row_stride, p, st) : launch_fwd<128>(qkv, row_stride, p, max_seqlen, st);
+        case 16: return launch_fwd<16>(qkv, row_stride, p, st);
+        case 32: return launch_fwd<32>(qkv, row_stride, p, st);
+        case 64: return launch_fwd<64>(qkv, row_stride, p, st);
+        case 80: return launch_fwd<80>(qkv, row_stride, p, st);
+        case 96: return launch_fwd<96>(qkv, row_stride, p, st);
+        case 128: return launch_fwd<128>(qkv, row_stride, p, st);
         default: return dolo_set_error("attn_fwd: unsupported head_dim %d (supported: 16,32,64,80,96,128)", head_dim);
     }
 }

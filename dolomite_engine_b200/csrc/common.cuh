@@ -1,8 +1,8 @@
-// Shared device/host helpers for the dolomite-b200 C-ABI library (sm_100a only).
+// Shared device/host helpers for the dolomite-b200 C-ABI library (sm_90a, H100).
 //
-// Everything here is hand-written inline PTX for Blackwell: mbarrier, TMA
-// (cp.async.bulk.tensor), tcgen05 (MMA / TMEM alloc / ld / st / commit) and a
-// few vector load/store helpers.  No CUTLASS / CuTe types are used.
+// Everything here is hand-written inline PTX for Hopper: mbarrier, TMA (cp.async.bulk.tensor), wgmma descriptors and
+// fences (the MMA wrappers themselves are in wgmma.cuh) and a few vector load/store helpers.  No CUTLASS / CuTe types
+// are used.
 #pragma once
 
 #include <cuda.h>
@@ -36,25 +36,13 @@ int dolo_check_cuda(cudaError_t e, const char* what);
     } while (0)
 
 int dolo_num_sms();
-int dolo_option_gemm_cta_pair();     // 1 = dense GEMMs use the CTA-pair (cta_group::2) kernel when M >= 256
 // SMs left free by the persistent GEMM grids.  A persistent grid sized to ALL SMs runs up to 2x longer when a
 // communication kernel (NCCL all-gather / reduce-scatter, a few CTAs) occupies some SMs: the GEMM CTAs that do not fit
 // only start when a whole persistent CTA retires.  The sharded data-parallel runtime sets this to NCCL's CTA budget.
 int dolo_option_gemm_sm_margin();
-// 1 = fp32 outputs (weight gradients) leave through shared memory + TMA tile store / reduce-add; 0 (default) = per-thread
-// 128-byte row segments.  Measured on the four weight gradients of a C2 block (profiles/r02_probe_call70.jsonl): the TMA
-// path is 5 % (reduce-add) to 13 % (store) SLOWER -- 32 extra TMA operations per tile share the queue of the operand loads.
-int dolo_option_gemm_f32_tma_epilogue();
-int dolo_option_attn_fwd_split();  // 0 never / 1 (default) head_dim >= 96 / 2 also head_dim 64, 80: split-softmax forward (two threads per query row); 3 = every head_dim >= 64 with four threads per row
-int dolo_option_attn_bwd_variant();  // head_dim 64 / 80 backward: 0 = round-1 softmax warps, 1 = lean, 2 (default) = lean + uniform 16-column chunks at head_dim 80 (0.701 vs 0.752 ms, profiles/r02_probe_attn_bwd_uniform_chunks_call80.jsonl; identical to 1 at head_dim 64)
-int dolo_option_attn_bwd_ablate();
 // attention CTA order (attention_common.cuh: attn_cta_order): heads per chunk (default 8; heads fastest inside a chunk, the
-// longest tiles of a document first, so that the last wave holds short tiles only); 0 = round 1's order (tiles fastest)
+// longest tiles of a document first, so that the last wave holds short tiles only); 0 = tiles fastest
 int dolo_option_attn_head_fastest();
-// 1 (default) = GEMM grids have one cluster per tile and running clusters take over pending ones through cluster launch
-// control (hardware work stealing): the grid uses every SM that is free, no margin for concurrent communication kernels
-// needed; 0 = static persistent workers (tile w, w + W, ...) on `SMs - gemm_sm_margin` SMs
-int dolo_option_gemm_dynamic();
 int dolo_option_gemm_l2_hints();  // 1 (default) = evict-first / evict-last operand loads for long-contraction GEMMs
 
 // TMA descriptor encode through the driver entry point (no link-time libcuda dependency).
@@ -121,20 +109,17 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
     return ok != 0;
 }
 
-// Watchdog: a pipeline bug must surface as a trap (reported by the host as a CUDA error), never as a
-// hung GPU.  ~4 s at 2 GHz.  `tag` identifies the waiting role in the printf.
+// Watchdog: a pipeline bug must surface as a trap (reported by the host as a CUDA error), never as a hung GPU.  ~4 s at
+// 2 GHz.  No printf here: a function call inside a wgmma pipeline makes ptxas serialise every wgmma of the kernel.
 #ifndef DOLO_WATCHDOG_CYCLES
 #define DOLO_WATCHDOG_CYCLES (8000000000LL)
 #endif
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int tag = 0) {
+    (void)tag;  // identifies the waiting role at the call site
     if (mbar_try_wait(bar, parity)) return;
     long long t0 = clock64();
     while (!mbar_try_wait(bar, parity)) {
-        if (clock64() - t0 > DOLO_WATCHDOG_CYCLES) {
-            printf("[dolomite_b200] mbarrier watchdog: block (%d,%d,%d) thread %d tag %d parity %u\n", blockIdx.x,
-                   blockIdx.y, blockIdx.z, threadIdx.x, tag, parity);
-            __trap();
-        }
+        if (clock64() - t0 > DOLO_WATCHDOG_CYCLES) __trap();
     }
 }
 
@@ -142,8 +127,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int ta
 __device__ __forceinline__ void fence_proxy_async_smem() {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
@@ -161,8 +144,7 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
 }
 // L2 eviction-priority hints for TMA loads (the fixed policy encodings of the sm_90+ `createpolicy` instruction).  A GEMM
 // whose contraction is long streams one operand once per wave of tiles and re-uses the other in every wave: the streamed
-// operand is loaded evict-first, the re-used one evict-last, so the re-used panels survive in the 126 MB L2 (ncu before:
-// dgrad / wgrad read 2.0-2.2x their algorithmic bytes from DRAM, profiles/r02_gemm_traffic_table.json).
+// operand is loaded evict-first, the re-used one evict-last, so the re-used panels survive in the 50 MB L2.
 constexpr uint64_t TMA_HINT_NORMAL = 0x1000000000000000ull;
 constexpr uint64_t TMA_HINT_EVICT_FIRST = 0x12F0000000000000ull;
 constexpr uint64_t TMA_HINT_EVICT_LAST = 0x14F0000000000000ull;
@@ -178,17 +160,6 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
     asm volatile(
         "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
         ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
-// TMA gather4 (sm_100): four rows of a rank-2 tensor, chosen by four row coordinates, land as four consecutive rows of the
-// (swizzled) shared-memory tile.  The tensor map's box is {columns, 1 row}.  The ScatterMoE gather-on-load of the grouped
-// expert GEMM (moe_dolomite/moe/scatter.py:38-49 `parallel_linear(grouped_in=False)`) is 32 of these per 128-row A tile.
-__device__ __forceinline__ void tma_gather4_2d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int r0, int r1,
-                                               int r2, int r3) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.tile::gather4.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(r0), "r"(r1), "r"(r2),
-        "r"(r3)
         : "memory");
 }
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {
@@ -236,50 +207,8 @@ __device__ __forceinline__ void bulk_reduce_add_f32(float* gdst, uint32_t smem_s
                  : "memory");
 }
 
-// ---------------- tcgen05 ----------------
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_slot) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_slot)),
-                 "r"(NCOLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(NCOLS) : "memory");
-}
 
-// D[tmem] (+)= A[smem desc] * B[smem desc]
-__device__ __forceinline__ void umma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                        uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]
-__device__ __forceinline__ void umma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                        uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-        "}\n" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// mbarrier arrive when all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-
-// ---------------- CTA-pair (cta_group::2) variants: two SMs of one cluster cooperate on a 256-row MMA ----------------
+// ---------------- thread-block clusters ----------------
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -289,244 +218,34 @@ __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
     asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t* smem_slot) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_slot)),
-                 "r"(NCOLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(NCOLS) : "memory");
-}
-// TMA load issued by either CTA of the pair; the transaction bytes are credited to the LEADER CTA's mbarrier
-// (same smem offset, peer bit cleared), which is the barrier the MMA-issuing thread waits on.
-__device__ __forceinline__ void tma_load_2d_2cta(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-    const uint32_t bar_leader = smem_u32(bar) & 0xFEFFFFFFu;
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_leader), "r"(c0), "r"(c1)
-        : "memory");
-}
-// gather4 issued by either CTA of a pair; bytes are credited to the leader CTA's mbarrier (see tma_load_2d_2cta)
-__device__ __forceinline__ void tma_gather4_2d_2cta(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int r0,
-                                                    int r1, int r2, int r3) {
-    const uint32_t bar_leader = smem_u32(bar) & 0xFEFFFFFFu;
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.tile::gather4.mbarrier::complete_tx::bytes.cta_group::2 [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_leader), "r"(c0), "r"(r0), "r"(r1), "r"(r2),
-        "r"(r3)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2cta_hint(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                                      uint64_t hint) {
-    const uint32_t bar_leader = smem_u32(bar) & 0xFEFFFFFFu;
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5;"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_leader), "r"(c0), "r"(c1), "l"(hint)
-        : "memory");
-}
-__device__ __forceinline__ void umma_ss_2cta(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                             uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on the barrier at this smem offset in BOTH CTAs of the pair once all prior MMAs of this thread retired
-__device__ __forceinline__ void umma_commit_2cta(uint64_t* bar) {
-    const uint16_t mask = 3;
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-            smem_u32(bar)),
-        "h"(mask)
-        : "memory");
-}
-// arrive on the barrier at the same smem offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t rank) {
-    uint32_t remote;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(rank));
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
-}
-// arrive + expect `bytes` on the barrier at the same smem offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_expect_tx_remote(uint64_t* bar, uint32_t bytes, uint32_t rank) {
-    uint32_t remote;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(rank));
-    asm volatile("mbarrier.arrive.expect_tx.release.cluster.shared::cluster.b64 _, [%0], %1;" ::"r"(remote), "r"(bytes)
-                 : "memory");
-}
 
-// ---------------- cluster launch control: work stealing over the clusters of the grid that have not started ----------------
-// A running cluster asks the hardware to CANCEL one pending cluster of its own grid and receives that cluster's first CTA
-// id (16-byte response written to shared memory, completion signalled on an mbarrier as 16 transaction bytes) -- or a
-// "nothing left" response, after which no further request may be issued.  A grid of one cluster per tile therefore
-// behaves like a persistent kernel whose workers take tiles as they get free, on however many SMs the hardware could
-// give the grid (concurrent NCCL kernels hold some).
-__device__ __forceinline__ void clc_try_cancel(void* response, uint64_t* bar) {
-    asm volatile("clusterlaunchcontrol.try_cancel.async.shared::cta.mbarrier::complete_tx::bytes.b128 [%0], [%1];" ::"r"(
-                     smem_u32(response)),
-                 "r"(smem_u32(bar))
-                 : "memory");
-}
-// the response (and the 16 transaction bytes) go to the same shared-memory offsets in EVERY CTA of the requesting cluster
-__device__ __forceinline__ void clc_try_cancel_multicast(void* response, uint64_t* bar) {
-    asm volatile(
-        "clusterlaunchcontrol.try_cancel.async.shared::cta.mbarrier::complete_tx::bytes.multicast::cluster::all.b128 [%0], [%1];" ::
-            "r"(smem_u32(response)),
-        "r"(smem_u32(bar))
-        : "memory");
-}
-// decodes a response: true + blockIdx.x of the first CTA of the cancelled cluster, or false (no pending cluster was left)
-__device__ __forceinline__ bool clc_query(const void* response, int& first_ctaid_x) {
-    uint32_t ok, x;
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        ".reg .b128 resp;\n\t"
-        "ld.shared.b128 resp, [%2];\n\t"
-        "clusterlaunchcontrol.query_cancel.is_canceled.pred.b128 p, resp;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t"
-        "mov.u32 %1, 0;\n\t"
-        "@p clusterlaunchcontrol.query_cancel.get_first_ctaid::x.b32.b128 %1, resp;\n\t"
-        "}\n"
-        : "=r"(ok), "=r"(x)
-        : "r"(smem_u32(response))
-        : "memory");
-    first_ctaid_x = int(x);
-    return ok != 0;
-}
-
-// kind::f16 instruction descriptor: bf16 x bf16 -> fp32
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N, bool a_mn_major, bool b_mn_major) {
-    return (1u << 4)      // D format: F32
-           | (1u << 7)    // A format: BF16
-           | (1u << 10)   // B format: BF16
-           | ((a_mn_major ? 1u : 0u) << 15) | ((b_mn_major ? 1u : 0u) << 16) | (uint32_t(N >> 3) << 17) |
-           (uint32_t(M >> 4) << 24);
-}
-
-// Shared-memory matrix descriptor (sm_100 "version 1").  layout_type: 0 none, 2 SW128, 4 SW64, 6 SW32.
-__device__ __forceinline__ uint64_t umma_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                   uint32_t layout_type) {
+// ---------------- wgmma (sm_90a warpgroup MMA) ----------------
+// Shared-memory matrix descriptor of sm_90 wgmma.  layout_type: 0 none, 1 SW128, 2 SW64, 3 SW32.  K-major swizzled
+// operands: SBO = byte stride between 8-row groups (LBO unused); MN-major: LBO = byte stride between MN swizzle atoms,
+// SBO = byte stride between 8-row groups of the contraction.
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout_type) {
     uint64_t d = 0;
     d |= uint64_t((saddr & 0x3FFFFu) >> 4);
     d |= uint64_t((lbo_bytes >> 4) & 0x3FFFu) << 16;
     d |= uint64_t((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= uint64_t(1) << 46;
-    d |= uint64_t(layout_type & 7u) << 61;
+    d |= uint64_t(layout_type & 3u) << 62;
     return d;
 }
-
-// TMEM -> registers, 32 lanes x 32 columns (one row per thread of the warp's sub-partition)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
+// registers of the accumulators / register A operands are ready for (or were written by) wgmma
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// Compile-time only: "redefines" the 16 registers of an earlier tcgen05.ld after its wait, so that no consumer can be
-// scheduled above the wait when several loads are kept in flight (software-pipelined TMEM reads).
-__device__ __forceinline__ void reg_fence16(uint32_t (&r)[16]) {
-    asm volatile("" : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                      "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]),
-                      "+r"(r[15]));
-}
-// Blackwell packed fp32 pipes: FFMA2 / FADD2 (two lanes per issue slot) and the 3-input FMNMX3.
-__device__ __forceinline__ void ffma2_bcast(float& d0, float& d1, float a0, float a1, float s, float c) {
-    uint64_t a, sb, cb, d;  // (a0, a1) * (s, s) + (c, c)
-    asm("mov.b64 %0, {%1, %2};" : "=l"(a) : "f"(a0), "f"(a1));
-    asm("mov.b64 %0, {%1, %1};" : "=l"(sb) : "f"(s));
-    asm("mov.b64 %0, {%1, %1};" : "=l"(cb) : "f"(c));
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(sb), "l"(cb));
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(d0), "=f"(d1) : "l"(d));
-}
-// (a0, a1) * (s, s) + (c0, c1)
-__device__ __forceinline__ void ffma2_sv(float& d0, float& d1, float a0, float a1, float s, float c0, float c1) {
-    uint64_t a, sb, cb, d;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(a) : "f"(a0), "f"(a1));
-    asm("mov.b64 %0, {%1, %1};" : "=l"(sb) : "f"(s));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(cb) : "f"(c0), "f"(c1));
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(sb), "l"(cb));
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(d0), "=f"(d1) : "l"(d));
-}
-// (a0, a1) + (b0, b1)  and  (a0, a1) * (b0, b1)
-__device__ __forceinline__ void fadd2_v(float& d0, float& d1, float a0, float a1, float b0, float b1) {
-    uint64_t a, b, d;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(a) : "f"(a0), "f"(a1));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(b) : "f"(b0), "f"(b1));
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(d0), "=f"(d1) : "l"(d));
-}
-__device__ __forceinline__ void fmul2_v(float& d0, float& d1, float a0, float a1, float b0, float b1) {
-    uint64_t a, b, d;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(a) : "f"(a0), "f"(a1));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(b) : "f"(b0), "f"(b1));
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(d0), "=f"(d1) : "l"(d));
-}
-__device__ __forceinline__ void fadd2(float& acc0, float& acc1, float b0, float b1) {
-    uint64_t a, b, d;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(a) : "f"(acc0), "f"(acc1));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(b) : "f"(b0), "f"(b1));
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(acc0), "=f"(acc1) : "l"(d));
-}
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-    float d;
-    asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-    return d;
+// Compile-time only: ties accumulator registers to the asm stream, so that no read of them is scheduled above a
+// wgmma_wait (the asm of the MMA and of the wait do not name them together).
+template <int N>
+__device__ __forceinline__ void reg_fence(float* d) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-__device__ __forceinline__ void reg_fence32(uint32_t (&r)[32]) {
-    asm volatile("" : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                      "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]),
-                      "+r"(r[15]));
-    asm volatile("" : "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]),
-                      "+r"(r[23]), "+r"(r[24]), "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]),
-                      "+r"(r[30]), "+r"(r[31]));
-}
-
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%32], "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31};" ::"r"(r[0]),
-        "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-        "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]),
-        "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]),
-        "r"(r[29]), "r"(r[30]), "r"(r[31]), "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%16], "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15};" ::"r"(r[0]),
-        "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-        "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // ---------------- small numeric helpers ----------------
 __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
@@ -536,6 +255,14 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
 __device__ __forceinline__ float bf16_lo(uint32_t v) { return __uint_as_float(v << 16); }
 __device__ __forceinline__ float bf16_hi(uint32_t v) { return __uint_as_float(v & 0xFFFF0000u); }
 __device__ __forceinline__ float bf16_round(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
+// The bf16 A fragment (m64k16, register operand of wgmma) of contraction step kk from an fp32 accumulator whose columns
+// are that contraction: n8 blocks 2kk and 2kk + 1 hold exactly the A elements this thread owns.
+__device__ __forceinline__ void acc_to_a_frag(const float* d, int kk, uint32_t (&a)[4]) {
+    a[0] = pack_bf16(d[8 * kk + 0], d[8 * kk + 1]);
+    a[1] = pack_bf16(d[8 * kk + 2], d[8 * kk + 3]);
+    a[2] = pack_bf16(d[8 * kk + 4], d[8 * kk + 5]);
+    a[3] = pack_bf16(d[8 * kk + 6], d[8 * kk + 7]);
+}
 
 // 2^x on the MUFU pipe in ONE instruction (exp2f() adds range fix-ups we do not need: inputs are <= 0 or -inf)
 // ---------------- dropout masks (counter-based: the same mask is regenerated in backward and in recomputed blocks) -----------

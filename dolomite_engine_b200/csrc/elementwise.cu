@@ -22,6 +22,43 @@ __device__ __forceinline__ float block_sum(float v, float* red) {
     return t;
 }
 
+// Deterministic column sums across the CTAs of a (1, CS, 1) cluster that split the rows of one column tile: every CTA
+// leaves its per-column partials in shared memory, and rank 0 adds them in rank order (distributed shared memory) and
+// applies the result to `out` -- the same order on every run, unlike one fp32 atomic per CTA.  Must be reached by every
+// CTA of the cluster.
+constexpr int kColsumCluster = 8;
+__device__ __forceinline__ float ld_cluster_f32(const float* local_smem, uint32_t rank) {
+    uint32_t remote;
+    float v;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(local_smem)), "r"(rank));
+    asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(remote) : "memory");
+    return v;
+}
+__device__ __forceinline__ void cluster_colsum_apply(const float* part, float* out, bool ok, float scale) {
+    cluster_sync_all();  // every CTA's partials are in its shared memory
+    if (cluster_ctarank() == 0 && ok) {
+        float s = 0.f;
+        for (int r = 0; r < int(gridDim.y); ++r) s += ld_cluster_f32(part, uint32_t(r));
+        *out += s * scale;
+    }
+    cluster_sync_all();  // the partials stay alive until rank 0 has read them
+}
+template <typename Kern, typename... Args>
+static int launch_row_cluster(Kern kern, int col_tiles, cudaStream_t st, Args... args) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(unsigned(col_tiles), kColsumCluster, 1);
+    cfg.blockDim = dim3(kThreads);
+    cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = 1;
+    attr[0].val.clusterDim.y = kColsumCluster;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return int(cudaLaunchKernelEx(&cfg, kern, args...));
+}
+
 __device__ __forceinline__ void unpack8(const uint4& v, float (&f)[8]) {
     f[0] = bf16_lo(v.x); f[1] = bf16_hi(v.x);
     f[2] = bf16_lo(v.y); f[3] = bf16_hi(v.y);
@@ -353,7 +390,8 @@ __global__ void __launch_bounds__(kThreads) swiglu_bwd_kernel(const uint4* __res
 
 // SwiGLU backward that also accumulates the bias gradient of the producing linear layer (column sums of the bf16 dx it
 // writes): saves the separate pass that re-read the whole [T, 2F] tensor.  Block = 32 column vectors (256 up + 256 gate
-// columns) x 8 row lanes over `rows_per_block` rows; per-thread fp32 column sums, smem combine, one atomicAdd per column.
+// columns) x 8 row lanes over `rows_per_block` rows; per-thread fp32 column sums, smem combine, and the row splits of a
+// column tile (one cluster) combined in a fixed order (cluster_colsum_apply).
 __global__ void __launch_bounds__(kThreads)
     swiglu_bwd_bias_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x, uint4* __restrict__ dx,
                            float* __restrict__ dbias, int64_t T, int64_t F8, int rows_per_block) {
@@ -395,6 +433,7 @@ __global__ void __launch_bounds__(kThreads)
         sm[rl][1][lane * 8 + j] = sg[j];
     }
     __syncthreads();
+    __shared__ float part[2][256];
     const int col = threadIdx.x;
     float a = 0.f, b = 0.f;
 #pragma unroll
@@ -402,11 +441,12 @@ __global__ void __launch_bounds__(kThreads)
         a += sm[w][0][col];
         b += sm[w][1][col];
     }
+    part[0][col] = a;
+    part[1][col] = b;
     const int64_t gc = int64_t(blockIdx.x) * 256 + col;
-    if (gc < F8 * 8) {
-        atomicAdd(dbias + gc, a);
-        atomicAdd(dbias + F8 * 8 + gc, b);
-    }
+    const bool ok = gc < F8 * 8;
+    cluster_colsum_apply(&part[0][col], dbias + (ok ? gc : 0), ok, 1.f);
+    cluster_colsum_apply(&part[1][col], dbias + (ok ? F8 * 8 + gc : 0), ok, 1.f);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -467,15 +507,18 @@ __global__ void __launch_bounds__(kThreads)
             }
         }
     }
-    if (dbias == nullptr) return;
+    if (dbias == nullptr) return;  // uniform over the cluster
 #pragma unroll
     for (int j = 0; j < 8; ++j) sm[rl][lane * 8 + j] = s[j];
     __syncthreads();
+    __shared__ float part[256];
     float a = 0.f;
 #pragma unroll
     for (int w = 0; w < 8; ++w) a += sm[w][threadIdx.x];
+    part[threadIdx.x] = a;
     const int64_t gc = int64_t(blockIdx.x) * 256 + threadIdx.x;
-    if (gc < F8 * 8) atomicAdd(dbias + gc, a);
+    const bool ok = gc < F8 * 8;
+    cluster_colsum_apply(&part[threadIdx.x], dbias + (ok ? gc : 0), ok, 1.f);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -638,18 +681,36 @@ __global__ void __launch_bounds__(kThreads)
     }
 }
 
+// One warp per token.  The warp of the FIRST token with a given id owns that row of dwte and adds the rows of all tokens
+// with that id in ascending token order: a fixed summation order (bit-identical runs) without atomics.
+__device__ __forceinline__ int64_t clamp_id(int64_t id, int64_t V) { return id < 0 ? 0 : (id >= V ? V - 1 : id); }
 __global__ void __launch_bounds__(kThreads)
     embedding_bwd_kernel(const int64_t* __restrict__ ids, const uint4* __restrict__ dout, float* __restrict__ dwte,
                          int64_t T, int H8, int64_t V, float scale) {
-    for (int64_t t = blockIdx.x; t < T; t += gridDim.x) {
-        int64_t id = ids[t];
-        id = id < 0 ? 0 : (id >= V ? V - 1 : id);
-        float* dst = dwte + id * H8 * 8;
-        for (int i = threadIdx.x; i < H8; i += blockDim.x) {
-            float f[8];
-            unpack8(__ldg(dout + t * H8 + i), f);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) atomicAdd(dst + i * 8 + j, f[j] * scale);
+    const int lane = threadIdx.x & 31;
+    const int64_t t = int64_t(blockIdx.x) * (kThreads / 32) + (threadIdx.x >> 5);
+    if (t >= T) return;  // uniform per warp
+    const int64_t id = clamp_id(ids[t], V);
+    for (int64_t base = 0; base < t; base += 32) {
+        const int64_t u = base + lane;
+        if (__any_sync(0xffffffffu, u < t && clamp_id(ids[u], V) == id)) return;  // an earlier token owns the row
+    }
+    float4* dst = reinterpret_cast<float4*>(dwte + id * H8 * 8);
+    for (int64_t base = t; base < T; base += 32) {
+        const int64_t u0 = base + lane;
+        uint32_t m = __ballot_sync(0xffffffffu, u0 < T && clamp_id(ids[u0], V) == id);
+        while (m) {
+            const int64_t u = base + (__ffs(m) - 1);
+            m &= m - 1;
+            for (int i = lane; i < H8; i += 32) {
+                float f[8];
+                unpack8(__ldg(dout + u * H8 + i), f);
+                float4 a = dst[2 * i], b = dst[2 * i + 1];
+                a.x += f[0] * scale; a.y += f[1] * scale; a.z += f[2] * scale; a.w += f[3] * scale;
+                b.x += f[4] * scale; b.y += f[5] * scale; b.z += f[6] * scale; b.w += f[7] * scale;
+                dst[2 * i] = a;
+                dst[2 * i + 1] = b;
+            }
         }
     }
 }
@@ -681,8 +742,7 @@ __global__ void ce_count_kernel(const int64_t* __restrict__ labels, int64_t T, i
 // Row-resident cross entropy: a row (or, for wide vocabularies, 1/SPLIT of a row per CTA of a SPLIT-CTA cluster) is read
 // from HBM ONCE into registers (NV 16-byte vectors per thread), max and sum-of-exponentials are reduced in the block (and
 // across the cluster through distributed shared memory), and the gradient row is written from the same registers: 4 B per
-// logit of traffic, the algorithmic minimum (the first version re-read the row: 6 B per logit, 0.58 of the copy peak in
-// profiles/r01_ncu_ce_call28.txt).  logits and dlogits may alias, hence no __restrict__ / __ldg on them.
+// logit of traffic, the algorithmic minimum.  logits and dlogits may alias, hence no __restrict__ / __ldg on them.
 __device__ __forceinline__ float ce_block_reduce(float v, float* red, bool is_max) {
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     v = is_max ? warp_max(v) : warp_sum(v);
@@ -844,8 +904,8 @@ __global__ void ce_mean_kernel(const float* __restrict__ loss_tok, int64_t T, co
 }
 
 // ------------------------------------------------------------------------------------------
-// column sums: grid (col tiles of 256 columns, row splits).  each thread owns 8 columns (one 16-B vector)
-// of 32 lanes; 8 warps stride rows; smem combine; atomicAdd to out.
+// column sums: grid (col tiles of 256 columns, row splits = one cluster).  each thread owns 8 columns (one 16-B vector)
+// of 32 lanes; 8 warps stride rows; smem combine; row splits combined in a fixed order (cluster_colsum_apply).
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kThreads)
     colsum_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx, float* __restrict__ out, int64_t T, int64_t N,
@@ -869,12 +929,15 @@ __global__ void __launch_bounds__(kThreads)
 #pragma unroll
     for (int j = 0; j < 8; ++j) sm[wid][lane * 8 + j] = acc[j];
     __syncthreads();
+    __shared__ float part[256];
     const int c = threadIdx.x;
     float s = 0.f;
 #pragma unroll
     for (int w = 0; w < 8; ++w) s += sm[w][c];
+    part[c] = s;
     const int64_t gc = int64_t(blockIdx.x) * 256 + c;
-    if (gc < N) atomicAdd(out + gc, s * scale);
+    const bool ok = gc < N;
+    cluster_colsum_apply(&part[c], out + (ok ? gc : 0), ok, scale);
 }
 
 __global__ void __launch_bounds__(kThreads) add_scaled_kernel(const uint4* __restrict__ a, const uint4* __restrict__ b,
@@ -892,7 +955,11 @@ __global__ void __launch_bounds__(kThreads) add_scaled_kernel(const uint4* __res
 // ------------------------------------------------------------------------------------------
 // optimizer kernels on flat fp32 shards
 // ------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kThreads) sumsq_kernel(const float* __restrict__ g, int64_t n, float* __restrict__ out) {
+// sum of squares in two launches with a fixed reduction tree: kSumsqBlocks grid-stride partials (fixed grid, so every
+// element always lands in the same partial), then one block adds them in a fixed order -- bit-identical runs.
+constexpr int kSumsqBlocks = 1024;
+__global__ void __launch_bounds__(kThreads)
+    sumsq_partial_kernel(const float* __restrict__ g, int64_t n, float* __restrict__ partials) {
     __shared__ float red[8];
     float s = 0.f;
     const int64_t n4 = n >> 2;
@@ -905,7 +972,14 @@ __global__ void __launch_bounds__(kThreads) sumsq_kernel(const float* __restrict
          i += int64_t(gridDim.x) * blockDim.x)
         s += g[i] * g[i];
     s = block_sum(s, red);
-    if (threadIdx.x == 0) atomicAdd(out, s);
+    if (threadIdx.x == 0) partials[blockIdx.x] = s;
+}
+__global__ void __launch_bounds__(kThreads) sumsq_final_kernel(const float* __restrict__ partials, float* __restrict__ out) {
+    __shared__ float red[8];
+    float s = 0.f;
+    for (int i = threadIdx.x; i < kSumsqBlocks; i += kThreads) s += partials[i];
+    s = block_sum(s, red);
+    if (threadIdx.x == 0) out[0] += s;
 }
 
 __global__ void clip_coef_kernel(const float* sumsq, float max_norm, float* coef, float* norm_out) {
@@ -1169,16 +1243,10 @@ extern "C" int dolomite_b200_gelu_bwd(const void* dy, const void* x, void* dx, f
     if (T == 0) return DOLO_OK;
     const int64_t F8 = F / 8;
     const int col_tiles = int((F8 + 31) / 32);
-    int row_splits = (dolo_num_sms() * 8 + col_tiles - 1) / col_tiles;
-    if (row_splits > (T + 7) / 8) row_splits = int((T + 7) / 8);
-    if (row_splits < 1) row_splits = 1;
-    if (row_splits > 65535) row_splits = 65535;
-    const int rows_per_block = int((T + row_splits - 1) / row_splits);
-    dim3 grid(col_tiles, (unsigned)((T + rows_per_block - 1) / rows_per_block));
-    gelu_bwd_kernel<<<grid, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-        static_cast<const uint4*>(dy), static_cast<const uint4*>(x), static_cast<uint4*>(dx), dbias_accum, T, F8,
-        rows_per_block);
-    DOLO_LAUNCH_OK("gelu_bwd");
+    const int rows_per_block = int((T + kColsumCluster - 1) / kColsumCluster);  // one cluster of row splits per column tile
+    DOLO_CUDA_OK(cudaError_t(launch_row_cluster(gelu_bwd_kernel, col_tiles, static_cast<cudaStream_t>(stream),
+                                                static_cast<const uint4*>(dy), static_cast<const uint4*>(x),
+                                                static_cast<uint4*>(dx), dbias_accum, T, F8, rows_per_block)));
     return DOLO_OK;
 }
 
@@ -1248,16 +1316,10 @@ extern "C" int dolomite_b200_swiglu_bwd_bias(const void* dy, const void* x, void
     if (T == 0) return DOLO_OK;
     const int64_t F8 = F / 8;
     const int col_tiles = int((F8 + 31) / 32);
-    int row_splits = (dolo_num_sms() * 8 + col_tiles - 1) / col_tiles;
-    if (row_splits > (T + 7) / 8) row_splits = int((T + 7) / 8);
-    if (row_splits < 1) row_splits = 1;
-    if (row_splits > 65535) row_splits = 65535;
-    const int rows_per_block = int((T + row_splits - 1) / row_splits);
-    dim3 grid(col_tiles, (unsigned)((T + rows_per_block - 1) / rows_per_block));
-    swiglu_bwd_bias_kernel<<<grid, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-        static_cast<const uint4*>(dy), static_cast<const uint4*>(x), static_cast<uint4*>(dx), dbias_accum, T, F8,
-        rows_per_block);
-    DOLO_LAUNCH_OK("swiglu_bwd_bias");
+    const int rows_per_block = int((T + kColsumCluster - 1) / kColsumCluster);  // one cluster of row splits per column tile
+    DOLO_CUDA_OK(cudaError_t(launch_row_cluster(swiglu_bwd_bias_kernel, col_tiles, static_cast<cudaStream_t>(stream),
+                                                static_cast<const uint4*>(dy), static_cast<const uint4*>(x),
+                                                static_cast<uint4*>(dx), dbias_accum, T, F8, rows_per_block)));
     return DOLO_OK;
 }
 
@@ -1278,7 +1340,8 @@ extern "C" int dolomite_b200_embedding_bwd(const int64_t* ids, const void* dout,
     DOLO_REQUIRE(H > 0 && H % 8 == 0, "embedding_bwd: H=%d must be a multiple of 8", H);
     DOLO_REQUIRE(aligned16(dout), "embedding_bwd: pointers must be 16-byte aligned");
     if (T == 0) return DOLO_OK;
-    const int grid = int(T < int64_t(dolo_num_sms()) * 16 ? T : int64_t(dolo_num_sms()) * 16);
+    DOLO_REQUIRE(T < (int64_t(1) << 36), "embedding_bwd: T too large");
+    const unsigned grid = unsigned((T + kThreads / 32 - 1) / (kThreads / 32));  // one warp per token
     embedding_bwd_kernel<<<grid, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
         ids, static_cast<const uint4*>(dout), dwte, T, H / 8, V, scale);
     DOLO_LAUNCH_OK("embedding_bwd");
@@ -1343,14 +1406,10 @@ extern "C" int dolomite_b200_colsum_accum(const void* x, int64_t ldx, float* out
     DOLO_REQUIRE(aligned16(x), "colsum: pointer must be 16-byte aligned");
     if (T == 0) return DOLO_OK;
     const int col_tiles = int((N + 255) / 256);
-    int row_splits = (dolo_num_sms() * 4 + col_tiles - 1) / col_tiles;
-    if (row_splits > (T + 63) / 64) row_splits = int((T + 63) / 64);
-    if (row_splits < 1) row_splits = 1;
-    const int rows_per_block = int((T + row_splits - 1) / row_splits);
-    dim3 grid(col_tiles, row_splits);
-    colsum_kernel<<<grid, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(static_cast<const __nv_bfloat16*>(x), ldx,
-                                                                            out, T, N, rows_per_block, scale);
-    DOLO_LAUNCH_OK("colsum");
+    const int rows_per_block = int((T + kColsumCluster - 1) / kColsumCluster);  // one cluster of row splits per column tile
+    DOLO_CUDA_OK(cudaError_t(launch_row_cluster(colsum_kernel, col_tiles, static_cast<cudaStream_t>(stream),
+                                                static_cast<const __nv_bfloat16*>(x), ldx, out, T, N, rows_per_block,
+                                                scale)));
     return DOLO_OK;
 }
 
@@ -1390,11 +1449,18 @@ extern "C" int dolomite_b200_add_scaled(const void* a, const void* b, void* out,
     return DOLO_OK;
 }
 
-extern "C" int dolomite_b200_sumsq_accum(const float* g, int64_t n, float* out, void* stream) {
+extern "C" int64_t dolomite_b200_sumsq_workspace_bytes(void) { return int64_t(kSumsqBlocks) * 4; }
+
+extern "C" int dolomite_b200_sumsq_accum(const float* g, int64_t n, float* out, void* workspace, void* stream) {
     DOLO_REQUIRE(aligned16(g), "sumsq: pointer must be 16-byte aligned");
+    DOLO_REQUIRE(workspace != nullptr && (reinterpret_cast<uintptr_t>(workspace) & 3) == 0, "sumsq: workspace missing or misaligned");
     if (n == 0) return DOLO_OK;
-    sumsq_kernel<<<grid_for(n / 4 + 1, kThreads), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(g, n, out);
-    DOLO_LAUNCH_OK("sumsq");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    float* partials = static_cast<float*>(workspace);
+    sumsq_partial_kernel<<<kSumsqBlocks, kThreads, 0, st>>>(g, n, partials);
+    DOLO_LAUNCH_OK("sumsq_partial");
+    sumsq_final_kernel<<<1, kThreads, 0, st>>>(partials, out);
+    DOLO_LAUNCH_OK("sumsq_final");
     return DOLO_OK;
 }
 

@@ -1,7 +1,8 @@
-// bf16 GEMM for sm_100a:  TMA (cp.async.bulk.tensor) -> 128B-swizzled smem ring -> tcgen05.mma (UMMA 128x256x16,
-// fp32 accumulators in TMEM, double buffered) -> epilogue warps (tcgen05.ld, alpha/bias/beta*C, bf16|fp32 store).
+// bf16 GEMM for sm_90a (H100):  TMA (cp.async.bulk.tensor) -> 128B-swizzled smem ring -> wgmma (m64n128k16 per consumer
+// warpgroup, fp32 accumulators in registers) -> epilogue straight from the registers (alpha / bias / beta*C, bf16 | fp32).
 //
-// Persistent, warp-specialised:  warp 0 = TMA producer, warp 1 = MMA issuer (+ TMEM alloc), warps 2..5 = epilogue.
+// Persistent, warp-specialised: warpgroup 0 = producer (one elected thread issues the TMA loads; the whole first warp for
+// gather-on-load), warpgroups 1 and 2 = consumers, each owning 64 rows of the 128 x 128 output tile.
 // Both operands may be K-major (row-major [rows, K]) or MN-major (stored [K, rows]); the latter is what dgrad / wgrad
 // need, so no transposes are ever materialised:
 //     fwd   Y[T,N]  = X[T,K]  . W[N,K]^T          A K-major,  B K-major
@@ -10,6 +11,7 @@
 #include <string.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 #include "../../include/dolomite_b200.h"
 
 using namespace dolo;
@@ -17,31 +19,20 @@ using namespace dolo;
 namespace {
 
 constexpr int BM = 128;
-constexpr int BN = 256;
+constexpr int BN = 128;
 constexpr int BK = 64;  // 64 bf16 = 128 bytes = one swizzle span
-constexpr int STAGES = 4;
+constexpr int STAGES = 6;
 constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KB
-constexpr int B_STAGE_BYTES = BN * BK * 2;  // 32 KB
+constexpr int B_STAGE_BYTES = BN * BK * 2;  // 16 KB
 constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-constexpr int EPI_SLAB_BYTES = BM * 64 * 2;  // 128 rows x 64 bf16 columns, SW128
-constexpr int EPI_BUFS = 2;
-constexpr int GEMM_THREADS = 224;  // warp 0 TMA producer, 1 MMA issuer, 2..5 epilogue, 6 tile scheduler (dynamic mode)
-constexpr int CLC_DEPTH = 8;       // tile-id responses in flight between the scheduler warp and the slowest role
-constexpr int TMEM_COLS = 512;  // 2 accumulator stages x 256 fp32 columns
-
-constexpr int SMEM_BYTES = 1024 /*align slack*/ + STAGES * STAGE_BYTES + EPI_BUFS * EPI_SLAB_BYTES + 512 /*barriers*/;
-static_assert(SMEM_BYTES <= 232448, "shared memory budget exceeded");
+constexpr int GEMM_THREADS = 384;  // warpgroup 0 producer, 1..2 consumers
+constexpr int SMEM_BYTES = 1024 /*align slack*/ + STAGES * STAGE_BYTES + 256 /*barriers*/;
+static_assert(SMEM_BYTES <= 232448, "shared memory budget exceeded (227 KB per block on sm_90)");
 
 constexpr int MAXP = 4;  // problems per launch (the four weight gradients of a transformer block share one launch)
 
-// Epilogue variants.  The fp32 TMA modes exist for the weight gradients: every epilogue warp stages its 32 rows x 32 fp32
-// columns in a private shared-memory slab and hands it to the TMA engine as a tile store (first gradient of a window:
-// overwrite) or a tile REDUCE-ADD performed by the L2 (accumulation) -- the first version read-modify-wrote the fp32
-// accumulator with per-thread float4 accesses, one 128-byte line per lane.
-enum EpiMode { EPI_DIRECT = 0, EPI_BF16_TMA = 1, EPI_F32_TMA_STORE = 2, EPI_F32_TMA_ADD = 3 };
-
 struct GemmMaps {
-    CUtensorMap a[MAXP], b[MAXP], d[MAXP];
+    CUtensorMap a[MAXP], b[MAXP];
 };
 
 struct Problem {
@@ -53,7 +44,6 @@ struct Problem {
     int num_m, num_n, num_kb;
     int group_m;     // m-blocks per rasterisation panel
     int tile_start;  // first launch-wide tile index of this problem
-    int epi;         // EpiMode
     float alpha, beta;
     uint64_t hint_a, hint_b;  // L2 eviction priority of the operand loads (TMA_HINT_*)
 };
@@ -62,7 +52,6 @@ struct GemmParams {
     Problem pr[MAXP];
     int n_prob;
     int num_tiles;  // over all problems (grouped modes: single problem, includes the group factor)
-    int dynamic;    // 1 = the grid has one cluster per tile and running clusters steal pending ones (cluster launch control)
     int d_is_f32;
     // grouped modes (MoE experts; moe_dolomite/moe/scatter.py:38-49 parallel_linear):
     //   1 = M-grouped: every 128-row tile of A/D belongs to one group (m_tile_group[m_blk], -1 = unused tile); B's outer
@@ -71,8 +60,10 @@ struct GemmParams {
     //       [group_k_offsets[g], group_k_offsets[g+1]) and D/C are offset by g * d_group_stride (expert wgrad)
     int grouped;
     const int* m_tile_group;
-    int m_tile_shift;        // CTA-pair mode: a 256-row super tile covers entries 2m, 2m+1 of the 128-row tile table
     const int* a_row_index;  // gather-on-load: source row of A for every (grouped) row of the problem, or NULL
+    const void* gather_a;    // gather-on-load: the ungrouped A [a_rows, K] (row stride gather_lda), read by the producer warp
+    int64_t gather_lda;
+    int gather_k;
     int b_group_rows;
     const int* group_k_offsets;
     int num_groups;
@@ -86,8 +77,8 @@ struct TileInfo {
 };
 
 // Tile rasterisation: sweep all n-blocks for a panel of `gm` m-blocks, so that the A panel (gm x 128 rows x K) stays
-// L2-resident while B streams; gm is chosen on the host so that the panel is ~24 MB (ncu on the first version with a
-// fixed panel of 8: B re-read 8x from DRAM, 870 MB of reads for 147 MB of operands).
+// L2-resident while B streams; gm is chosen on the host so that the panel is ~12 MB of the 50 MB L2 (with a
+// fixed panel of 8, B is re-read 8x from DRAM).
 __device__ __forceinline__ void tile_coords(int t, int num_m, int num_n, int gm, int& m_blk, int& n_blk) {
     const int per_group = gm * num_n;
     const int group = t / per_group;
@@ -129,556 +120,245 @@ __device__ __forceinline__ TileInfo tile_info(int t, const GemmParams& p) {
     } else {
         tile_coords(t, pr.num_m, pr.num_n, pr.group_m, ti.m_blk, ti.n_blk);
         if (p.grouped == 1) {
-            ti.grp = p.m_tile_group[ti.m_blk << p.m_tile_shift];
+            ti.grp = p.m_tile_group[ti.m_blk];
             ti.valid = ti.grp >= 0;
         }
     }
     return ti;
 }
 
-// Where a role (producer / MMA issuer / epilogue warp) gets its next tile from.  Static mode: worker w takes tiles w,
-// w + W, ...  Dynamic mode: the scheduler warp of the leader CTA keeps up to CLC_DEPTH cluster-launch-control requests
-// ahead; every role of every CTA of the cluster consumes every response (the last one says "grid exhausted") and releases
-// the slot on the LEADER's empty barrier.
-template <bool CTA2>
-struct TileFeed {
-    const uint4* resp;
-    uint64_t* full;
-    uint64_t* empty;
-    int slot;
-    uint32_t phase;
-    int step;  // static mode: number of workers
-    bool dynamic;
-    __device__ __forceinline__ TileFeed(const GemmParams& p, const uint4* r, uint64_t* f, uint64_t* e, int num_workers)
-        : resp(r), full(f), empty(e), slot(0), phase(0), step(num_workers), dynamic(p.dynamic != 0) {}
-    // `release` = this thread reports the slot as consumed for its role (one thread per role instance)
-    __device__ __forceinline__ bool next(int& t, int num_tiles, bool release, bool whole_warp, int tag) {
-        if (!dynamic) {
-            t += step;
-            return t < num_tiles;
-        }
-        mbar_wait(&full[slot], phase, tag);
-        int x;
-        const bool ok = clc_query(&resp[slot], x);
-        fence_proxy_async_smem();  // the slot's next write comes from the async proxy
-        if (whole_warp) __syncwarp();  // every lane has read the response before lane 0 hands the slot back
-        if (release) {
-            if constexpr (CTA2) mbar_arrive_remote(&empty[slot], 0);
-            else mbar_arrive(&empty[slot]);
-        }
-        if (++slot == CLC_DEPTH) { slot = 0; phase ^= 1; }
-        t = CTA2 ? (x >> 1) : x;
-        return ok;
-    }
-};
-
-// CTA2 = CTA-pair mode: a cluster of two CTAs computes a 256 x 256 tile with tcgen05.mma.cta_group::2 (M = 256).  Each
-// CTA stages its own 128 rows of A and HALF of the B tile (128 of the 256 N rows), so a pipeline stage is 32 KB instead
-// of 48 KB (6 stages instead of 4) and B is fetched from L2 once per pair.  The MMA is issued by the leader CTA
-// (cluster rank 0); accumulator rows 0..127 land in the leader's TMEM, rows 128..255 in the peer's, and each CTA runs its
-// own epilogue.  In CTA2 mode p.num_m counts 256-row super tiles and grouped modes are not used.
-template <bool A_MN, bool B_MN, bool CTA2>
+template <bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
     gemm_bf16_kernel(const __grid_constant__ GemmMaps maps, const __grid_constant__ GemmParams p) {
-    constexpr int NSTAGE = CTA2 ? 6 : STAGES;
-    constexpr int B_BYTES = CTA2 ? B_STAGE_BYTES / 2 : B_STAGE_BYTES;
-    constexpr int STG_BYTES = A_STAGE_BYTES + B_BYTES;
-    static_assert(NSTAGE * STG_BYTES == STAGES * STAGE_BYTES, "both modes use the same 192 KB operand ring");
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_align_1024(smem_raw);
     uint8_t* smem_a = smem;
-    uint8_t* smem_b = smem + NSTAGE * A_STAGE_BYTES;
-    uint8_t* smem_epi = smem + NSTAGE * STG_BYTES;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem_epi + EPI_BUFS * EPI_SLAB_BYTES);
-    uint64_t* full_bar = bars;                   // [NSTAGE]
-    uint64_t* empty_bar = bars + NSTAGE;         // [NSTAGE]
-    uint64_t* tmem_full = bars + 2 * NSTAGE;     // [2]
-    uint64_t* tmem_empty = bars + 2 * NSTAGE + 2;  // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * NSTAGE + 4);
-    uint4* clc_resp = reinterpret_cast<uint4*>(bars + 24);  // [CLC_DEPTH] 16-byte responses (dynamic mode)
-    uint64_t* clc_full = bars + 24 + 2 * CLC_DEPTH;         // [CLC_DEPTH]
-    uint64_t* clc_empty = clc_full + CLC_DEPTH;             // [CLC_DEPTH] (the leader CTA's are the ones in use)
-    static_assert(2 * NSTAGE + 5 <= 24 && (24 + 4 * CLC_DEPTH) * 8 <= 512, "barrier block layout");
+    uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
+    uint64_t* full_bar = bars;            // [STAGES]
+    uint64_t* empty_bar = bars + STAGES;  // [STAGES]
 
+    const int wg = threadIdx.x >> 7;
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     const int num_tiles = p.num_tiles;
-    const int cta_rank = CTA2 ? int(blockIdx.x & 1) : 0;          // == %cluster_ctarank for cluster dims (2,1,1)
-    const int worker = CTA2 ? int(blockIdx.x >> 1) : int(blockIdx.x);  // persistent worker (CTA or CTA pair) index
-                                                                       // == first tile in dynamic mode
-    const int num_workers = CTA2 ? int(gridDim.x >> 1) : int(gridDim.x);
+    const bool gather = !A_MN && p.a_row_index != nullptr;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         for (int q = 0; q < p.n_prob; ++q) {
-            tma_prefetch_desc(&maps.a[q]);
+            if (!gather) tma_prefetch_desc(&maps.a[q]);
             tma_prefetch_desc(&maps.b[q]);
-            if (p.pr[q].epi != EPI_DIRECT) tma_prefetch_desc(&maps.d[q]);
         }
-        for (int i = 0; i < NSTAGE; ++i) {
-            mbar_init(&full_bar[i], 1);
-            mbar_init(&empty_bar[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&tmem_full[i], 1);
-            mbar_init(&tmem_empty[i], CTA2 ? 8 : 4);  // one arrive per epilogue warp (of both CTAs in pair mode)
-        }
-        for (int i = 0; i < CLC_DEPTH; ++i) {
-            mbar_init(&clc_full[i], 1);                // the scheduler's arrive.expect_tx (+ 16 response bytes)
-            mbar_init(&clc_empty[i], CTA2 ? 11 : 6);   // producer(s) + MMA issuer + epilogue warps
+        for (int i = 0; i < STAGES; ++i) {
+            // gather-on-load: the 32 producer lanes arrive after their shared-memory stores, lane 0 also carries B's bytes
+            mbar_init(&full_bar[i], gather ? 33 : 1);
+            mbar_init(&empty_bar[i], 8);  // one arrive per consumer warp
         }
         mbar_fence_init();
     }
-    if (warp == 1) {
-        if (CTA2) tmem_alloc_2cta<TMEM_COLS>(tmem_slot);
-        else tmem_alloc<TMEM_COLS>(tmem_slot);
-    }
-    tc_fence_before();
-    if (CTA2) cluster_sync_all();  // barriers of both CTAs initialised before any remote arrive / multicast commit
-    else __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    __syncthreads();
 
-    if (warp == 0) {
-        // ================= TMA producer =================
-        if (!A_MN && p.a_row_index != nullptr) {
-            // Gather-on-load (grouped expert GEMM reading the UNGROUPED activations): the whole warp takes part, lane l
-            // owns rows 4l .. 4l+3 of the 128-row A tile and issues one gather4 per pipeline stage for them; lane 0 also
-            // arms the barrier and loads B.
+    if (wg == 0) {
+        // ================= producer =================
+        if (warp != 0) return;
+        if (gather) {
+            // Gather-on-load (grouped expert GEMM reading the UNGROUPED activations): lane l copies rows 4l .. 4l+3 of the
+            // 128-row A tile from their source rows into the 128B-swizzled stage (16-byte chunk c of row r lands at chunk
+            // c ^ (r % 8), the layout TMA would have written); lane 0 also loads B through TMA.
+            const __nv_bfloat16* A = static_cast<const __nv_bfloat16*>(p.gather_a);
             int stage = 0;
             uint32_t phase = 0;
-            for (int t = worker; t < num_tiles; t += num_workers) {
+            for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
                 const TileInfo ti = tile_info(t, p);
                 if (!ti.valid) continue;
-                const CUtensorMap* tmap_a = &maps.a[ti.q];
                 const CUtensorMap* tmap_b = &maps.b[ti.q];
-                const int m_blk = CTA2 ? ti.m_blk * 2 + cta_rank : ti.m_blk, n_blk = ti.n_blk;
-                const int b_outer = (p.grouped == 1) ? ti.grp * p.b_group_rows : 0;
-                const int4 src = *reinterpret_cast<const int4*>(p.a_row_index + int64_t(m_blk) * BM + lane * 4);
+                const int b_outer = ti.grp * p.b_group_rows;
+                const int4 src = *reinterpret_cast<const int4*>(p.a_row_index + int64_t(ti.m_blk) * BM + lane * 4);
+                const int srow[4] = {src.x, src.y, src.z, src.w};
                 for (int kb = ti.kb0; kb < ti.kb1; ++kb) {
                     mbar_wait(&empty_bar[stage], phase ^ 1, 1);
                     uint8_t* sa = smem_a + stage * A_STAGE_BYTES;
-                    uint8_t* sb = smem_b + stage * B_BYTES;
+                    uint8_t* sb = smem_b + stage * B_STAGE_BYTES;
                     if (lane == 0) {
-                        if constexpr (CTA2) {
-                            if (cta_rank == 0) mbar_expect_tx(&full_bar[stage], 2 * STG_BYTES);
-                            const int n_row = n_blk * BN + cta_rank * (BN / 2);
-                            if (!B_MN) {
-                                tma_load_2d_2cta(sb, tmap_b, &full_bar[stage], kb * BK, b_outer + n_row);
-                            } else {
-#pragma unroll
-                                for (int i = 0; i < BN / 128; ++i)
-                                    tma_load_2d_2cta(sb + i * (BK * 128), tmap_b, &full_bar[stage], n_row + i * 64,
-                                                     b_outer + kb * BK);
-                            }
+                        mbar_expect_tx(&full_bar[stage], B_STAGE_BYTES);
+                        if (!B_MN) {
+                            tma_load_2d(sb, tmap_b, &full_bar[stage], kb * BK, b_outer + ti.n_blk * BN);
                         } else {
-                            mbar_expect_tx(&full_bar[stage], STG_BYTES);
-                            if (!B_MN) {
-                                tma_load_2d(sb, tmap_b, &full_bar[stage], kb * BK, b_outer + n_blk * BN);
-                            } else {
 #pragma unroll
-                                for (int i = 0; i < BN / 64; ++i)
-                                    tma_load_2d(sb + i * (BK * 128), tmap_b, &full_bar[stage], n_blk * BN + i * 64,
-                                                b_outer + kb * BK);
-                            }
+                            for (int i = 0; i < BN / 64; ++i)
+                                tma_load_2d(sb + i * (BK * 128), tmap_b, &full_bar[stage], ti.n_blk * BN + i * 64,
+                                            b_outer + kb * BK);
                         }
                     }
-                    __syncwarp();
-                    if constexpr (CTA2)
-                        tma_gather4_2d_2cta(sa + lane * 512, tmap_a, &full_bar[stage], kb * BK, src.x, src.y, src.z, src.w);
-                    else
-                        tma_gather4_2d(sa + lane * 512, tmap_a, &full_bar[stage], kb * BK, src.x, src.y, src.z, src.w);
-                    if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        const int r = lane * 4 + i;
+                        const __nv_bfloat16* g = A + int64_t(srow[i]) * p.gather_lda + int64_t(kb) * BK;
+#pragma unroll
+                        for (int c = 0; c < 8; ++c) {
+                            uint4 v = make_uint4(0u, 0u, 0u, 0u);
+                            if (kb * BK + c * 8 < p.gather_k) v = __ldg(reinterpret_cast<const uint4*>(g + c * 8));
+                            *reinterpret_cast<uint4*>(sa + r * 128 + ((c ^ (r & 7)) << 4)) = v;
+                        }
+                    }
+                    fence_proxy_async_smem();  // generic-proxy stores -> visible to wgmma (async proxy)
+                    mbar_arrive(&full_bar[stage]);
+                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
             }
-        } else if (elect_one()) {  // uniform single-thread region: ptxas keeps descriptors in uniform registers
+        } else if (elect_one()) {
             int stage = 0;
             uint32_t phase = 0;
-            TileFeed<CTA2> feed(p, clc_resp, clc_full, clc_empty, num_workers);
-            int t = worker, t_next = 0;
-            bool have_next = false;
-            for (bool have = t < num_tiles; have; t = t_next, have = have_next) {
-                t_next = t;  // the next tile id is taken BEFORE this tile's work: its latency hides behind the pipeline waits
-                have_next = feed.next(t_next, num_tiles, true, false, 11);
+            for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
                 const TileInfo ti = tile_info(t, p);
                 if (!ti.valid) continue;
                 const CUtensorMap* tmap_a = &maps.a[ti.q];
                 const CUtensorMap* tmap_b = &maps.b[ti.q];
                 const uint64_t ha = p.pr[ti.q].hint_a, hb = p.pr[ti.q].hint_b;
-                const int m_blk = CTA2 ? ti.m_blk * 2 + cta_rank : ti.m_blk, n_blk = ti.n_blk;
+                const int m_blk = ti.m_blk, n_blk = ti.n_blk;
                 const int b_outer = (p.grouped == 1) ? ti.grp * p.b_group_rows : 0;
                 for (int kb = ti.kb0; kb < ti.kb1; ++kb) {
                     mbar_wait(&empty_bar[stage], phase ^ 1, 1);
                     uint8_t* sa = smem_a + stage * A_STAGE_BYTES;
-                    uint8_t* sb = smem_b + stage * B_BYTES;
-                    if constexpr (CTA2) {
-                        // the leader's barrier collects the bytes of both CTAs (its own arrive carries the expectation)
-                        if (cta_rank == 0) mbar_expect_tx(&full_bar[stage], 2 * STG_BYTES);
-                        const int n_row = n_blk * BN + cta_rank * (BN / 2);  // this CTA's half of the B tile
-                        if (!A_MN) {
-                            tma_load_2d_2cta_hint(sa, tmap_a, &full_bar[stage], kb * BK, m_blk * BM, ha);
-                        } else {
-#pragma unroll
-                            for (int i = 0; i < BM / 64; ++i)
-                                tma_load_2d_2cta_hint(sa + i * (BK * 128), tmap_a, &full_bar[stage], m_blk * BM + i * 64, kb * BK, ha);
-                        }
-                        if (!B_MN) {
-                            tma_load_2d_2cta_hint(sb, tmap_b, &full_bar[stage], kb * BK, b_outer + n_row, hb);
-                        } else {
-#pragma unroll
-                            for (int i = 0; i < BN / 128; ++i)
-                                tma_load_2d_2cta_hint(sb + i * (BK * 128), tmap_b, &full_bar[stage], n_row + i * 64,
-                                                 b_outer + kb * BK, hb);
-                        }
+                    uint8_t* sb = smem_b + stage * B_STAGE_BYTES;
+                    mbar_expect_tx(&full_bar[stage], STAGE_BYTES);
+                    if (!A_MN) {
+                        tma_load_2d_hint(sa, tmap_a, &full_bar[stage], kb * BK, m_blk * BM, ha);
                     } else {
-                        mbar_expect_tx(&full_bar[stage], STG_BYTES);
-                        if (!A_MN) {
-                            tma_load_2d_hint(sa, tmap_a, &full_bar[stage], kb * BK, m_blk * BM, ha);
-                        } else {
 #pragma unroll
-                            for (int i = 0; i < BM / 64; ++i)
-                                tma_load_2d_hint(sa + i * (BK * 128), tmap_a, &full_bar[stage], m_blk * BM + i * 64, kb * BK, ha);
-                        }
-                        if (!B_MN) {
-                            tma_load_2d_hint(sb, tmap_b, &full_bar[stage], kb * BK, b_outer + n_blk * BN, hb);
-                        } else {
-#pragma unroll
-                            for (int i = 0; i < BN / 64; ++i)
-                                tma_load_2d_hint(sb + i * (BK * 128), tmap_b, &full_bar[stage], n_blk * BN + i * 64,
-                                            b_outer + kb * BK, hb);
-                        }
+                        for (int i = 0; i < BM / 64; ++i)
+                            tma_load_2d_hint(sa + i * (BK * 128), tmap_a, &full_bar[stage], m_blk * BM + i * 64, kb * BK, ha);
                     }
-                    if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ================= MMA issuer =================
-        if (cta_rank == 0 && elect_one()) {  // pair mode: only the leader CTA issues (for both SMs)
-            constexpr uint32_t idesc = umma_idesc_bf16(CTA2 ? 2 * BM : BM, BN, A_MN, B_MN);
-            int stage = 0;
-            uint32_t phase = 0;
-            int acc = 0;
-            uint32_t acc_phase = 0;
-            TileFeed<CTA2> feed(p, clc_resp, clc_full, clc_empty, num_workers);
-            int t = worker, t_next = 0;
-            bool have_next = false;
-            for (bool have = t < num_tiles; have; t = t_next, have = have_next) {
-                t_next = t;  // the next tile id is taken BEFORE this tile's work: its latency hides behind the pipeline waits
-                have_next = feed.next(t_next, num_tiles, true, false, 12);
-                const TileInfo ti = tile_info(t, p);
-                if (!ti.valid) continue;
-                mbar_wait(&tmem_empty[acc], acc_phase ^ 1, 2);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + uint32_t(acc * BN);
-                for (int kb = ti.kb0; kb < ti.kb1; ++kb) {
-                    mbar_wait(&full_bar[stage], phase, 3);
-                    tc_fence_after();
-                    const uint32_t sa = smem_u32(smem_a + stage * A_STAGE_BYTES);
-                    const uint32_t sb = smem_u32(smem_b + stage * B_BYTES);
-#pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) {
-                        // K-major: +32 B per K=16 step inside the 128 B swizzle span; SBO = 8 rows x 128 B.
-                        // MN-major: +16 K-rows x 128 B per step; LBO = next 64-wide MN chunk (BK rows x 128 B), SBO = 8 K-rows.
-                        // (pair mode: the same descriptors address each CTA's own A rows / B half at equal smem offsets)
-                        const uint64_t adesc = A_MN ? umma_smem_desc(sa + k * 2048, BK * 128, 1024, 2)
-                                                    : umma_smem_desc(sa + k * 32, 16, 1024, 2);
-                        const uint64_t bdesc = B_MN ? umma_smem_desc(sb + k * 2048, BK * 128, 1024, 2)
-                                                    : umma_smem_desc(sb + k * 32, 16, 1024, 2);
-                        if constexpr (CTA2) umma_ss_2cta(d_tmem, adesc, bdesc, idesc, (kb != ti.kb0 || k != 0) ? 1u : 0u);
-                        else umma_ss(d_tmem, adesc, bdesc, idesc, (kb != ti.kb0 || k != 0) ? 1u : 0u);
-                    }
-                    // smem slot reusable (in both CTAs) once these MMAs retire
-                    if constexpr (CTA2) umma_commit_2cta(&empty_bar[stage]);
-                    else umma_commit(&empty_bar[stage]);
-                    if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
-                }
-                // accumulator complete (each CTA's epilogue drains its own 128 rows)
-                if constexpr (CTA2) umma_commit_2cta(&tmem_full[acc]);
-                else umma_commit(&tmem_full[acc]);
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-            }
-        }
-    } else if (warp == 6) {
-        // ================= tile scheduler (dynamic mode; leader CTA only) =================
-        if (p.dynamic != 0 && cta_rank == 0 && elect_one()) {
-            int slot = 0;
-            uint32_t phase = 0;
-            for (;;) {
-                mbar_wait(&clc_empty[slot], phase ^ 1, 20);  // every role of both CTAs has read the previous response
-                mbar_expect_tx(&clc_full[slot], 16);
-                if constexpr (CTA2) {
-                    mbar_expect_tx_remote(&clc_full[slot], 16, 1);
-                    clc_try_cancel_multicast(&clc_resp[slot], &clc_full[slot]);
-                } else {
-                    clc_try_cancel(&clc_resp[slot], &clc_full[slot]);
-                }
-                mbar_wait(&clc_full[slot], phase, 21);
-                int x;
-                const bool ok = clc_query(&clc_resp[slot], x);
-                fence_proxy_async_smem();
-                if (++slot == CLC_DEPTH) { slot = 0; phase ^= 1; }
-                if (!ok) break;  // no request may follow a failed one
-            }
-        }
-    } else {
-        // ================= epilogue (4 warps, TMEM sub-partition = warp % 4) =================
-        const int sub = warp & 3;
-        const int et = sub * 32 + lane;  // row within the tile == TMEM lane
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        int epi_buf = 0;
-        bool cta_stores = false, warp_stores = false;  // which kind of bulk group this thread may still have in flight
-        uint8_t* wslab = smem_epi + sub * (EPI_BUFS * EPI_SLAB_BYTES / 4);  // this warp's two private 4 KB slabs (fp32 modes)
-        int wbuf = 0;
-        TileFeed<CTA2> feed(p, clc_resp, clc_full, clc_empty, num_workers);
-        int t = worker, t_next = 0;
-        bool have_next = false;
-        for (bool have = t < num_tiles; have; t = t_next, have = have_next) {
-            t_next = t;  // the next tile id is taken BEFORE this tile's work: its latency hides behind the pipeline waits
-            have_next = feed.next(t_next, num_tiles, lane == 0, true, 13);
-            const TileInfo ti = tile_info(t, p);
-            if (!ti.valid) {
-                // K-grouped launch (expert weight gradients) and this expert received NO rows: its product is zero.  A launch
-                // that OVERWRITES (beta = 0, no C) must still write the tile -- the caller did not clear the buffer -- so the
-                // epilogue warps store zeros themselves; no MMA ran and no accumulator stage is involved.
-                const Problem& pz = p.pr[ti.q];
-                if (p.grouped == 2 && p.d_is_f32 && pz.C == nullptr) {
-                    const int64_t zrow = int64_t(CTA2 ? ti.m_blk * 2 + cta_rank : ti.m_blk) * BM + et;
-                    if (zrow < pz.M) {
-                        float* zr = static_cast<float*>(pz.D) + int64_t(ti.grp) * p.d_group_stride + zrow * pz.ldd;
-                        const int c1 = min(pz.N, (ti.n_blk + 1) * BN);
-                        for (int c = ti.n_blk * BN; c < c1; c += 4)  // N % 8 == 0: whole float4 in range
-                            *reinterpret_cast<float4*>(zr + c) = make_float4(0.f, 0.f, 0.f, 0.f);
-                    }
-                }
-                continue;
-            }
-            const Problem& pr = p.pr[ti.q];
-            const CUtensorMap* tmap_d = &maps.d[ti.q];
-            const int m_blk = CTA2 ? ti.m_blk * 2 + cta_rank : ti.m_blk, n_blk = ti.n_blk;
-            const int64_t d_off = (p.grouped == 2) ? int64_t(ti.grp) * p.d_group_stride : 0;
-            mbar_wait(&tmem_full[acc], acc_phase, 4);
-            tc_fence_after();
-            const uint32_t t_addr = tmem_base + (uint32_t(sub * 32) << 16) + uint32_t(acc * BN);
-            const int64_t row = int64_t(m_blk) * BM + et;
-            const bool row_ok = row < pr.M;
-            const int col0 = n_blk * BN;
-            const float alpha = pr.alpha, beta = pr.beta;
-            const __nv_bfloat16* bias = pr.bias;
-            const int N = pr.N;
-
-            if (pr.epi == EPI_BF16_TMA) {
-                cta_stores = true;
-                // 4 slabs of 64 columns: regs -> swizzled smem -> TMA store
-#pragma unroll 1
-                for (int slab = 0; slab < BN / 64; ++slab) {
-                    if (col0 + slab * 64 >= N) break;
-                    uint8_t* buf = smem_epi + epi_buf * EPI_SLAB_BYTES;
-                    // the buffer must have been fully read by the TMA store issued two slabs ago
-                    if (et == 0) tma_store_wait_read<EPI_BUFS - 1>();
-                    named_bar_sync(1, 128);
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        uint32_t r[32];
-                        tmem_ld32(t_addr + slab * 64 + h * 32, r);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int c = 0; c < 4; ++c) {  // 4 x 16-byte chunks (8 columns each)
-                            float f[8];
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) f[j] = __uint_as_float(r[c * 8 + j]);
-                            if (bias != nullptr) {
-                                const int cb = col0 + slab * 64 + h * 32 + c * 8;
-#pragma unroll
-                                for (int j = 0; j < 8; ++j)
-                                    if (cb + j < N) f[j] += __bfloat162float(bias[cb + j]);
-                            }
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) f[j] *= alpha;
-                            uint4 v;
-                            v.x = pack_bf16(f[0], f[1]);
-                            v.y = pack_bf16(f[2], f[3]);
-                            v.z = pack_bf16(f[4], f[5]);
-                            v.w = pack_bf16(f[6], f[7]);
-                            const int chunk = h * 4 + c;  // logical 16-byte chunk inside the 128-byte row
-                            *reinterpret_cast<uint4*>(buf + et * 128 + ((chunk ^ (et & 7)) << 4)) = v;
-                        }
-                    }
-                    fence_proxy_async_smem();
-                    named_bar_sync(1, 128);
-                    if (et == 0) {
-                        tma_store_2d(tmap_d, buf, col0 + slab * 64, m_blk * BM);
-                        tma_store_commit();
-                    }
-                    epi_buf ^= 1;
-                }
-            } else if (pr.epi == EPI_F32_TMA_STORE || pr.epi == EPI_F32_TMA_ADD) {
-                // fp32 D (weight gradients): 8 slabs of 32 columns.  Each warp owns its 32 rows: TMEM -> registers -> a
-                // private SW128 slab (32 rows x 128 B) -> one TMA tile store / reduce-add per slab.  No CTA-wide barrier.
-                warp_stores = true;
-                const bool add = pr.epi == EPI_F32_TMA_ADD;
-                const int row0 = m_blk * BM + sub * 32;
-#pragma unroll 1
-                for (int slab = 0; slab < BN / 32; ++slab) {
-                    const int cb = col0 + slab * 32;
-                    if (cb >= N) break;
-                    uint8_t* buf = wslab + wbuf * 4096;
-                    if (lane == 0) tma_store_wait_read<1>();  // the operation issued from this slab two slabs ago has read it
-                    __syncwarp();
-                    uint32_t r[32];
-                    tmem_ld32(t_addr + slab * 32, r);
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int c = 0; c < 8; ++c) {
-                        uint4 v;
-                        v.x = __float_as_uint(__uint_as_float(r[c * 4 + 0]) * alpha);
-                        v.y = __float_as_uint(__uint_as_float(r[c * 4 + 1]) * alpha);
-                        v.z = __float_as_uint(__uint_as_float(r[c * 4 + 2]) * alpha);
-                        v.w = __float_as_uint(__uint_as_float(r[c * 4 + 3]) * alpha);
-                        *reinterpret_cast<uint4*>(buf + lane * 128 + ((c ^ (lane & 7)) << 4)) = v;
-                    }
-                    fence_proxy_async_smem();
-                    __syncwarp();
-                    if (lane == 0) {
-                        if (row0 < pr.M) {  // rows / columns beyond the tensor are clipped by the TMA unit
-                            if (add) tma_reduce_add_3d(tmap_d, buf, cb, row0, ti.grp);
-                            else tma_store_3d(tmap_d, buf, cb, row0, ti.grp);
-                        }
-                        tma_store_commit();
-                    }
-                    wbuf ^= 1;
-                }
-            } else {
-#pragma unroll 1
-                for (int ch = 0; ch < BN / 32; ++ch) {
-                    const int cb = col0 + ch * 32;
-                    if (cb >= N) break;
-                    uint32_t r[32];
-                    tmem_ld32(t_addr + ch * 32, r);
-                    tmem_ld_wait();
-                    if (!row_ok) continue;
-                    float f[32];
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(r[j]);
-                    if (bias != nullptr) {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            if (cb + j < N) f[j] += __bfloat162float(bias[cb + j]);
-                    }
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) f[j] *= alpha;
-                    if (p.d_is_f32) {
-                        float* drow = static_cast<float*>(pr.D) + d_off + row * pr.ldd + cb;
-                        const float* crow = pr.C ? static_cast<const float*>(pr.C) + d_off + row * pr.ldc + cb : nullptr;
-#pragma unroll
-                        for (int q = 0; q < 8; ++q) {
-                            if (cb + q * 4 < N) {  // N % 8 == 0 -> whole float4 in range
-                                float4 o = make_float4(f[q * 4], f[q * 4 + 1], f[q * 4 + 2], f[q * 4 + 3]);
-                                if (p.grouped == 3) {  // split-K partial: D += o
-                                    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(drow + q * 4),
-                                                 "f"(o.x), "f"(o.y), "f"(o.z), "f"(o.w)
-                                                 : "memory");
-                                    continue;
-                                }
-                                if (crow) {
-                                    const float4 c4 = *reinterpret_cast<const float4*>(crow + q * 4);
-                                    o.x += beta * c4.x; o.y += beta * c4.y; o.z += beta * c4.z; o.w += beta * c4.w;
-                                }
-                                *reinterpret_cast<float4*>(drow + q * 4) = o;
-                            }
-                        }
+                    if (!B_MN) {
+                        tma_load_2d_hint(sb, tmap_b, &full_bar[stage], kb * BK, b_outer + n_blk * BN, hb);
                     } else {
-                        __nv_bfloat16* drow = static_cast<__nv_bfloat16*>(pr.D) + d_off + row * pr.ldd + cb;
-                        const __nv_bfloat16* crow =
-                            pr.C ? static_cast<const __nv_bfloat16*>(pr.C) + d_off + row * pr.ldc + cb : nullptr;
 #pragma unroll
-                        for (int q = 0; q < 4; ++q) {
-                            if (cb + q * 8 < N) {
-                                if (crow) {
-                                    const uint4 cv = *reinterpret_cast<const uint4*>(crow + q * 8);
-                                    f[q * 8 + 0] += beta * bf16_lo(cv.x); f[q * 8 + 1] += beta * bf16_hi(cv.x);
-                                    f[q * 8 + 2] += beta * bf16_lo(cv.y); f[q * 8 + 3] += beta * bf16_hi(cv.y);
-                                    f[q * 8 + 4] += beta * bf16_lo(cv.z); f[q * 8 + 5] += beta * bf16_hi(cv.z);
-                                    f[q * 8 + 6] += beta * bf16_lo(cv.w); f[q * 8 + 7] += beta * bf16_hi(cv.w);
-                                }
-                                uint4 v;
-                                v.x = pack_bf16(f[q * 8 + 0], f[q * 8 + 1]);
-                                v.y = pack_bf16(f[q * 8 + 2], f[q * 8 + 3]);
-                                v.z = pack_bf16(f[q * 8 + 4], f[q * 8 + 5]);
-                                v.w = pack_bf16(f[q * 8 + 6], f[q * 8 + 7]);
-                                *reinterpret_cast<uint4*>(drow + q * 8) = v;
-                            }
-                        }
+                        for (int i = 0; i < BN / 64; ++i)
+                            tma_load_2d_hint(sb + i * (BK * 128), tmap_b, &full_bar[stage], n_blk * BN + i * 64,
+                                             b_outer + kb * BK, hb);
                     }
+                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
             }
-            // release the accumulator stage back to the MMA warp
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-                if constexpr (CTA2) mbar_arrive_remote(&tmem_empty[acc], 0);  // the leader's MMA thread waits for both CTAs
-                else mbar_arrive(&tmem_empty[acc]);
-            }
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
         }
-        // shared memory must outlive every bulk operation that still reads it
-        if ((cta_stores && et == 0) || (warp_stores && lane == 0)) tma_store_wait_all<0>();
+        return;
     }
 
-    tc_fence_before();
-    if constexpr (CTA2) {
-        cluster_sync_all();  // the peer's smem / TMEM / barriers stay valid until both CTAs are done
-        if (warp == 1) {
-            tc_fence_after();
-            tmem_dealloc_2cta<TMEM_COLS>(tmem_base);
+    // ================= consumers: warpgroup cw owns rows [64 cw, 64 cw + 64) of the tile =================
+    const int cw = wg - 1;
+    const int wr = (warp & 3) * 16 + (lane >> 2);  // accumulator row of this thread inside the warpgroup (and +8)
+    const int wc = 2 * (lane & 3);                 // first accumulator column inside each n8 block
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[BN / 2];
+    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+        const TileInfo ti = tile_info(t, p);
+        const Problem& pr = p.pr[ti.q];
+        const int64_t row0 = int64_t(ti.m_blk) * BM + cw * 64 + wr;
+        const int col0 = ti.n_blk * BN + wc;
+        if (!ti.valid) {
+            // K-grouped launch (expert weight gradients) and this expert received NO rows: its product is zero.  A launch
+            // that OVERWRITES (beta = 0, no C) must still write the tile -- the caller did not clear the buffer.
+            if (p.grouped == 2 && p.d_is_f32 && pr.C == nullptr) {
+                float* D = static_cast<float*>(pr.D) + int64_t(ti.grp) * p.d_group_stride;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int64_t row = row0 + 8 * h;
+                    if (row >= pr.M) continue;
+                    for (int j = 0; j < BN / 8; ++j)
+                        if (col0 + 8 * j < pr.N)
+                            *reinterpret_cast<float2*>(D + row * pr.ldd + col0 + 8 * j) = make_float2(0.f, 0.f);
+                }
+            }
+            continue;
         }
-    } else {
-        __syncthreads();
-        if (warp == 1) {
-            tc_fence_after();
-            tmem_dealloc<TMEM_COLS>(tmem_base);
+        int prev_stage = -1;
+        for (int kb = ti.kb0; kb < ti.kb1; ++kb) {
+            mbar_wait(&full_bar[stage], phase, 3);
+            wgmma_fence();
+            const uint32_t sa = smem_u32(smem_a + stage * A_STAGE_BYTES);
+            const uint32_t sb = smem_u32(smem_b + stage * B_STAGE_BYTES);
+#pragma unroll
+            for (int k = 0; k < BK / 16; ++k) {
+                // K-major: +32 B per K=16 step inside the 128 B swizzle span; SBO = 8 rows x 128 B; this warpgroup's
+                // 64 rows start 64 x 128 B into the tile.
+                // MN-major: +16 K-rows x 128 B per step; LBO = next 64-wide MN chunk (BK rows x 128 B), SBO = 8 K-rows;
+                // this warpgroup's 64 rows are the cw-th chunk.
+                const uint64_t adesc = A_MN ? gmma_desc(sa + cw * (BK * 128) + k * 2048, BK * 128, 1024, 1)
+                                            : gmma_desc(sa + cw * (64 * 128) + k * 32, 16, 1024, 1);
+                const uint64_t bdesc = B_MN ? gmma_desc(sb + k * 2048, BK * 128, 1024, 1) : gmma_desc(sb + k * 32, 16, 1024, 1);
+                wgmma_ss<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc, bdesc, (kb != ti.kb0 || k != 0) ? 1u : 0u);
+            }
+            wgmma_commit();
+            wgmma_wait<1>();  // the previous k-block's MMAs retired: its stage may be refilled
+            if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+            prev_stage = stage;
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+        reg_fence<BN / 2>(acc);
+        if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+
+        // ---------------- epilogue: registers -> global ----------------
+        const int64_t d_off = (p.grouped == 2) ? int64_t(ti.grp) * p.d_group_stride : 0;
+        const float alpha = pr.alpha, beta = pr.beta;
+        const __nv_bfloat16* bias = pr.bias;
+        const int N = pr.N;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+            const int col = col0 + 8 * j;
+            if (col >= N) continue;  // N % 8 == 0: the column pair is either wholly in range or wholly out
+            float b0 = 0.f, b1 = 0.f;
+            if (bias != nullptr) {
+                const uint32_t bv = *reinterpret_cast<const uint32_t*>(bias + col);
+                b0 = bf16_lo(bv);
+                b1 = bf16_hi(bv);
+            }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int64_t row = row0 + 8 * h;
+                if (row >= pr.M) continue;
+                float v0 = (acc[4 * j + 2 * h] + b0) * alpha;
+                float v1 = (acc[4 * j + 2 * h + 1] + b1) * alpha;
+                if (p.d_is_f32) {
+                    float* d = static_cast<float*>(pr.D) + d_off + row * pr.ldd + col;
+                    if (p.grouped == 3) {  // split-K partial: D += v
+                        asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(d), "f"(v0), "f"(v1) : "memory");
+                        continue;
+                    }
+                    if (pr.C) {
+                        const float2 c2 = *reinterpret_cast<const float2*>(static_cast<const float*>(pr.C) + d_off + row * pr.ldc + col);
+                        v0 += beta * c2.x;
+                        v1 += beta * c2.y;
+                    }
+                    *reinterpret_cast<float2*>(d) = make_float2(v0, v1);
+                } else {
+                    __nv_bfloat16* d = static_cast<__nv_bfloat16*>(pr.D) + d_off + row * pr.ldd + col;
+                    if (pr.C) {
+                        const uint32_t cv =
+                            *reinterpret_cast<const uint32_t*>(static_cast<const __nv_bfloat16*>(pr.C) + d_off + row * pr.ldc + col);
+                        v0 += beta * bf16_lo(cv);
+                        v1 += beta * bf16_hi(cv);
+                    }
+                    *reinterpret_cast<uint32_t*>(d) = pack_bf16(v0, v1);
+                }
+            }
         }
     }
 }
 
 template <bool A_MN, bool B_MN>
-int launch_gemm(const GemmMaps& maps, const GemmParams& p_in, cudaStream_t st, bool cta_pair) {
-    // Dynamic mode: one cluster per tile, running clusters cancel + take over pending ones (TileFeed).  The grid then
-    // uses whatever SMs are free when it starts -- and the ones that get free while it runs -- so gemm_sm_margin is moot.
-    GemmParams p = p_in;
-    p.dynamic = (dolo_option_gemm_dynamic() != 0 && p.a_row_index == nullptr) ? 1 : 0;
-    const int tiles = p.num_tiles;
-    if (cta_pair) {
-        auto kern = gemm_bf16_kernel<A_MN, B_MN, true>;
-        static bool attr_set2 = false;  // per instantiation
-        if (!attr_set2) {
-            DOLO_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-            attr_set2 = true;
-        }
-        const int pairs = (dolo_num_sms() - dolo_option_gemm_sm_margin()) / 2;
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(unsigned(2 * ((p.dynamic || tiles < pairs) ? tiles : pairs)));
-        cfg.blockDim = dim3(GEMM_THREADS);
-        cfg.dynamicSmemBytes = SMEM_BYTES;
-        cfg.stream = st;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 2;
-        attr[0].val.clusterDim.y = 1;
-        attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
-        DOLO_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, maps, p));
-        return DOLO_OK;
-    }
-    auto kern = gemm_bf16_kernel<A_MN, B_MN, false>;
+int launch_gemm(const GemmMaps& maps, const GemmParams& p, cudaStream_t st) {
+    auto kern = gemm_bf16_kernel<A_MN, B_MN>;
     static bool attr_set = false;  // per instantiation
     if (!attr_set) {
         DOLO_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
         attr_set = true;
     }
-    const int sms = dolo_num_sms() - dolo_option_gemm_sm_margin();
-    const int grid = (p.dynamic || tiles < sms) ? tiles : sms;
+    // static persistent schedule: worker w takes tiles w, w + W, ... on `SMs - gemm_sm_margin` SMs
+    int sms = dolo_num_sms() - dolo_option_gemm_sm_margin();
+    if (sms < 1) sms = 1;
+    const int grid = p.num_tiles < sms ? p.num_tiles : sms;
     kern<<<grid, GEMM_THREADS, SMEM_BYTES, st>>>(maps, p);
     DOLO_LAUNCH_OK("gemm_bf16");
     return DOLO_OK;
@@ -709,10 +389,9 @@ struct GemmProblemArgs {
     int64_t M, N, K;
 };
 
-// Fills maps.{a,b,d}[q] and p.pr[q] for one problem.  All problems of a launch share the operand layouts, the output type,
-// the epilogue kind and the CTA-pair decision.
+// Fills maps.{a,b}[q] and p.pr[q] for one problem.  All problems of a launch share the operand layouts and the output type.
 static int setup_problem(GemmMaps& maps, GemmParams& p, int q, const GemmProblemArgs& g, int a_mn_major, int b_mn_major,
-                         int d_is_f32, int epi, bool cta_pair, const GroupArgs& ga) {
+                         int d_is_f32, const GroupArgs& ga) {
     const int64_t M = g.M, N = g.N, K = g.K;
     DOLO_REQUIRE(K > 0, "gemm: K must be > 0");
     DOLO_REQUIRE(K % 8 == 0 && N % 8 == 0, "gemm: K=%lld and N=%lld must be multiples of 8", (long long)K, (long long)N);
@@ -722,48 +401,37 @@ static int setup_problem(GemmMaps& maps, GemmParams& p, int q, const GemmProblem
     DOLO_REQUIRE(g.C == nullptr || g.ldc % (d_is_f32 ? 4 : 8) == 0, "gemm: ldc alignment");
     DOLO_REQUIRE(M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31), "gemm: dimension too large");
     // K-major: dims {K, rows}, box {64, tile rows}.  MN-major: dims {rows, K}, box {64, 64}.
-    uint64_t dims[3], strides[3];
-    uint32_t box[3];
+    uint64_t dims[2], strides[2];
+    uint32_t box[2];
+    int rc;
     if (ga.a_row_index != nullptr) {
-        // gather4: box = one row of 64 columns; the instruction names four rows of the UNGROUPED matrix
+        // gather-on-load: the producer warp reads A's rows itself (no tensor map)
         DOLO_REQUIRE(!a_mn_major, "gemm: gather-on-load needs a K-major A");
-        dims[0] = uint64_t(K); dims[1] = uint64_t(ga.a_rows); strides[0] = 2; strides[1] = uint64_t(g.lda) * 2;
-        box[0] = BK; box[1] = 1;
-    } else if (!a_mn_major) {
-        dims[0] = uint64_t(K); dims[1] = uint64_t(M); strides[0] = 2; strides[1] = uint64_t(g.lda) * 2;
-        box[0] = BK; box[1] = BM;
+        DOLO_REQUIRE((reinterpret_cast<uintptr_t>(g.A) & 15) == 0, "gemm: gather-on-load needs a 16-byte aligned A");
+        p.gather_a = g.A;
+        p.gather_lda = g.lda;
+        p.gather_k = int(K);
     } else {
-        dims[0] = uint64_t(M); dims[1] = uint64_t(K); strides[0] = 2; strides[1] = uint64_t(g.lda) * 2;
-        box[0] = 64; box[1] = BK;
+        if (!a_mn_major) {
+            dims[0] = uint64_t(K); dims[1] = uint64_t(M); strides[0] = 2; strides[1] = uint64_t(g.lda) * 2;
+            box[0] = BK; box[1] = BM;
+        } else {
+            dims[0] = uint64_t(M); dims[1] = uint64_t(K); strides[0] = 2; strides[1] = uint64_t(g.lda) * 2;
+            box[0] = 64; box[1] = BK;
+        }
+        rc = dolo_make_tmap(&maps.a[q], g.A, 2, 2, dims, strides, box, DOLO_SW_128);
+        if (rc) return rc;
     }
-    int rc = dolo_make_tmap(&maps.a[q], g.A, 2, 2, dims, strides, box, DOLO_SW_128);
-    if (rc) return rc;
+    strides[0] = 2;
     if (!b_mn_major) {
         dims[0] = uint64_t(K); dims[1] = uint64_t(ga.mode == 1 ? ga.b_total_outer : N); strides[1] = uint64_t(g.ldb) * 2;
-        box[0] = BK; box[1] = cta_pair ? BN / 2 : BN;  // pair mode: each CTA stages half of the B tile
+        box[0] = BK; box[1] = BN;
     } else {
         dims[0] = uint64_t(N); dims[1] = uint64_t(ga.mode == 1 ? ga.b_total_outer : K); strides[1] = uint64_t(g.ldb) * 2;
         box[0] = 64; box[1] = BK;
     }
     rc = dolo_make_tmap(&maps.b[q], g.B, 2, 2, dims, strides, box, DOLO_SW_128);
     if (rc) return rc;
-    if (epi == EPI_BF16_TMA) {
-        dims[0] = uint64_t(N); dims[1] = uint64_t(M); strides[1] = uint64_t(g.ldd) * 2;
-        box[0] = 64; box[1] = BM;
-        rc = dolo_make_tmap(&maps.d[q], g.D, 2, 2, dims, strides, box, DOLO_SW_128);
-        if (rc) return rc;
-    } else if (epi == EPI_F32_TMA_STORE || epi == EPI_F32_TMA_ADD) {
-        // fp32 [groups, M, N]: one box = 32 columns (128 B) x 32 rows, the slab of one epilogue warp
-        const int64_t groups = ga.mode == 2 ? ga.num_groups : 1;
-        dims[0] = uint64_t(N); dims[1] = uint64_t(M); dims[2] = uint64_t(groups);
-        strides[1] = uint64_t(g.ldd) * 4;
-        strides[2] = uint64_t(ga.mode == 2 ? ga.d_group_stride : M * g.ldd) * 4;
-        box[0] = 32; box[1] = 32; box[2] = 1;
-        rc = dolo_make_tmap(&maps.d[q], g.D, 4, 3, dims, strides, box, DOLO_SW_128);
-        if (rc) return rc;
-    } else {
-        maps.d[q] = maps.a[q];  // unused
-    }
     Problem& pr = p.pr[q];
     pr.D = g.D;
     pr.C = g.C;
@@ -774,21 +442,20 @@ static int setup_problem(GemmMaps& maps, GemmParams& p, int q, const GemmProblem
     pr.N = int(N);
     pr.alpha = g.alpha;
     pr.beta = g.C ? g.beta : 0.f;
-    pr.epi = epi;
     pr.hint_a = pr.hint_b = TMA_HINT_NORMAL;
-    if (dolo_option_gemm_l2_hints() && ga.mode == 0 && K >= 4096 && (M + N) * K * 2 > (48ll << 20)) {
+    if (dolo_option_gemm_l2_hints() && ga.mode == 0 && K >= 4096 && (M + N) * K * 2 > (24ll << 20)) {
         // long contraction, operands larger than what the L2 keeps anyway: stream the bigger one, keep the smaller one
         const bool a_smaller = M <= N;
         pr.hint_a = a_smaller ? TMA_HINT_EVICT_LAST : TMA_HINT_EVICT_FIRST;
         pr.hint_b = a_smaller ? TMA_HINT_EVICT_FIRST : TMA_HINT_EVICT_LAST;
     }
-    pr.num_m = cta_pair ? int((M + 2 * BM - 1) / (2 * BM)) : int((M + BM - 1) / BM);  // pair mode: 256-row super tiles
+    pr.num_m = int((M + BM - 1) / BM);
     pr.num_n = int((N + BN - 1) / BN);
     pr.num_kb = int((K + BK - 1) / BK);
     {
-        // A panel of group_m x 128 rows x K bf16 should fit comfortably in L2 next to the streaming B tiles
-        const int64_t panel_bytes = int64_t(cta_pair ? 2 * BM : BM) * K * 2;
-        int64_t gm = (24ll << 20) / (panel_bytes > 0 ? panel_bytes : 1);
+        // A panel of group_m x 128 rows x K bf16 should fit comfortably in the 50 MB L2 next to the streaming B tiles
+        const int64_t panel_bytes = int64_t(BM) * K * 2;
+        int64_t gm = (12ll << 20) / (panel_bytes > 0 ? panel_bytes : 1);
         if (gm < 4) gm = 4;
         if (gm > 64) gm = 64;
         pr.group_m = int(gm);
@@ -804,17 +471,6 @@ static int dispatch_layout(int a_mn_major, int b_mn_major, Ts&&... args) {
     return launch_gemm<true, true>(args...);
 }
 
-// fp32 outputs go through the TMA epilogue when they are a plain overwrite (no C) or an in-place accumulation
-// (C == D, beta == 1) without bias: exactly the two forms a weight gradient takes
-static int pick_epilogue(int d_is_f32, const void* C, const void* D, float beta, const void* bias, bool tma_store,
-                         int group_mode) {
-    if (!d_is_f32) return tma_store ? EPI_BF16_TMA : EPI_DIRECT;
-    if (bias != nullptr || group_mode == 3 || !dolo_option_gemm_f32_tma_epilogue()) return EPI_DIRECT;
-    if (C == nullptr) return EPI_F32_TMA_STORE;
-    if (C == D && beta == 1.f) return EPI_F32_TMA_ADD;
-    return EPI_DIRECT;
-}
-
 static int gemm_impl(const void* A, int64_t lda, int a_mn_major, const void* B, int64_t ldb, int b_mn_major, void* D,
                      int64_t ldd, int d_is_f32, const void* C, int64_t ldc, float alpha, float beta, const void* bias,
                      int64_t M, int64_t N, int64_t K, int flags, void* stream, const GroupArgs& ga) {
@@ -822,20 +478,11 @@ static int gemm_impl(const void* A, int64_t lda, int a_mn_major, const void* B, 
     if (M == 0 || N == 0) return DOLO_OK;
     const bool tma_store = (flags & DOLO_GEMM_FLAG_TMA_STORE) != 0;
     DOLO_REQUIRE(!tma_store || (!d_is_f32 && C == nullptr), "gemm: TMA-store epilogue needs bf16 D and no C");
-    // CTA-pair (cta_group::2) kernel: at least one full 256-row super tile; M-grouped problems need their expert segments
-    // padded to 256 rows (both halves of a super tile then belong to the same expert); not for split-K
-    const bool cta_pair = (ga.mode == 0 || (ga.mode == 1 && M % (2 * BM) == 0) || ga.mode == 2) && M >= 2 * BM &&
-                          ((flags & DOLO_GEMM_FLAG_CTA_PAIR) != 0 || dolo_option_gemm_cta_pair() != 0) &&
-                          (flags & DOLO_GEMM_FLAG_NO_CTA_PAIR) == 0;
-    int epi = pick_epilogue(d_is_f32, C, D, beta, bias, tma_store, ga.mode);
-    if ((flags & DOLO_GEMM_FLAG_DIRECT_EPILOGUE) != 0 && d_is_f32) epi = EPI_DIRECT;
-    if ((flags & DOLO_GEMM_FLAG_F32_TMA_EPILOGUE) != 0 && d_is_f32 && bias == nullptr && ga.mode != 3)
-        epi = C == nullptr ? EPI_F32_TMA_STORE : ((C == D && beta == 1.f) ? EPI_F32_TMA_ADD : EPI_DIRECT);
     GemmMaps maps;
     GemmParams p;
     memset(&p, 0, sizeof(p));
     GemmProblemArgs g{A, lda, B, ldb, D, ldd, C, ldc, bias, alpha, beta, M, N, K};
-    int rc = setup_problem(maps, p, 0, g, a_mn_major, b_mn_major, d_is_f32, epi, cta_pair, ga);
+    int rc = setup_problem(maps, p, 0, g, a_mn_major, b_mn_major, d_is_f32, ga);
     if (rc) return rc;
     p.n_prob = 1;
     p.pr[0].tile_start = 0;
@@ -843,19 +490,18 @@ static int gemm_impl(const void* A, int64_t lda, int a_mn_major, const void* B, 
     p.d_is_f32 = d_is_f32;
     p.grouped = ga.mode;
     p.m_tile_group = ga.m_tile_group;
-    p.m_tile_shift = cta_pair ? 1 : 0;
     p.a_row_index = ga.a_row_index;
     p.b_group_rows = int(ga.b_group_rows);
     p.group_k_offsets = ga.group_k_offsets;
     p.num_groups = ga.num_groups;
     p.d_group_stride = ga.d_group_stride;
-    return dispatch_layout(a_mn_major, b_mn_major, maps, p, static_cast<cudaStream_t>(stream), cta_pair);
+    return dispatch_layout(a_mn_major, b_mn_major, maps, p, static_cast<cudaStream_t>(stream));
 }
 
 // The weight gradients of one transformer block in ONE persistent launch (autograd of linear.py:5-25 for c_attn, attention
 // c_proj, c_fc and mlp c_proj): dW_i[M_i, N_i] (+)= alpha_i * dY_i^T X_i with dY_i [K, M_i], X_i [K, N_i] row-major
-// activations (both operands MN-major).  Launched one by one these GEMMs lose 10-30 % to wave quantisation (c_attn: 300
-// pair tiles on 74 CTA pairs = 4.05 waves; attention c_proj: 1.35 waves); together they are 1600 tiles = 21.6 waves.
+// activations (both operands MN-major).  Launched one by one these GEMMs lose to wave quantisation on the last,
+// partly filled wave of each; together the tail is paid once.
 extern "C" int dolomite_b200_gemm_bf16_wgrad_multi(int n_problems, const void* const* dY, const int64_t* ld_dy,
                                                    const void* const* X, const int64_t* ld_x, float* const* dW,
                                                    const int64_t* ld_dw, const int64_t* M, const int64_t* N, int64_t K,
@@ -864,15 +510,12 @@ extern "C" int dolomite_b200_gemm_bf16_wgrad_multi(int n_problems, const void* c
     GemmMaps maps;
     GemmParams p;
     memset(&p, 0, sizeof(p));
-    bool pair = dolo_option_gemm_cta_pair() != 0;
-    for (int q = 0; q < n_problems; ++q) pair = pair && M[q] >= 2 * BM;
     int tiles = 0;
     for (int q = 0; q < n_problems; ++q) {
         DOLO_REQUIRE(M[q] > 0 && N[q] > 0, "wgrad_multi: empty problem %d", q);
         GemmProblemArgs g{dY[q], ld_dy[q], X[q], ld_x[q], dW[q], ld_dw[q], accumulate[q] ? dW[q] : nullptr, ld_dw[q], nullptr,
                           alpha[q], 1.f, M[q], N[q], K};
-        const int epi = !dolo_option_gemm_f32_tma_epilogue() ? EPI_DIRECT : (accumulate[q] ? EPI_F32_TMA_ADD : EPI_F32_TMA_STORE);
-        int rc = setup_problem(maps, p, q, g, 1, 1, 1, epi, pair, GroupArgs());
+        int rc = setup_problem(maps, p, q, g, 1, 1, 1, GroupArgs());
         if (rc) return rc;
         p.pr[q].tile_start = tiles;
         tiles += p.pr[q].num_m * p.pr[q].num_n;
@@ -882,7 +525,7 @@ extern "C" int dolomite_b200_gemm_bf16_wgrad_multi(int n_problems, const void* c
     p.d_is_f32 = 1;
     p.grouped = 0;
     p.num_groups = 1;
-    return launch_gemm<true, true>(maps, p, static_cast<cudaStream_t>(stream), pair);
+    return launch_gemm<true, true>(maps, p, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int dolomite_b200_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const void* B, int64_t ldb,

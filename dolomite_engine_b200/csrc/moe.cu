@@ -4,11 +4,11 @@
 //
 // Device-side only, no host sync (the eager reference calls .tolist(), moe/base.py:33):
 //   route      : top-k on the raw router logits, fp32 softmax over the k selected, per-expert histogram
-//   plan       : expert segments padded to 256 rows (CTA-pair super tiles) -> offsets, 128-row tile->expert table, row assignment
+//   plan       : expert segments padded to 256 rows (two 128-row GEMM tiles) -> offsets, 128-row tile->expert table, row assignment
 //   gather     : X_g[row] = x[token(row)] (zero rows for padding) -- operand of the grouped c_fc GEMM
 //   combine    : y[t] = sum_j w[t,j] * Y_g[row(t,j)]            -- after the grouped c_proj GEMM
 //   backward   : dY_g rows / gate-weight grads, token-sum of dX_g rows, softmax-over-k backward to dense dlogits
-// The expert GEMMs themselves are the tcgen05 GEMM in grouped mode (gemm.cu).
+// The expert GEMMs themselves are the wgmma GEMM in grouped mode (gemm.cu).
 #include "common.cuh"
 #include "../../include/dolomite_b200.h"
 
@@ -17,7 +17,7 @@ using namespace dolo;
 namespace {
 
 constexpr int MOE_TILE = 128;  // granularity of the tile -> expert table (one entry per 128 grouped rows)
-constexpr int MOE_PAD = 256;   // expert segments are padded to 256 rows: one CTA-pair super tile of the grouped GEMM
+constexpr int MOE_PAD = 256;   // expert segments are padded to 256 rows (a multiple of the 128-row GEMM tile)
 
 __device__ __forceinline__ void unpack8(const uint4& v, float (&f)[8]) {
     f[0] = bf16_lo(v.x); f[1] = bf16_hi(v.x);
@@ -113,18 +113,37 @@ __global__ void moe_plan_kernel(const int32_t* __restrict__ counts, int E, int32
     }
 }
 
-__global__ void moe_assign_kernel(const int32_t* __restrict__ sel_idx, int64_t n_slots,
-                                  const int32_t* __restrict__ offsets_padded, int32_t* __restrict__ cursors,
-                                  int32_t* __restrict__ row_of_slot, int32_t* __restrict__ slot_of_row,
-                                  int32_t* __restrict__ token_of_row, int k) {
-    const int64_t s = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
-    if (s >= n_slots) return;
-    const int e = sel_idx[s];
-    const int pos = atomicAdd(cursors + e, 1);
-    const int row = offsets_padded[e] + pos;
-    row_of_slot[s] = row;
-    slot_of_row[row] = int32_t(s);
-    token_of_row[row] = int32_t(s / k);
+// Grouped row of every token-slot: expert e's slots take the rows of its segment in slot (= token) order, a stable
+// assignment that is the same on every run (an atomic cursor would hand out rows in arrival order).  One block per
+// expert scans all slots in chunks of blockDim: ballot + popc give each matching slot its rank inside the chunk.
+__global__ void __launch_bounds__(1024)
+    moe_assign_kernel(const int32_t* __restrict__ sel_idx, int64_t n_slots, const int32_t* __restrict__ offsets_padded,
+                      int32_t* __restrict__ row_of_slot, int32_t* __restrict__ slot_of_row,
+                      int32_t* __restrict__ token_of_row, int k) {
+    __shared__ int warp_cnt[32];
+    const int e = blockIdx.x;
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    int base = offsets_padded[e];
+    for (int64_t c0 = 0; c0 < n_slots; c0 += blockDim.x) {
+        const int64_t s = c0 + threadIdx.x;
+        const bool m = s < n_slots && sel_idx[s] == e;
+        const uint32_t bal = __ballot_sync(0xffffffffu, m);
+        if (lane == 0) warp_cnt[wid] = __popc(bal);
+        __syncthreads();
+        int before = 0, total = 0;
+        for (int w = 0; w < nw; ++w) {
+            before += w < wid ? warp_cnt[w] : 0;
+            total += warp_cnt[w];
+        }
+        if (m) {
+            const int row = base + before + __popc(bal & ((1u << lane) - 1u));
+            row_of_slot[s] = row;
+            slot_of_row[row] = int32_t(s);
+            token_of_row[row] = int32_t(s / k);
+        }
+        base += total;
+        __syncthreads();  // warp_cnt is rewritten by the next chunk
+    }
 }
 
 // X_g[row] = x[slot_of_row[row] / k]  (zeros for padding rows); one warp per row
@@ -272,8 +291,7 @@ extern "C" int dolomite_b200_moe_route(const void* router_logits, int64_t T, int
     DOLO_LAUNCH_OK("moe_plan");
     if (T > 0) {
         const int64_t n = T * k;
-        moe_assign_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(sel_idx, n, offsets_padded, cursors, row_of_slot,
-                                                                       slot_of_row, token_of_row, k);
+        moe_assign_kernel<<<E, 1024, 0, st>>>(sel_idx, n, offsets_padded, row_of_slot, slot_of_row, token_of_row, k);
         DOLO_LAUNCH_OK("moe_assign");
     }
     return DOLO_OK;

@@ -10,7 +10,7 @@ One FlatUnit per transformer block + one root unit (same wrapping as `transforme
             done (last micro-step only, i.e. outside `no_sync`) `ncclReduceScatter(AVG)` on the communication
             stream overlaps the next unit's backward (N2)
 
-B200-first choices: the gathered bf16 parameters of a 3.5 B (8 B) model are 7 GB (16 GB) of 180 GB HBM, so units
+Placement choices: the gathered bf16 parameters of a 3.5 B (8 B) model are 7 GB (16 GB) of an 80 GB H100, so units
 stay resident between forward and backward (`reshard_after_forward=False`; one all-gather per unit per optimizer
 step instead of the reference's two per micro-step) unless stage-3 resharding is requested; gather/gradient buffers
 are allocated once (no allocator churn, no record_stream); scalar collectives (loss AVG, grad-norm SUM) stay on
@@ -49,7 +49,7 @@ def hybrid_layout(world_size: int, sharding_world_size: int | None, replication_
     sharded inside a shard group and replicated across the groups; gradients are reduce-scattered inside the shard group
     and then all-reduced between the ranks that own the same slice.
 
-    B200-first placement: a shard group is `sharding_world_size` CONSECUTIVE ranks (one NVSwitch domain), so the large
+    Placement: a shard group is `sharding_world_size` CONSECUTIVE ranks (one NVSwitch domain), so the large
     per-unit all-gather / reduce-scatter stay on NVLink and only the 1/S-sized shard all-reduce crosses nodes."""
     if replication_world_size is None or sharding_world_size is None:
         if replication_world_size is not None or sharding_world_size is not None:
@@ -423,7 +423,7 @@ def wrap_model_for_distributed_training(args, model: nn.Module) -> nn.Module:
     what `reshard_after_forward = stage == 3` / FULL_SHARD does in the reference (distributed/__init__.py:161-176,
     :205-213); 0 / 2 keep every unit's gathered parameters and full gradients resident (SHARD_GRAD_OP-like) --,
     `communication_dtype`, `fsdp_algorithm` (both map to the same flat-bucket runtime), and rejects what is out of scope.
-    The one B200-specific key is `reshard_after_forward` (default None = follow `stage`): `false` together with
+    The one key the reference does not have is `reshard_after_forward` (default None = follow `stage`): `false` together with
     `stage: 3` opts into the resident mode, which trades ~6 B / parameter of HBM for one all-gather per unit and step."""
     dargs = getattr(args, "distributed_args", None)
     stage = getattr(dargs, "stage", 3) if dargs is not None else 3

@@ -117,7 +117,7 @@ class DolomitePreTrainedModel(nn.Module):
         if device is None:
             if not torch.cuda.is_available():
                 raise RuntimeError(
-                    "dolomite_engine_b200 needs a CUDA device (sm_100a); there is no CPU path. "
+                    "dolomite_engine_b200 needs a CUDA device (sm_90a); there is no CPU path. "
                     "Use oracle/ for CPU reference computations in tests."
                 )
             device = torch.device("cuda", torch.cuda.current_device())
@@ -300,8 +300,8 @@ class DolomitePreTrainedModel(nn.Module):
 
     def extra_repr(self) -> str:
         return (
-            f"{type(self).__name__}(PaddingFreeAttention[tcgen05], RMSNorm[cuda], RoPE[cuda], "
-            f"{'ScatterMoE[tcgen05 grouped gemm]' if self.engine.is_moe else 'MLP[tcgen05 gemm]'}, "
+            f"{type(self).__name__}(PaddingFreeAttention[wgmma], RMSNorm[cuda], RoPE[cuda], "
+            f"{'ScatterMoE[wgmma grouped gemm]' if self.engine.is_moe else 'MLP[wgmma gemm]'}, "
             f"params={self.engine.num_parameters():,})"
         )
 

@@ -1,6 +1,6 @@
 """Thin torch-tensor wrappers over the C ABI (include/dolomite_b200.h).
 
-torch is used only for device memory and streams; every computation below is a hand-written sm_100a kernel.
+torch is used only for device memory and streams; every computation below is a hand-written sm_90a kernel.
 All functions launch on torch's current CUDA stream and never synchronise.
 """
 
@@ -279,7 +279,8 @@ def dropout_bwd(dy, p: float, keys: tuple[int, int], pre_mul: float = 1.0, out=N
 # ------------------------------------------------------------------------------------------------
 def sumsq_accum(g, out):
     _req(g, torch.float32, "g")
-    _lib.call("dolomite_b200_sumsq_accum", g.data_ptr(), g.numel(), out.data_ptr(), _stream())
+    ws = _workspace(_lib.load().dolomite_b200_sumsq_workspace_bytes(), g.device)
+    _lib.call("dolomite_b200_sumsq_accum", g.data_ptr(), g.numel(), out.data_ptr(), ws.data_ptr(), _stream())
 
 
 def clip_coef(sumsq, max_norm: float, coef_out, norm_out=None):
@@ -307,11 +308,10 @@ def accum_bf16_into_f32(src, dst, scale=1.0):
 # ------------------------------------------------------------------------------------------------
 GEMM_TMA_STORE = 1
 GEMM_SPLITK_ACCUMULATE = 2
-GEMM_DIRECT_EPILOGUE = 16  # fp32 D through per-thread 128-byte row segments (the default)
-GEMM_F32_TMA_EPILOGUE = 32  # fp32 D through shared memory + TMA tile store / reduce-add (measured slower; A/B tests)
-# Split-K + fp32-atomic accumulation of weight gradients was measured SLOWER than read-modify-write on B200
-# (profiles/r01_probe_wgrad_splitk.json: 20480x2560x8192 2.64 ms vs 0.65 ms -- L2 atomic throughput), so it is off;
-# the entry point stays for shapes with very few output tiles.
+GEMM_DIRECT_EPILOGUE = 16  # epilogue selection flags of the ABI: accepted, no effect on sm_90 (see include/dolomite_b200.h)
+GEMM_F32_TMA_EPILOGUE = 32
+# Split-K + fp32-atomic accumulation of weight gradients is off for the block weight gradients (many output tiles, the
+# fp32 atomics cost L2 throughput); the entry point stays for shapes with very few output tiles.
 wgrad_splitk = False
 _default_gemm_flags = GEMM_TMA_STORE
 gemm_timer = None  # bench.py: list collecting (flops, start_event, end_event) per GEMM launch
@@ -541,7 +541,7 @@ def gemm_grouped_m(a, w3, plan: MoEPlan, *, b_mn: bool, alpha: float = 1.0, flag
 
 
 def gemm_grouped_m_gather(x, w3, plan: MoEPlan, alpha: float = 1.0, flags=None):
-    """expert forward with the gather fused into the operand load (TMA gather4): x [T, K] UNGROUPED, w3 [E, N, K] ->
+    """expert forward with the gather fused into the operand load (rows copied by the producer warp): x [T, K] UNGROUPED, w3 [E, N, K] ->
     D[row] = x[token_of_row[row]] W[expert(row)]^T for every grouped row (moe/scatter.py:38-49 `parallel_linear`)"""
     _req(x, _BF16, "x"), _req(w3, _BF16, "w3")
     T, K = x.shape

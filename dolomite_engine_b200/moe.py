@@ -2,7 +2,7 @@
 ScatterMoE, moe_dolomite/layer.py:51-95 SparseMoEBlock).
 
     router logits = x gate^T -> top-k on raw logits -> fp32 softmax over the k selected -> bf16 weights
-    tokens grouped by expert (segments padded to 128 rows)  -> grouped tcgen05 GEMM c_fc -> SwiGLU
+    tokens grouped by expert (segments padded to 128 rows)  -> grouped wgmma GEMM c_fc -> SwiGLU
     -> grouped GEMM c_proj -> gate-weighted combine (+ m_residual scale + residual add fused)
 
 ScatterMoE forbids biases (moe/scatter.py:22); so does this path.  Activations stay grouped between the two expert
@@ -15,9 +15,8 @@ import os
 
 from . import kernels as K
 
-# DOLO_MOE_FUSED_GATHER=1: the expert c_fc GEMM gathers its token rows itself (TMA gather4 in the producer warp).  Exact, but
-# measured 2.3x SLOWER than gather kernel + grouped GEMM on the C4 layer (3.09 vs 1.35 ms, profiles/r02_probe_call70.jsonl):
-# one gather4 moves 512 B and the operand ring needs one every 16 cycles, which the TMA unit does not sustain.  Off by default.
+# DOLO_MOE_FUSED_GATHER=1: the expert c_fc GEMM gathers its token rows itself (the producer warp copies them into the
+# operand ring).  Exact; off by default: one warp's loads do not keep the ring as full as TMA loads of a gathered copy.
 FUSED_GATHER = os.environ.get("DOLO_MOE_FUSED_GATHER", "0") == "1"
 
 
@@ -31,7 +30,7 @@ def forward(engine, unit, p: str, x, residual, m_res: float, layer: int = 0):
     plan = K.moe_route(logits, k)
     if FUSED_GATHER:
         # scattermoe `parallel_linear(grouped_in=False, grouped_out=True)`: the expert GEMM reads the token rows straight
-        # out of x (TMA gather4 in its producer warp); no grouped copy of x is written in forward
+        # out of x (copied by its producer warp); no grouped copy of x is written in forward
         fc = K.gemm_grouped_m_gather(x, unit.views[p + "mlp.c_fc.weight"], plan)
     else:
         fc = K.gemm_grouped_m(K.moe_gather(x, plan), unit.views[p + "mlp.c_fc.weight"], plan, b_mn=False)
@@ -71,8 +70,8 @@ def backward(engine, unit, p: str, x, dh, m_res: float, saved, layer: int = 0):
     dlogits = K.moe_router_bwd(plan, dw)
     gate = unit.views[p + "mlp.gate.weight"]
     ggate = unit.gviews[p + "mlp.gate.weight"]
-    # dGate[E, H] += dlogits^T x: E = 8 rows are ONE row of output tiles (8 tiles at H = 2048) with the whole token stream as
-    # contraction -- split-K over the SMs (fp32 atomics on 8 valid rows per tile) instead of 8 busy SMs for 70 us per layer
-    K.gemm(dlogits, x, a_mn=True, b_mn=True, out=ggate, c=ggate, beta=1.0, flags=K.GEMM_SPLITK_ACCUMULATE)
+    # dGate[E, H] += dlogits^T x: E rows are one row of output tiles with the whole token stream as contraction.  Not split
+    # over K: the fp32 atomics of a split-K launch sum in arrival order, and the training step is bit-identical run to run.
+    K.gemm(dlogits, x, a_mn=True, b_mn=True, out=ggate, c=ggate, beta=1.0, flags=0)
     dx = K.gemm(dlogits, gate, b_mn=True, out=dx, c=dx, beta=1.0, flags=0)          # dx += dlogits gate
     return dx

@@ -2,7 +2,7 @@
 
 Same control flow: zero_grad, (grad_accum-1) micro-steps under no_sync, last micro-step with gradient sync
 (reduce-scatter), clip, optimizer + scheduler step, loss /= grad_accum, loss AVG all-reduce.  Differences, all
-B200-first: the loss / grad-norm stay on the device (`return_tensors=True`) so that the host never stalls the
+for throughput: the loss / grad-norm stay on the device (`return_tensors=True`) so that the host never stalls the
 launch queue -- `.item()` is only paid when the caller asks for floats, like the reference does every step."""
 
 from __future__ import annotations
@@ -79,8 +79,8 @@ def get_model_tflops(config, batch_size: int, sequence_length: int, checkpointed
 
 def get_torch_profiler(trace_path: str | None, rank: int = 0, wait: int = 5, warmup: int = 5):
     """`logging_args.torch_profiler_trace_path` (train_utils.py:182-194): one traced step on rank 0 after `wait + warmup`
-    steps, written as a TensorBoard trace; other ranks never reach their window.  The kernel-level evidence of this repo
-    comes from ncu (profiles/); this is the reference's timeline view of the same loop."""
+    steps, written as a TensorBoard trace; other ranks never reach their window.  This is the reference's timeline view of
+    the loop."""
     if trace_path is None:
         return None
     acts = [torch.profiler.ProfilerActivity.CPU]

@@ -1,5 +1,5 @@
 /*
- * dolomite_b200.h -- C ABI of the B200-native (sm_100a) hot path of dolomite-engine.
+ * dolomite_b200.h -- C ABI of the H100-native (sm_90a) hot path of dolomite-engine.
  *
  * Scope: the data-parallel GPTDolomite / MoEDolomite training step (SURVEY.md section 8).  The reference
  * (ibm-granite/dolomite-engine @ 2024_08_07) is pure Python and reaches its GPU kernels through
@@ -14,6 +14,8 @@
  *   - all pointers are DEVICE pointers unless the name ends in _host.  The callee never allocates, frees
  *     or retains device memory and never synchronises the stream.
  *   - `stream` is a cudaStream_t passed as void*.
+ *   - results are bit-identical from run to run on the same inputs (every reduction sums in a fixed order), except
+ *     for the split-K flag of dolomite_b200_gemm_bf16.
  *   - activations/weights are bf16 (uint16 storage), statistics / master weights / gradients-of-weights fp32.
  *   - row-major everywhere; `ld*` are leading dimensions in ELEMENTS.
  */
@@ -37,17 +39,12 @@ const char* dolomite_b200_last_error(void);
 int dolomite_b200_abi_version(void);
 int dolomite_b200_device_info(int* sm_count, int* cc_major, int* cc_minor);
 /* process-wide tuning knobs:
- *   "gemm_cta_pair"    0 | 1 (dense GEMMs on 2-CTA clusters with tcgen05.mma.cta_group::2)
- *   "gemm_sm_margin"   SMs the persistent GEMM grids leave free for concurrent communication kernels (static schedule only)
- *   "gemm_dynamic"     1 | 0 (default 1: one cluster per output tile; running clusters take over pending ones through cluster launch
- *                      control, so the grid uses every SM that is or becomes free -- no margin needed next to NCCL kernels)
- *   "attn_fwd_split"   1 | 0 | 2 | 3 (split-softmax attention forward -- one CTA per SM, double-buffered scores in TMEM, several
- *                      threads per query row -- for head_dim >= 96 (1, default), never (0), also for head_dim 64 / 80 (2);
- *                      3 = like 2 with FOUR instead of two threads per query row)
+ *   "gemm_sm_margin"   SMs the persistent GEMM grids leave free for concurrent communication kernels
  *   "attn_head_fastest" heads per chunk of the attention CTA order (default 8: inside a chunk heads fastest + longest tiles
- *                      first, so that the last wave is short tiles; 0 = tiles fastest, round 1's order)
+ *                      first, so that the last wave is short tiles; 0 = tiles fastest)
  *   "gemm_l2_hints"    1 | 0 (long-contraction GEMMs load the streamed operand evict-first and the re-used one evict-last)
- *   "gemm_f32_tma_epilogue" 0 | 1 (fp32 weight gradients through TMA tile store / reduce-add instead of per-thread stores) */
+ * Accepted and reported back, but without effect on sm_90 (one kernel per job): "gemm_cta_pair", "gemm_dynamic",
+ * "gemm_f32_tma_epilogue", "attn_fwd_split", "attn_bwd_variant", "attn_bwd_ablate". */
 int dolomite_b200_set_option(const char* key, int value);
 int dolomite_b200_get_option(const char* key, int* value);
 
@@ -171,11 +168,13 @@ int dolomite_b200_dropout_bwd(const void* dy, void* dx, int64_t n, float p, floa
 
 /* ------------------------------------------------------------------------------------------------
  * Optimizer-side flat-shard kernels (train_utils.py:99-106: clip_grad_norm_ + AdamW step).
- *   sumsq: out[0] += sum(g^2)  (fp32 grads).   clip coef: coef = min(1, max_norm / (sqrt(sumsq) + 1e-6)).
+ *   sumsq: out[0] += sum(g^2)  (fp32 grads), summed in a fixed order (bit-identical from run to run); workspace:
+ *   dolomite_b200_sumsq_workspace_bytes() bytes, 4-byte aligned.   clip coef: coef = min(1, max_norm / (sqrt(sumsq) + 1e-6)).
  *   adamw: torch.optim.AdamW semantics on fp32 master shard; also emits the bf16 copy that the next
  *   all-gather ships.  `clip_coef` is a device pointer (nullable -> 1).  step >= 1.
  * ------------------------------------------------------------------------------------------------ */
-int dolomite_b200_sumsq_accum(const float* g, int64_t n, float* out, void* stream);
+int64_t dolomite_b200_sumsq_workspace_bytes(void);
+int dolomite_b200_sumsq_accum(const float* g, int64_t n, float* out, void* workspace, void* stream);
 int dolomite_b200_clip_coef(const float* sumsq, float max_norm, float* coef_out, float* norm_out, void* stream);
 int dolomite_b200_adamw_step(float* p, const float* g, float* m, float* v, void* p_bf16, int64_t n, float lr,
                              float beta1, float beta2, float eps, float weight_decay, int64_t step,
@@ -198,7 +197,7 @@ int dolomite_b200_attn_decode(const void* qkv, int64_t row_stride, const void* k
                               float softmax_scale, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * bf16 GEMM on tcgen05 tensor cores (TMA -> smem -> tcgen05.mma -> TMEM -> epilogue), replacing the cuBLAS
+ * bf16 GEMM on Hopper tensor cores (TMA -> smem -> wgmma -> register accumulators -> epilogue), replacing the cuBLAS
  * calls behind nn.Linear (linear.py:5-25; call sites attention/base.py:100, padding_free.py:74,
  * gpt_dolomite/mlp.py:46-48, gpt_dolomite/main.py:172-177) and their autograd (dgrad / wgrad).
  *
@@ -208,18 +207,17 @@ int dolomite_b200_attn_decode(const void* qkv, int64_t row_stride, const void* k
  *   B is logical [N,K]: b_mn_major == 0 -> stored row-major [N,K] (ld = ldb);  1 -> stored [K,N] (ld = ldb).
  *   D/C: row-major [M,N]; d_is_f32 selects fp32 (else bf16) for BOTH D and C.  C may be NULL (beta ignored)
  *   or alias D.  bias: bf16 [N] or NULL.   K % 8 == 0, lds % 8 == 0, 16-byte aligned bases.
- *   flags: bit0 = epilogue via smem staging + TMA store (bf16 D, no C), else direct vector stores.
+ *   flags: bit0 = the caller promises bf16 D and no C (checked); the epilogue always stores from the registers.
  * ------------------------------------------------------------------------------------------------ */
 #define DOLO_GEMM_FLAG_TMA_STORE 1
 /* bit1: D(fp32) += alpha*A.B^T with split-K + fp32 vector atomics (weight gradients); C must be NULL or alias D with
  * beta == 1, bias NULL.  Summation order over K splits is not deterministic (like FSDP's own reduce order). */
 #define DOLO_GEMM_FLAG_SPLITK_ACCUMULATE 2
-/* bit2 / bit3: force / forbid the CTA-pair kernel (tcgen05.mma.cta_group::2, 256 x 256 tiles on a 2-CTA cluster);
- * default follows the "gemm_cta_pair" option. */
+/* bit2 / bit3: force / forbid a CTA-pair kernel: accepted, no effect on sm_90 (no paired MMA). */
 #define DOLO_GEMM_FLAG_CTA_PAIR 4
 #define DOLO_GEMM_FLAG_NO_CTA_PAIR 8
-/* bit4 / bit5: fp32 D through per-thread 128-byte row segments (the default) / through shared memory + TMA tile store or
- * reduce-add (measured slower, kept for A/B tests; also the "gemm_f32_tma_epilogue" option) */
+/* bit4 / bit5: epilogue selection of other GPU generations: accepted, no effect on sm_90 (fp32 D is stored from the
+ * registers). */
 #define DOLO_GEMM_FLAG_DIRECT_EPILOGUE 16
 #define DOLO_GEMM_FLAG_F32_TMA_EPILOGUE 32
 int dolomite_b200_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const void* B, int64_t ldb, int b_mn_major,
@@ -247,7 +245,7 @@ int dolomite_b200_gemm_bf16_wgrad_multi(int n_problems, const void* const* dY, c
 int dolomite_b200_gemm_bf16_grouped_m(const void* A, int64_t lda, const void* B, int64_t ldb, int b_mn_major, void* D,
                                       int64_t ldd, float alpha, int64_t M_max, int64_t N, int64_t K,
                                       const int32_t* m_tile_group, int num_groups, int flags, void* stream);
-/* grouped_m with the gather fused into the operand load (TMA gather4): A is the UNGROUPED [a_rows, K] activation matrix,
+/* grouped_m with the gather fused into the operand load: A is the UNGROUPED [a_rows, K] activation matrix,
  * a_row_index[r] (int32, 16-byte aligned, M_max entries) the source row of grouped row r; W stored [G, N, K]. */
 int dolomite_b200_gemm_bf16_grouped_m_gather(const void* A, int64_t lda, int64_t a_rows, const int32_t* a_row_index,
                                              const void* B, int64_t ldb, void* D, int64_t ldd, float alpha, int64_t M_max,
@@ -264,7 +262,7 @@ int dolomite_b200_gemm_bf16_grouped_k(const void* A, int64_t lda, const void* B,
  *              counts[E] (== bincount, bit exact), offsets_padded[E+1], m_tile_group[max_rows/128], cursors[E] scratch,
  *              row_of_slot[T*k] (grouped row of token-slot), slot_of_row[max_rows] (-1 = padding row),
  *              token_of_row[max_rows] (source token of a grouped row; padding rows name token 0) -- the row index of
- *              dolomite_b200_gemm_bf16_grouped_m_gather.  Segments are padded to 256 rows (CTA-pair super tiles).
+ *              dolomite_b200_gemm_bf16_grouped_m_gather.  Segments are padded to 256 rows.
  *   moe_gather: X_g[row] = x[slot_of_row[row] / k] or 0.     moe_combine: out = c + alpha * sum_j w_j * Y_g[row_j].
  *   moe_combine_bwd / moe_token_sum / moe_router_bwd: their backward pieces.
  * ------------------------------------------------------------------------------------------------ */

@@ -2,8 +2,8 @@
 
 TEST / MEASUREMENT INFRASTRUCTURE ONLY (same rule as oracle/dolomite_oracle.py): nothing under dolomite_engine_b200/
 imports this module; `bench.py --impl gpu_reference` (and the `gpu_reference` key of the normal bench line) times it next
-to the B200 engine on the same GPU, tests use it as a bf16 cross-check.  It answers BASELINE.md section 3 row 2: what the
-unmodified reference would run on this B200 --
+to the H100 engine on the same GPU, tests use it as a bf16 cross-check.  It answers: what the
+unmodified reference would run on the same GPU --
 
     nn.Linear                    -> F.linear on bf16 copies of fp32 parameters (cuBLAS; FSDP MixedPrecision(param_dtype=bf16),
                                     distributed/__init__.py:146-159)

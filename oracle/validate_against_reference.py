@@ -131,7 +131,7 @@ def close(a, b, atol, what):
 
 
 CONFIGS = {
-    # C1 of BASELINE.json / SURVEY section 8d
+    # C1 of SURVEY section 8d
     "c1": dict(vocab_size=2048, n_positions=1024, n_embd=256, n_layer=2, n_head=4, n_inner=1024,
                activation_function="swiglu", attention_head_type="mha", add_bias=False),
     # granite-style multipliers + bias + gqa, head_dim 16

@@ -16,7 +16,7 @@ def pytest_configure(config):
         torch.set_num_threads(min(16, os.cpu_count() or 1))
     except Exception:
         pass
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def _has_cuda() -> bool:

@@ -57,8 +57,8 @@ def test_argument_validation_happens_before_any_launch(lib):
         _lib.call("dolomite_b200_attn_varlen_fwd", None, 1024, None, None, None, 1, 16, 16, 1, 1, 24, 1.0, None)
 
 
-def test_sass_is_blackwell_native():
-    """the GEMM/attention kernels really are tcgen05 + TMA (B200_PROFILING.md SASS table)"""
+def test_sass_is_hopper_native():
+    """the GEMM/attention kernels really are wgmma + TMA (HGMMA / UTMALDG in the sm_90a SASS), no mma.sync path"""
     import shutil
     import subprocess
 
@@ -67,8 +67,8 @@ def test_sass_is_blackwell_native():
     if shutil.which("cuobjdump") is None:
         pytest.skip("cuobjdump not available")
     sass = subprocess.run(["cuobjdump", "-sass", _lib.LIB_PATH], capture_output=True, text=True).stdout
-    assert "UTCHMMA" in sass and "UTMALDG" in sass and "LDTM" in sass
-    assert "HMMA." not in sass.replace("UTCHMMA", ""), "legacy mma.sync path found"
+    assert "HGMMA" in sass and "UTMALDG" in sass
+    assert "HMMA." not in sass, "legacy mma.sync path found"
 
 
 def test_data_feed_library_exports_every_symbol_of_its_header():

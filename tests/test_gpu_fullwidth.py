@@ -1,4 +1,4 @@
-"""Full-WIDTH parity of the hot path against the CPU fp32 oracle: the three benchmark shapes of BASELINE.json at their real
+"""Full-WIDTH parity of the hot path against the CPU fp32 oracle: the three benchmark shapes of bench.py at their real
 hidden sizes / vocabularies / sequence lengths with a reduced depth (the oracle finishes in tens of seconds):
 
   C2 shape  2 x GPTDolomite block 2560d / 32 heads hd 80 / F 10240 / V 49152 (biases), 2 x 4096 packed tokens, ragged docs

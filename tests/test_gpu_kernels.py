@@ -1,5 +1,5 @@
 """GPU parity tests: every CUDA kernel, called through the C ABI, against the CPU oracle on seeded inputs; plus
-size-independent properties at BASELINE.json's full sizes (C2: T=8192, H=2560, F=10240, V=49152, S=4096, hd=80)."""
+size-independent properties at the benchmark's full sizes (C2: T=8192, H=2560, F=10240, V=49152, S=4096, hd=80)."""
 
 import math
 
@@ -129,7 +129,7 @@ def test_gemm_vs_oracle(M, N, Kd, a_mn, b_mn):
     ref = O.linear(A.float(), B.float(), bias.float(), bf16=True)
     a = (A.t().contiguous() if a_mn else A).cuda()
     b = (B.t().contiguous() if b_mn else B).cuda()
-    # bit0: TMA-store epilogue; bit2 / bit3: force / forbid the CTA-pair (cta_group::2) kernel
+    # bit0: bf16 D without C; bit2 / bit3: CTA-pair flags (accepted, no effect on sm_90)
     for flags in (0, 1, 4, 5, 8, 9):
         out = K().gemm(a, b, a_mn=a_mn, b_mn=b_mn, bias=bias.cuda(), flags=flags)
         # fp32 accumulation order differs from the CPU: allow one bf16 ulp of the result magnitude
@@ -148,9 +148,8 @@ def test_gemm_epilogue_alpha_beta_accumulate():
 
 
 def test_gemm_tile_schedules_are_bit_identical():
-    """`gemm_dynamic` = 1 (one cluster per tile, running clusters take over pending ones through cluster launch control) and
-    = 0 (static persistent workers) compute the same tiles with the same arithmetic: outputs are bit-identical for every
-    operand layout / epilogue, in the CTA-pair and the single-CTA kernel, with many more tiles than SMs"""
+    """the `gemm_dynamic` option (a tile-scheduling choice of other GPU generations, accepted on sm_90) never changes the
+    arithmetic: outputs are bit-identical for every operand layout / epilogue flag, with many more tiles than SMs"""
     g = torch.Generator().manual_seed(12)
     default = K().get_option("gemm_dynamic")
     cases = [(4096, 4096, 512, False, False, 5, torch.bfloat16), (1024, 3072, 1024, False, True, 5, torch.bfloat16),
@@ -180,7 +179,7 @@ def test_gemm_split_k_accumulate(M, N, Kd):
     A, B = bf(torch.randn(Kd, M, generator=g) * 0.1), bf(torch.randn(Kd, N, generator=g) * 0.1)
     C = torch.randn(M, N, generator=g)
     default = K().get_option("gemm_dynamic")
-    for dyn in (0, 1):  # static persistent schedule / cluster-launch-control schedule
+    for dyn in (0, 1):  # both values of the scheduling option
         try:
             K().set_option("gemm_dynamic", dyn)
             d = C.cuda().clone()

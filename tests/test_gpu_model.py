@@ -251,6 +251,46 @@ def test_train_steps_reduce_loss_and_match_cpu_adamw(opt_name):
         assert abs(a - b) / b < 2e-3, (losses, ref_losses)
 
 
+def test_training_steps_are_bit_identical_from_run_to_run():
+    """the same model, batch and optimizer run twice give bit-identical losses, gradients and parameters: every reduction
+    of the step (attention dQ over key tiles, bias / embedding / norm gradients, the gradient norm) sums in a fixed
+    order.  Sequences of 512 tokens give the attention backward several key tiles per query tile, tied embeddings with
+    repeated token ids give the embedding gradient several rows to sum."""
+    from dolomite_engine_b200.distributed import ShardedDataParallel
+    from dolomite_engine_b200.model_wrapper import ModelWrapperForPretraining
+    from dolomite_engine_b200.optimization import get_optimizer
+    from dolomite_engine_b200.train_utils import train_step
+
+    kw = GPU_CONFIGS["hd80_bias"]
+    ocfg = O.OracleConfig(**kw)
+    params = oracle_params(ocfg)
+    tokens = torch.from_numpy(sample_tokens(ocfg, mbs=4, seq=512) % 97)  # few distinct ids: many repeats
+
+    def run():
+        w = ModelWrapperForPretraining(pretrained_config=gpu_config(kw).to_dict(), micro_batch_size=4, sequence_length=512)
+        w.model.load_state_dict(params)
+        sdp = ShardedDataParallel(w)
+        opt = get_optimizer("DolomiteFusedAdamW", {"lr": 1e-3, "weight_decay": 0.1, "betas": [0.9, 0.95], "eps": 1e-10}, sdp)
+
+        def batches():
+            while True:
+                yield {"text": tokens}
+
+        dl = batches()
+        losses = [train_step(sdp, opt, None, train_dataloader=dl, gradient_accumulation_steps=1, gradient_clipping=1.0)
+                  for _ in range(3)]
+        torch.cuda.synchronize()
+        units = w.model.engine.units
+        return losses, [u.master.detach().clone() for u in units], [u.master.grad.clone() for u in units]
+
+    (l1, p1, g1), (l2, p2, g2) = run(), run()
+    assert l1 == l2
+    for a, b in zip(g1, g2):
+        assert torch.equal(a, b)
+    for a, b in zip(p1, p2):
+        assert torch.equal(a, b)
+
+
 @pytest.mark.parametrize("every", [1, 2])
 def test_block_activation_checkpointing_gives_identical_gradients(every):
     """gradient_checkpointing/block.py:13-37: blocks 0, k, 2k, ... are re-run in backward; the recomputation launches the

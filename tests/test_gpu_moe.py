@@ -1,4 +1,4 @@
-"""GPU parity of the MoE path (router, dispatch plan, grouped tcgen05 GEMMs, combine) against the oracle's eager
+"""GPU parity of the MoE path (router, dispatch plan, grouped wgmma GEMMs, combine) against the oracle's eager
 SparseMoE restatement and the reference-derived golden layer (tests/golden/moe_layer.npz).
 Tolerances follow tests/hf_models/single_gpu/hf_models/scattermoe_test.py:38-48 (bf16: atol 2e-3 on logits)."""
 
@@ -137,7 +137,7 @@ def _moe_cfgs():
 
 @pytest.mark.parametrize("T,H,N,E,k", [(1000, 256, 512, 8, 2), (4096, 2048, 1024, 8, 2), (37, 64, 264, 16, 4)])
 def test_gather_on_load_equals_gather_then_gemm(T, H, N, E, k):
-    """grouped expert GEMM with the token gather fused into its operand load (TMA gather4) == gather kernel + grouped GEMM,
+    """grouped expert GEMM with the token gather fused into its operand load (rows copied by the producer warp) == gather kernel + grouped GEMM,
     bit for bit on every real row; CTA-pair and single-CTA grids (the reference: scattermoe parallel_linear, moe/scatter.py:38-49)"""
     g = torch.Generator(device="cuda").manual_seed(5)
     x = bf(torch.randn(T, H, device="cuda", generator=g))

@@ -500,7 +500,7 @@ def test_lazy_gradient_clearing_bookkeeping(monkeypatch):
 
 
 def test_lm_head_chunking_covers_the_token_rows_within_the_budget():
-    """engine._head_chunk_rows: the LM head + cross entropy run chunk by chunk so that [T, V] logits never exist (DESIGN 11.3).
+    """engine._head_chunk_rows: the LM head + cross entropy run chunk by chunk so that [T, V] logits never exist (DESIGN 8.1).
     Properties: chunks of `rows` rows cover T with no remainder beyond the last chunk, every chunk but the last has a multiple of 8
     rows (it is the contraction length of the head's weight-gradient GEMM), a chunk's bf16 logits stay within the budget
     (except the 8-row minimum), and the split is as even as the 8-row granularity allows."""

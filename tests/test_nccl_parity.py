@@ -4,7 +4,7 @@ distributed/__init__.py:126-230 wrapping, train_utils.py:18-116 accumulation und
 Each case launches `tools/ddp_parity.py` with `torch.distributed.run` on the GPUs of this box: every rank feeds its own
 micro-batches to the sharded model while rank 0 also runs an unsharded copy over all of them; mean loss, every rank-0
 gradient shard (reduce-scatter AVG) and the parameters the next all-gather delivers must agree for four optimizer steps.
-Skipped on boxes with fewer GPUs than the case needs (the single-GPU test box of the driver)."""
+Skipped on machines with fewer GPUs than the case needs."""
 
 import os
 import subprocess

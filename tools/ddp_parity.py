@@ -102,8 +102,8 @@ def main():
             gtol = (2e-2 if comm_dtype == torch.bfloat16 else 1e-5) if step == 0 else 5e-2
             if moe and step > 0:
                 # the two trajectories drift apart (wire rounding, sign-like first Adam steps) and a router logit near a tie then
-                # selects another expert in one of them: a flip rate f moves the gradients by ~sqrt(2 f) (DESIGN 11.1; measured
-                # 1e-2 .. 7e-2 over steps 1-3, call 95).  Step 0 -- identical parameters -- keeps the strict bound.
+                # selects another expert in one of them: a flip rate f moves the gradients by ~sqrt(2 f) (DESIGN 8.4).
+                # Step 0 -- identical parameters -- keeps the strict bound.
                 gtol = 1.5e-1
             ptol = 1e-6 if step == 0 else 2e-2
             good = dl < 1e-3 and worst < gtol and pworst < ptol
