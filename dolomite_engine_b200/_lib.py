@@ -66,6 +66,16 @@ SIGNATURES: dict[str, tuple] = {
         [_P, _L, _I, _P, _L, _I, _P, _L, _I, _P, _L, _F, _F, _P, _L, _L, _L, _I, _P],
     ),
     "dolomite_b200_gemm_bf16_wgrad_multi": (_I, [_I, _P, _P, _P, _P, _P, _P, _P, _P, _L, _P, _P, _P]),
+    "dolomite_b200_gemm_fp8": (
+        _I,
+        [_P, _L, _I, _P, _L, _I, _P, _P, _P, _L, _I, _P, _L, _F, _F, _P, _L, _L, _L, _I, _P],
+    ),
+    "dolomite_b200_gemm_fp8_wgrad_multi": (
+        _I,
+        [_I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _L, _P, _P, _I, _I, _I, _P],
+    ),
+    "dolomite_b200_fp8_cast": (_I, [_P, _L, _L, _L, _I, _P, _P, _P, _P, _P]),
+    "dolomite_b200_fp8_scaling_update": (_I, [_P, _I, _L, _P, _P, _F, _P]),
     "dolomite_b200_gemm_bf16_grouped_m": (_I, [_P, _L, _P, _L, _I, _P, _L, _F, _L, _L, _L, _P, _I, _I, _P]),
     "dolomite_b200_gemm_bf16_grouped_k": (_I, [_P, _L, _P, _L, _P, _L, _F, _F, _L, _L, _L, _P, _I, _P]),
     "dolomite_b200_moe_max_rows": (_L, [_L, _I, _I]),

@@ -200,9 +200,17 @@ def _(a) -> None:
 
 @_rule("MixedPrecisionArgs")
 def _(a) -> None:
-    a.dtype = {"bfloat16": "bf16", "float32": "fp32", "float16": "fp16"}.get(a.dtype, a.dtype)
-    if a.fp8_backend is not None or a.dtype == "fp8":
-        raise NotImplementedError("FP8 backends are out of scope of the B200 hot path (bf16 target)")
+    a.dtype = {"bfloat16": "bf16", "float32": "fp32", "float16": "fp16", "float8": "fp8"}.get(a.dtype, a.dtype)
+    if a.fp8_backend is not None:
+        # arguments.py:278-280 of the reference
+        assert a.dtype == "fp8", "fp8_backend can only be used with fp8 dtype"
+        a.fp8_backend = str(getattr(a.fp8_backend, "value", a.fp8_backend))
+        if a.fp8_backend == "msamp":
+            raise NotImplementedError("fp8_backend msamp is not implemented; use nvte (TransformerEngine delayed scaling)")
+        if a.fp8_backend != "nvte":
+            raise ValueError(f"unexpected fp8_backend ({a.fp8_backend})")
+    elif a.dtype == "fp8":
+        raise ValueError("dtype fp8 needs an fp8_backend (nvte)")
 
 
 _OUT_OF_SCOPE_FLAGS = ("cpu_offload", "zero_quantized_weights", "zero_quantized_gradients", "torch_compile",
@@ -242,8 +250,9 @@ def _(a) -> None:
 def _(a) -> None:
     _need(a, "model_args", "tuning_args", "save_args")
     assert a.datasets, "datasets cannot be None"
-    if a.mixed_precision_args.dtype != "bf16":
-        raise NotImplementedError("the B200 path trains in bf16 mixed precision (mixed_precision_args.dtype: bf16)")
+    if a.mixed_precision_args.dtype not in ("bf16", "fp8"):
+        raise NotImplementedError("the B200 path trains in bf16 mixed precision, optionally with FP8 linears "
+                                  "(mixed_precision_args.dtype: bf16 | fp8)")
 
 
 @_rule("InferenceArgs")

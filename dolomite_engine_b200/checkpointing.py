@@ -42,6 +42,9 @@ def _rank_world() -> tuple[int, int]:
     return 0, 1
 
 
+FP8_RECIPE_FILE = "fp8_recipe.pt"  # delayed-scaling state of the FP8 linears (fp8.Fp8Recipe), written by rank 0
+
+
 def _engine(model):
     return model.engine if hasattr(model, "engine") else model.model.engine
 
@@ -141,6 +144,8 @@ def save_checkpoint(args, model, optimizer, lr_scheduler, train_dataloader, expe
     eng = _engine(model)
     if getattr(eng, "has_dropout", False):  # counter-based dropout masks: (seed, passes so far) is the whole generator state
         rng["dolomite_b200_dropout_state"] = (eng.dropout_seed, eng._dropout_passes)
+    if rank == 0 and getattr(eng, "fp8", None) is not None:  # identical on every rank (amaxes are all-reduced)
+        torch.save(eng.fp8.state_dict(), os.path.join(save_path, FP8_RECIPE_FILE))
     os.makedirs(os.path.join(save_path, "rng_state"), exist_ok=True)
     torch.save(rng, os.path.join(save_path, "rng_state", f"rng_state-{rank}.pt"))
     if train_dataloader is not None:
@@ -249,6 +254,9 @@ def load_checkpoint_for_training(args, model, optimizer, lr_scheduler, train_dat
         lr_scheduler.load_state_dict(torch.load(os.path.join(load_path, "lr_scheduler.pt"), weights_only=False))
     elif getattr(la, "resume_learning_rate", True) and lr_scheduler is not None and optimizer is not None:
         resume_learning_rate(args, optimizer, lr_scheduler, iteration)
+    fp8_state = os.path.join(load_path, FP8_RECIPE_FILE)
+    if getattr(_engine(model), "fp8", None) is not None and os.path.exists(fp8_state):
+        _engine(model).fp8.load_state_dict(torch.load(fp8_state, map_location="cpu"))
     if getattr(la, "load_rng_state", True):
         p = os.path.join(load_path, "rng_state", f"rng_state-{rank}.pt")
         if os.path.exists(p):

@@ -146,6 +146,7 @@ int dolo_make_tmap(CUtensorMap* out, const void* base, int elem_bytes, int rank,
     DOLO_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0, "tensor map base %p not 16-byte aligned", base);
     CUtensorMapDataType dt;
     switch (elem_bytes) {
+        case 1: dt = CU_TENSOR_MAP_DATA_TYPE_UINT8; break;  // fp8 operands (the MMA reads the bits, TMA only moves bytes)
         case 2: dt = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16; break;
         case 4: dt = CU_TENSOR_MAP_DATA_TYPE_FLOAT32; break;
         default: return dolo_set_error("unsupported TMA element size %d", elem_bytes);

@@ -46,7 +46,7 @@ int dolo_option_attn_head_fastest();
 int dolo_option_gemm_l2_hints();  // 1 (default) = evict-first / evict-last operand loads for long-contraction GEMMs
 
 // TMA descriptor encode through the driver entry point (no link-time libcuda dependency).
-// rank-2 / rank-3 bf16/f32 tiled maps.  dims/strides innermost first; strides in BYTES for dims >= 1.
+// rank-2 / rank-3 fp8 (elem_bytes 1) / bf16 / f32 tiled maps.  dims/strides innermost first; strides in BYTES for dims >= 1.
 enum DoloSwizzle { DOLO_SW_NONE = 0, DOLO_SW_32 = 1, DOLO_SW_64 = 2, DOLO_SW_128 = 3 };
 int dolo_make_tmap(CUtensorMap* out, const void* base, int elem_bytes, int rank, const uint64_t* dims,
                    const uint64_t* strides_bytes, const uint32_t* box, DoloSwizzle sw);

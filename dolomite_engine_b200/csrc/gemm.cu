@@ -364,6 +364,194 @@ int launch_gemm(const GemmMaps& maps, const GemmParams& p, cudaStream_t st) {
     return DOLO_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// FP8 GEMM (TransformerEngine te.Linear under fp8_autocast): the same persistent schedule, stage ring and epilogue as the
+// bf16 kernel, with a k-block of 128 fp8 elements (still one 128-byte swizzle span, so a stage is still 32 KB).  fp8 wgmma
+// takes K-major operands only: A [M, K] and B [N, K] are both row-major, the transposes come from the cast kernel.
+//   D = alpha * (scale_inv_a * scale_inv_b * acc + bias) + beta * C
+// SPLIT: the wgmma accumulator is promoted into a second fp32 register set once per k-block (TE's "split accumulator",
+// used for dgrad / wgrad); otherwise the MMA accumulates over the whole contraction (fprop, TE's fast accumulation).
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int BK8 = 128;  // 128 fp8 = 128 bytes = one swizzle span
+static_assert(BM * BK8 == A_STAGE_BYTES && BN * BK8 == B_STAGE_BYTES, "fp8 stage must match the bf16 stage size");
+
+struct Fp8Scales {
+    const float* a[MAXP];  // scale_inv of A (device scalar)
+    const float* b[MAXP];
+};
+
+template <int FA, int FB, bool SPLIT>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+    gemm_fp8_kernel(const __grid_constant__ GemmMaps maps, const __grid_constant__ GemmParams p,
+                    const __grid_constant__ Fp8Scales sc) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_align_1024(smem_raw);
+    uint8_t* smem_a = smem;
+    uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
+    uint64_t* full_bar = bars;
+    uint64_t* empty_bar = bars + STAGES;
+
+    const int wg = threadIdx.x >> 7;
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const int num_tiles = p.num_tiles;
+
+    if (threadIdx.x == 0) {
+        for (int q = 0; q < p.n_prob; ++q) {
+            tma_prefetch_desc(&maps.a[q]);
+            tma_prefetch_desc(&maps.b[q]);
+        }
+        for (int i = 0; i < STAGES; ++i) {
+            mbar_init(&full_bar[i], 1);
+            mbar_init(&empty_bar[i], 8);
+        }
+        mbar_fence_init();
+    }
+    __syncthreads();
+
+    if (wg == 0) {
+        if (warp == 0 && elect_one()) {
+            int stage = 0;
+            uint32_t phase = 0;
+            for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+                const TileInfo ti = tile_info(t, p);
+                for (int kb = ti.kb0; kb < ti.kb1; ++kb) {
+                    mbar_wait(&empty_bar[stage], phase ^ 1, 1);
+                    mbar_expect_tx(&full_bar[stage], STAGE_BYTES);
+                    tma_load_2d(smem_a + stage * A_STAGE_BYTES, &maps.a[ti.q], &full_bar[stage], kb * BK8, ti.m_blk * BM);
+                    tma_load_2d(smem_b + stage * B_STAGE_BYTES, &maps.b[ti.q], &full_bar[stage], kb * BK8, ti.n_blk * BN);
+                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+                }
+            }
+        }
+        return;
+    }
+
+    const int cw = wg - 1;
+    const int wr = (warp & 3) * 16 + (lane >> 2);
+    const int wc = 2 * (lane & 3);
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[BN / 2];
+    float tot[SPLIT ? BN / 2 : 1];
+    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+        const TileInfo ti = tile_info(t, p);
+        const Problem& pr = p.pr[ti.q];
+        const int64_t row0 = int64_t(ti.m_blk) * BM + cw * 64 + wr;
+        const int col0 = ti.n_blk * BN + wc;
+        int prev_stage = -1;
+        for (int kb = ti.kb0; kb < ti.kb1; ++kb) {
+            mbar_wait(&full_bar[stage], phase, 3);
+            wgmma_fence();
+            const uint32_t sa = smem_u32(smem_a + stage * A_STAGE_BYTES);
+            const uint32_t sb = smem_u32(smem_b + stage * B_STAGE_BYTES);
+#pragma unroll
+            for (int k = 0; k < BK8 / 32; ++k) {
+                // K-major, +32 B per K=32 step inside the swizzle span (the byte layout of the bf16 K=16 step)
+                const uint64_t adesc = gmma_desc(sa + cw * (64 * 128) + k * 32, 16, 1024, 1);
+                const uint64_t bdesc = gmma_desc(sb + k * 32, 16, 1024, 1);
+                const bool acc_on = SPLIT ? k != 0 : (kb != ti.kb0 || k != 0);
+                wgmma_fp8_n128<FA, FB>(acc, adesc, bdesc, acc_on ? 1u : 0u);
+            }
+            wgmma_commit();
+            if constexpr (SPLIT) {
+                wgmma_wait<0>();
+                reg_fence<BN / 2>(acc);
+                if (lane == 0) mbar_arrive(&empty_bar[stage]);
+                if (kb == ti.kb0) {
+#pragma unroll
+                    for (int i = 0; i < BN / 2; ++i) tot[i] = acc[i];
+                } else {
+#pragma unroll
+                    for (int i = 0; i < BN / 2; ++i) tot[i] += acc[i];
+                }
+            } else {
+                wgmma_wait<1>();
+                if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+                prev_stage = stage;
+            }
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+        if constexpr (!SPLIT) {
+            wgmma_wait<0>();
+            reg_fence<BN / 2>(acc);
+            if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+        }
+        const float* res = SPLIT ? tot : acc;
+
+        const float s = __ldg(sc.a[ti.q]) * __ldg(sc.b[ti.q]);
+        const float alpha = pr.alpha, beta = pr.beta;
+        const __nv_bfloat16* bias = pr.bias;
+        const int N = pr.N;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+            const int col = col0 + 8 * j;
+            if (col >= N) continue;
+            float b0 = 0.f, b1 = 0.f;
+            if (bias != nullptr) {
+                const uint32_t bv = *reinterpret_cast<const uint32_t*>(bias + col);
+                b0 = bf16_lo(bv);
+                b1 = bf16_hi(bv);
+            }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int64_t row = row0 + 8 * h;
+                if (row >= pr.M) continue;
+                float v0 = (s * res[4 * j + 2 * h] + b0) * alpha;
+                float v1 = (s * res[4 * j + 2 * h + 1] + b1) * alpha;
+                if (p.d_is_f32) {
+                    float* d = static_cast<float*>(pr.D) + row * pr.ldd + col;
+                    if (pr.C) {
+                        const float2 c2 = *reinterpret_cast<const float2*>(static_cast<const float*>(pr.C) + row * pr.ldc + col);
+                        v0 += beta * c2.x;
+                        v1 += beta * c2.y;
+                    }
+                    *reinterpret_cast<float2*>(d) = make_float2(v0, v1);
+                } else {
+                    __nv_bfloat16* d = static_cast<__nv_bfloat16*>(pr.D) + row * pr.ldd + col;
+                    if (pr.C) {
+                        const uint32_t cv =
+                            *reinterpret_cast<const uint32_t*>(static_cast<const __nv_bfloat16*>(pr.C) + row * pr.ldc + col);
+                        v0 += beta * bf16_lo(cv);
+                        v1 += beta * bf16_hi(cv);
+                    }
+                    *reinterpret_cast<uint32_t*>(d) = pack_bf16(v0, v1);
+                }
+            }
+        }
+    }
+}
+
+template <int FA, int FB, bool SPLIT>
+int launch_gemm_fp8(const GemmMaps& maps, const GemmParams& p, const Fp8Scales& sc, cudaStream_t st) {
+    auto kern = gemm_fp8_kernel<FA, FB, SPLIT>;
+    static bool attr_set = false;
+    if (!attr_set) {
+        DOLO_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+        attr_set = true;
+    }
+    int sms = dolo_num_sms() - dolo_option_gemm_sm_margin();
+    if (sms < 1) sms = 1;
+    const int grid = p.num_tiles < sms ? p.num_tiles : sms;
+    kern<<<grid, GEMM_THREADS, SMEM_BYTES, st>>>(maps, p, sc);
+    DOLO_LAUNCH_OK("gemm_fp8");
+    return DOLO_OK;
+}
+
+template <int FA, int FB>
+int dispatch_fp8_split(int split, const GemmMaps& maps, const GemmParams& p, const Fp8Scales& sc, cudaStream_t st) {
+    return split ? launch_gemm_fp8<FA, FB, true>(maps, p, sc, st) : launch_gemm_fp8<FA, FB, false>(maps, p, sc, st);
+}
+
+int dispatch_fp8(int a_fmt, int b_fmt, int split, const GemmMaps& maps, const GemmParams& p, const Fp8Scales& sc,
+                 cudaStream_t st) {
+    if (a_fmt == 0 && b_fmt == 0) return dispatch_fp8_split<0, 0>(split, maps, p, sc, st);
+    if (a_fmt == 0 && b_fmt == 1) return dispatch_fp8_split<0, 1>(split, maps, p, sc, st);
+    if (a_fmt == 1 && b_fmt == 0) return dispatch_fp8_split<1, 0>(split, maps, p, sc, st);
+    return dispatch_fp8_split<1, 1>(split, maps, p, sc, st);
+}
+
 }  // namespace
 
 struct GroupArgs {
@@ -610,4 +798,107 @@ extern "C" int dolomite_b200_gemm_bf16_grouped_k(const void* A, int64_t lda, con
     // A, B are both MN-major views of [K_max, M] / [K_max, N] row-major activations; D[g] (+)= A_g^T B_g in fp32
     return gemm_impl(A, lda, 1, B, ldb, 1, D, ldd, 1, beta != 0.f ? D : nullptr, ldd, alpha, beta, nullptr, M, N, K_max, 0,
                      stream, ga);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// FP8 entry points (te.Linear fprop / dgrad / wgrad under fp8_autocast)
+// ---------------------------------------------------------------------------------------------------------------------
+static int setup_problem_fp8(GemmMaps& maps, GemmParams& p, Fp8Scales& sc, int q, const GemmProblemArgs& g,
+                             const float* a_scale_inv, const float* b_scale_inv, int d_is_f32) {
+    const int64_t M = g.M, N = g.N, K = g.K;
+    DOLO_REQUIRE(M > 0 && N > 0 && K > 0, "gemm_fp8: empty problem (M=%lld N=%lld K=%lld)", (long long)M, (long long)N,
+                 (long long)K);
+    DOLO_REQUIRE(K % 16 == 0 && N % 16 == 0, "gemm_fp8: K=%lld and N=%lld must be multiples of 16", (long long)K,
+                 (long long)N);
+    DOLO_REQUIRE(g.lda % 16 == 0 && g.ldb % 16 == 0 && g.lda >= K && g.ldb >= K,
+                 "gemm_fp8: lda / ldb must be >= K and multiples of 16 (16-byte aligned fp8 rows)");
+    DOLO_REQUIRE(g.ldd % (d_is_f32 ? 4 : 8) == 0 && g.ldd >= N && (g.C == nullptr || g.ldc % (d_is_f32 ? 4 : 8) == 0),
+                 "gemm_fp8: ldd / ldc must keep 16-byte alignment");
+    const uintptr_t ptr_bits = reinterpret_cast<uintptr_t>(g.A) | reinterpret_cast<uintptr_t>(g.B) |
+                               reinterpret_cast<uintptr_t>(g.D) | reinterpret_cast<uintptr_t>(g.C);
+    DOLO_REQUIRE((ptr_bits & 15) == 0 && (reinterpret_cast<uintptr_t>(g.bias) & 3) == 0,
+                 "gemm_fp8: A, B, D and C must be 16-byte aligned");
+    DOLO_REQUIRE(a_scale_inv != nullptr && b_scale_inv != nullptr, "gemm_fp8: missing scale_inv pointer");
+    DOLO_REQUIRE(M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31), "gemm_fp8: dimension too large");
+    uint64_t dims[2] = {uint64_t(K), uint64_t(M)};
+    uint64_t strides[2] = {1, uint64_t(g.lda)};
+    uint32_t box[2] = {BK8, BM};
+    int rc = dolo_make_tmap(&maps.a[q], g.A, 1, 2, dims, strides, box, DOLO_SW_128);
+    if (rc) return rc;
+    dims[1] = uint64_t(N);
+    strides[1] = uint64_t(g.ldb);
+    box[1] = BN;
+    rc = dolo_make_tmap(&maps.b[q], g.B, 1, 2, dims, strides, box, DOLO_SW_128);
+    if (rc) return rc;
+    sc.a[q] = a_scale_inv;
+    sc.b[q] = b_scale_inv;
+    Problem& pr = p.pr[q];
+    pr.D = g.D;
+    pr.C = g.C;
+    pr.bias = static_cast<const __nv_bfloat16*>(g.bias);
+    pr.ldd = g.ldd;
+    pr.ldc = g.ldc;
+    pr.M = int(M);
+    pr.N = int(N);
+    pr.alpha = g.alpha;
+    pr.beta = g.C ? g.beta : 0.f;
+    pr.hint_a = pr.hint_b = TMA_HINT_NORMAL;
+    pr.num_m = int((M + BM - 1) / BM);
+    pr.num_n = int((N + BN - 1) / BN);
+    pr.num_kb = int((K + BK8 - 1) / BK8);
+    int64_t gm = (12ll << 20) / (int64_t(BM) * K);  // A panel of ~12 MB of the 50 MB L2, as for bf16
+    pr.group_m = int(gm < 4 ? 4 : (gm > 64 ? 64 : gm));
+    return DOLO_OK;
+}
+
+extern "C" int dolomite_b200_gemm_fp8(const void* A, int64_t lda, int a_fmt, const void* B, int64_t ldb, int b_fmt,
+                                      const float* a_scale_inv, const float* b_scale_inv, void* D, int64_t ldd,
+                                      int d_is_f32, const void* C, int64_t ldc, float alpha, float beta, const void* bias,
+                                      int64_t M, int64_t N, int64_t K, int split_accumulate, void* stream) {
+    DOLO_REQUIRE(M >= 0 && N >= 0 && K >= 0, "gemm_fp8: negative dimension");
+    DOLO_REQUIRE((a_fmt == 0 || a_fmt == 1) && (b_fmt == 0 || b_fmt == 1), "gemm_fp8: format must be 0 (e4m3) or 1 (e5m2)");
+    if (M == 0 || N == 0) return DOLO_OK;
+    GemmMaps maps;
+    GemmParams p;
+    Fp8Scales sc;
+    memset(&p, 0, sizeof(p));
+    memset(&sc, 0, sizeof(sc));
+    GemmProblemArgs g{A, lda, B, ldb, D, ldd, C, ldc, bias, alpha, beta, M, N, K};
+    int rc = setup_problem_fp8(maps, p, sc, 0, g, a_scale_inv, b_scale_inv, d_is_f32);
+    if (rc) return rc;
+    p.n_prob = 1;
+    p.num_tiles = p.pr[0].num_m * p.pr[0].num_n;
+    p.d_is_f32 = d_is_f32;
+    p.num_groups = 1;
+    return dispatch_fp8(a_fmt, b_fmt, split_accumulate, maps, p, sc, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int dolomite_b200_gemm_fp8_wgrad_multi(int n_problems, const void* const* dYt, const int64_t* ld_dyt,
+                                                  const void* const* Xt, const int64_t* ld_xt,
+                                                  const float* const* dy_scale_inv, const float* const* x_scale_inv,
+                                                  float* const* dW, const int64_t* ld_dw, const int64_t* M,
+                                                  const int64_t* N, int64_t K, const float* alpha, const int* accumulate,
+                                                  int dy_fmt, int x_fmt, int split_accumulate, void* stream) {
+    DOLO_REQUIRE(n_problems >= 1 && n_problems <= MAXP, "gemm_fp8_wgrad_multi: between 1 and %d problems per launch", MAXP);
+    DOLO_REQUIRE((dy_fmt == 0 || dy_fmt == 1) && (x_fmt == 0 || x_fmt == 1),
+                 "gemm_fp8_wgrad_multi: format must be 0 (e4m3) or 1 (e5m2)");
+    GemmMaps maps;
+    GemmParams p;
+    Fp8Scales sc;
+    memset(&p, 0, sizeof(p));
+    memset(&sc, 0, sizeof(sc));
+    int tiles = 0;
+    for (int q = 0; q < n_problems; ++q) {
+        GemmProblemArgs g{dYt[q], ld_dyt[q], Xt[q], ld_xt[q], dW[q], ld_dw[q], accumulate[q] ? dW[q] : nullptr, ld_dw[q],
+                          nullptr, alpha[q], 1.f, M[q], N[q], K};
+        int rc = setup_problem_fp8(maps, p, sc, q, g, dy_scale_inv[q], x_scale_inv[q], 1);
+        if (rc) return rc;
+        p.pr[q].tile_start = tiles;
+        tiles += p.pr[q].num_m * p.pr[q].num_n;
+    }
+    p.n_prob = n_problems;
+    p.num_tiles = tiles;
+    p.d_is_f32 = 1;
+    p.num_groups = 1;
+    return dispatch_fp8(dy_fmt, x_fmt, split_accumulate, maps, p, sc, static_cast<cudaStream_t>(stream));
 }

@@ -1,4 +1,4 @@
-// wgmma (sm_90a warpgroup MMA) wrappers: bf16 x bf16 -> fp32, M = 64 rows per warpgroup.
+// wgmma (sm_90a warpgroup MMA) wrappers: bf16 x bf16 -> fp32 and fp8 x fp8 -> fp32, M = 64 rows per warpgroup.
 //
 //   wgmma_ss<N, TA, TB>(d, a_desc, b_desc, scale_d)   A and B from shared memory (descriptors, see gmma_desc)
 //   wgmma_rs<N, TB>(d, a_regs, b_desc, scale_d)       A from registers (the m64k16 fragment of the accumulator layout)
@@ -59,6 +59,21 @@ __device__ __forceinline__ void wgmma_rs_n64(float* d, const uint32_t (&a)[4], u
                  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, %38;\n\t}\n"
                  : DOLO_F32(0) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d), "n"(TB));
 }
+
+// FP8 x FP8 -> fp32, m64n128k32, both operands K-major in shared memory (the only layout fp8 wgmma accepts).
+// FA / FB: 0 = e4m3, 1 = e5m2.  Same accumulator layout as the bf16 m64n128 form.
+#define DOLO_WGMMA_FP8_N128(TA, TB)                                                                                         \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\twgmma.mma_async.sync.aligned.m64n128k32.f32." TA "." TB " " \
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}\n" \
+                 : DOLO_F64(0) : "l"(da), "l"(db), "r"(scale_d))
+template <int FA, int FB>
+__device__ __forceinline__ void wgmma_fp8_n128(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+    if constexpr (FA == 0 && FB == 0) DOLO_WGMMA_FP8_N128("e4m3", "e4m3");
+    else if constexpr (FA == 0 && FB == 1) DOLO_WGMMA_FP8_N128("e4m3", "e5m2");
+    else if constexpr (FA == 1 && FB == 0) DOLO_WGMMA_FP8_N128("e5m2", "e4m3");
+    else DOLO_WGMMA_FP8_N128("e5m2", "e5m2");
+}
+#undef DOLO_WGMMA_FP8_N128
 
 // N-generic entry points (N must be one of the instantiated widths)
 template <int N, int TA, int TB>

@@ -277,12 +277,31 @@ class DolomiteEngine:
         self._fresh_grads: set[str] = set()  # weights whose gradient buffer will be overwritten by the next wgrad GEMM
         # DOLO_EAGER_GRAD_ZERO=1: zero_grad() clears every gradient buffer (A/B switch for the lazy clearing, `_lazy_zero`)
         self.lazy_grad_zero = os.environ.get("DOLO_EAGER_GRAD_ZERO", "0") != "1"
+        # FP8 linears (fp8.py): `fp8` holds the delayed-scaling state once enable_fp8() ran; `fp8_autocast` is switched on
+        # around the training forward (te.fp8_autocast); `_fp8_now` is the mode of the pass being run or backpropagated
+        self.fp8 = None
+        self.fp8_autocast = False
+        self._fp8_now = False
+        # fp8 copies of the weights named in `_fp8_keep` ((name, transposed) -> uint8 tensor), kept for the current pass: the
+        # scale is fixed for the step, so the LM head's chunk loop casts its [V, H] weight once, not once per chunk (other
+        # weights are cast once per pass anyway and are not kept, which would hold an fp8 copy of the whole model)
+        self._fp8_wcache: dict = {}
+        self._fp8_keep: set = set()
         if cfg.attention_multiplier is not None:
             self.softmax_scale = float(cfg.attention_multiplier)
         elif cfg.scale_attn_weights:
             self.softmax_scale = 1.0 / math.sqrt(self.hd)
         else:
             self.softmax_scale = 1.0
+
+    def enable_fp8(self) -> None:
+        """FP8 training of the linears fp8.fp8_weight_names(cfg) selects (mixed_precision_args dtype fp8, backend nvte)"""
+        from .fp8 import Fp8Recipe, fp8_weight_names
+
+        self.fp8 = Fp8Recipe(fp8_weight_names(self.cfg), self.device)
+
+    def _is_fp8(self, wname: str) -> bool:
+        return self._fp8_now and wname in self.fp8
 
     # ------------------------------------------------------------------------------------------
     def _ensure_rope(self, max_seqlen: int) -> None:
@@ -422,6 +441,35 @@ class DolomiteEngine:
     def _w(self, unit: FlatUnit, name: str):
         return unit.views.get(name)
 
+    def _linear(self, unit: FlatUnit, wname: str, x, bname: str | None = None, *, c=None, alpha: float = 1.0,
+                beta: float = 0.0, out=None, flags=None):
+        """y = alpha * (x W^T + b) + beta * c, in FP8 (te.Linear under fp8_autocast) when `wname` is an FP8 linear and the
+        pass runs under fp8_autocast, else in bf16"""
+        w = unit.views[wname]
+        bias = unit.views.get(bname) if bname is not None else None
+        if not self._is_fp8(wname):
+            return K.gemm(x, w, bias=bias, c=c, alpha=alpha, beta=beta, out=out, flags=flags)
+        xs, xsi, xam = self.fp8.input_slot(wname)
+        _, wsi, _ = self.fp8.weight_slot(wname)
+        xq, _ = K.fp8_cast(x, K.E4M3, xs, amax=xam)
+        wq = self._fp8_weight(wname, w, transposed=False)
+        # fprop: one accumulator over the whole contraction (TE's fast accumulation for the forward GEMM)
+        return K.gemm_fp8(xq, K.E4M3, xsi, wq, K.E4M3, wsi, bias=bias, c=c, alpha=alpha, beta=beta, out=out)
+
+    def _fp8_weight(self, wname: str, w, transposed: bool):
+        """e4m3 copy of weight `wname` (transposed: [in, out], the dgrad operand); kept for the pass if `_fp8_keep` names it"""
+        key = (wname, transposed)
+        q = self._fp8_wcache.get(key)
+        if q is None:
+            ws, _, wam = self.fp8.weight_slot(wname)
+            if transposed:  # backward: the forward already recorded this weight's amax
+                _, q = K.fp8_cast(w, K.E4M3, ws, plain=False, transpose=True)
+            else:
+                q, _ = K.fp8_cast(w, K.E4M3, ws, amax=wam)
+            if wname in self._fp8_keep:
+                self._fp8_wcache[key] = q
+        return q
+
     def _norm_fwd(self, x, unit: FlatUnit, prefix: str):
         """RMSNorm or LayerNorm (get_normalization_function, normalization/__init__.py:13-30) -> (y, saved statistics)"""
         eps = self.cfg.layer_norm_epsilon
@@ -467,7 +515,7 @@ class DolomiteEngine:
         p = f"transformer.h.{i}."
         m_res = 1.0 if cfg.m_residual is None else float(cfg.m_residual)
         ln1, rstd1 = self._norm_fwd(x_in, u, p + "ln_1.")
-        qkv = K.gemm(ln1, u.views[p + "attn.c_attn.weight"], bias=u.views.get(p + "attn.c_attn.bias"))
+        qkv = self._linear(u, p + "attn.c_attn.weight", ln1, p + "attn.c_attn.bias")
         if self.rope_cos is not None:
             K.rope_qk_inplace(qkv, self.n_groups, self.q_per_group, self.hd, self.rope_cos, self.rope_sin, position_ids)
         if self._kv_sink is not None:  # prefill of a KV cache: keys (rotated) and values of every prompt token
@@ -477,25 +525,23 @@ class DolomiteEngine:
                                       dropout_p=p_att, dropout_keys=self._drop_keys(4 * i + 3) if p_att > 0 else (0, 0))
         p_res = self._drop_p("resid_pdrop")
         if p_res > 0:  # resid_dropout sits between c_proj and `* m_residual` / `+ residual` (padding_free.py:75, layer.py:73-77)
-            y = K.gemm(attn, u.views[p + "attn.c_proj.weight"], bias=u.views.get(p + "attn.c_proj.bias"))
+            y = self._linear(u, p + "attn.c_proj.weight", attn, p + "attn.c_proj.bias")
             h_mid = K.dropout_fwd(y, p_res, self._drop_keys(4 * i + 1), residual=x_in, post_mul=m_res, out=y)
         else:
-            h_mid = K.gemm(attn, u.views[p + "attn.c_proj.weight"], bias=u.views.get(p + "attn.c_proj.bias"), c=x_in,
-                           alpha=m_res, beta=1.0)
+            h_mid = self._linear(u, p + "attn.c_proj.weight", attn, p + "attn.c_proj.bias", c=x_in, alpha=m_res, beta=1.0)
         ln2, rstd2 = self._norm_fwd(h_mid, u, p + "ln_2.")
         if self.is_moe:
             from . import moe
 
             h, moe_saved = moe.forward(self, u, p, ln2, h_mid, m_res, layer=i)
             return h, (x_in, rstd1, ln1, qkv, attn, lse, h_mid, rstd2, ln2, moe_saved)
-        fc = K.gemm(ln2, u.views[p + "mlp.c_fc.weight"], bias=u.views.get(p + "mlp.c_fc.bias"))
+        fc = self._linear(u, p + "mlp.c_fc.weight", ln2, p + "mlp.c_fc.bias")
         act = K.swiglu_fwd(fc) if self.is_glu else K.gelu_fwd(fc)
         if p_res > 0:  # gpt_dolomite/mlp.py:45-50 then layer.py:82-86
-            y = K.gemm(act, u.views[p + "mlp.c_proj.weight"], bias=u.views.get(p + "mlp.c_proj.bias"))
+            y = self._linear(u, p + "mlp.c_proj.weight", act, p + "mlp.c_proj.bias")
             h = K.dropout_fwd(y, p_res, self._drop_keys(4 * i + 2), residual=h_mid, post_mul=m_res, out=y)
         else:
-            h = K.gemm(act, u.views[p + "mlp.c_proj.weight"], bias=u.views.get(p + "mlp.c_proj.bias"), c=h_mid,
-                       alpha=m_res, beta=1.0)
+            h = self._linear(u, p + "mlp.c_proj.weight", act, p + "mlp.c_proj.bias", c=h_mid, alpha=m_res, beta=1.0)
         return h, (x_in, rstd1, ln1, qkv, attn, lse, h_mid, rstd2, ln2, fc, act)
 
     def forward(self, input_ids, position_ids, cu_seqlens, max_seqlen: int, labels=None, ignore_index: int = -100,
@@ -505,6 +551,8 @@ class DolomiteEngine:
         chunk-wise inside the loss computation and the [T, V] logits are never materialised."""
         cfg = self.cfg
         self._begin_dropout_pass()
+        self._fp8_now = self.fp8 is not None and self.fp8_autocast and self.training and save_for_backward
+        self._fp8_wcache.clear()
         T = input_ids.numel()
         root = self.units[0]
         comm = self.comm
@@ -550,17 +598,21 @@ class DolomiteEngine:
             scratch = K.cross_entropy_count(labels, ignore_index)
             loss_tok = torch.empty(T, dtype=torch.float32, device=hf.device)
             d_hf = torch.empty_like(hf)
-            rows = self._head_chunk_rows(T, head.shape[0], self.head_chunk_bytes)
+            # FP8 head: the chunk rows are the contraction of its weight-gradient GEMM, a multiple of 16
+            rows = self._head_chunk_rows(T, head.shape[0], self.head_chunk_bytes, 16 if self._is_fp8(head_name) else 8)
             buf = torch.empty(min(rows, T), head.shape[0], dtype=torch.bfloat16, device=hf.device)
+            self._fp8_keep = {head_name}
             for r0 in range(0, T, rows):
                 r1 = min(T, r0 + rows)
-                lg = K.gemm(hf[r0:r1], head, alpha=inv_width, out=buf[: r1 - r0])
+                lg = self._linear(root, head_name, hf[r0:r1], alpha=inv_width, out=buf[: r1 - r0])
                 K.cross_entropy_rows(lg, labels[r0:r1], loss_tok[r0:r1], scratch, ignore_index=ignore_index)
                 self._linear_bwd(root, head_name, None, hf[r0:r1], lg, alpha=inv_width, dx_out=d_hf[r0:r1])
             loss = K.cross_entropy_mean(loss_tok, scratch)
+            self._fp8_keep = set()
+            self._fp8_wcache.clear()
             del buf
         else:
-            logits = K.gemm(hf, head, alpha=inv_width)
+            logits = self._linear(root, head_name, hf, alpha=inv_width)
             if labels is not None:
                 # fused CE fwd+bwd: dlogits overwrites the logits
                 loss, _, dlogits = K.cross_entropy_fwd_bwd(logits, labels, ignore_index=ignore_index, dlogits=None)
@@ -569,17 +621,19 @@ class DolomiteEngine:
         if save_for_backward:
             self._saved = dict(input_ids=input_ids, position_ids=position_ids, cu_seqlens=cu_seqlens, max_seqlen=max_seqlen,
                                layers=saved_layers, h_last=h, rstd_f=rstd_f, hf=hf, dlogits=dlogits, d_hf=d_hf, T=T,
-                               dropout_seed=self._dropout_now)
+                               dropout_seed=self._dropout_now, fp8=self._fp8_now)
+        self._fp8_now = False
+        self._fp8_wcache.clear()
         return logits_out, loss
 
     @staticmethod
-    def _head_chunk_rows(T: int, V: int, budget_bytes: int = 1 << 30) -> int:
-        """token rows per LM-head chunk: equal chunks of at most `budget_bytes` of bf16 logits, multiples of 8 rows (the
-        rows of a chunk are the contraction length of its weight-gradient GEMM)"""
-        max_rows = max(8, budget_bytes // (2 * V) // 8 * 8)
+    def _head_chunk_rows(T: int, V: int, budget_bytes: int = 1 << 30, multiple: int = 8) -> int:
+        """token rows per LM-head chunk: equal chunks of at most `budget_bytes` of bf16 logits, multiples of `multiple`
+        rows (the rows of a chunk are the contraction length of its weight-gradient GEMM)"""
+        max_rows = max(multiple, budget_bytes // (2 * V) // multiple * multiple)
         n_chunks = -(-T // max_rows)
         per = -(-T // n_chunks)
-        return min(T, -(-per // 8) * 8)
+        return min(T, -(-per // multiple) * multiple)
 
     # ------------------------------------------------------------------------------------------
     # decoding with a KV cache (attention/sdpa.py:11-83, attention/flash.py:16-140 `past_key_values`)
@@ -666,6 +720,8 @@ class DolomiteEngine:
     def _linear_bwd(self, unit: FlatUnit, wname: str, bname: str | None, x, dy, alpha: float = 1.0, need_dx: bool = True,
                     dx_out=None):
         """autograd of y = alpha * (x W^T + b):  dx = alpha * dy W ; dW += alpha * dy^T x ; db += alpha * colsum(dy)"""
+        if self._is_fp8(wname):
+            return self._linear_bwd_fp8(unit, wname, bname, x, dy, alpha, need_dx, dx_out)
         w = unit.views[wname]
         gw = unit.gviews[wname]
         dx = K.gemm(dy, w, b_mn=True, alpha=alpha, out=dx_out) if need_dx else None
@@ -684,21 +740,72 @@ class DolomiteEngine:
             K.colsum_accum(dy, unit.gviews[bname], alpha)
         return dx
 
+    def _linear_bwd_fp8(self, unit: FlatUnit, wname: str, bname: str | None, x, dy, alpha: float = 1.0,
+                        need_dx: bool = True, dx_out=None, dx_add=None):
+        """te.Linear backward: dy is cast to e5m2 (plain for dgrad, transposed for wgrad); the weight and the input are
+        re-cast, transposed, from their bf16 copies with the scales of their forward (the update runs after the backward),
+        which gives the bits TE's saved fp8 copies hold.  dgrad / wgrad use the split accumulator, as TE does.
+        `dx_add`: dx += ... (fp8 form of the bf16 GEMM's c / beta accumulation)"""
+        if alpha != 1.0:
+            # te.Linear's output gradient is that of its own output, i.e. bf16(alpha * dy) for the `* m_residual` /
+            # `/ m_width` that follow it: cast (and record the amax of) that tensor, as TE does
+            dy = K.dropout_bwd(dy, 0.0, (0, 0), pre_mul=alpha)
+            alpha = 1.0
+        w = unit.views[wname] if need_dx else None
+        gw = unit.gviews[wname]
+        xs, xsi, _ = self.fp8.input_slot(wname)
+        _, wsi, _ = self.fp8.weight_slot(wname)
+        gs, gsi, gam = self.fp8.grad_slot(wname)
+        dyq, dyt = K.fp8_cast(dy, K.E5M2, gs, transpose=True, amax=gam)
+        dx = None
+        if need_dx:
+            wt = self._fp8_weight(wname, w, transposed=True)
+            if dx_add is not None:
+                dx = K.gemm_fp8(dyq, K.E5M2, gsi, wt, K.E4M3, wsi, alpha=alpha, out=dx_add, c=dx_add, beta=1.0,
+                                split_accumulate=True)
+            else:
+                dx = K.gemm_fp8(dyq, K.E5M2, gsi, wt, K.E4M3, wsi, alpha=alpha, out=dx_out, split_accumulate=True)
+            del wt
+        del dyq
+        _, xt = K.fp8_cast(x, K.E4M3, xs, plain=False, transpose=True)
+        fresh = self.take_fresh(wname)
+        wg = (dyt, gsi, xt, xsi, gw, alpha, not fresh)
+        if self._deferred_wgrads is not None:
+            self._deferred_wgrads.append(("fp8", wg))
+            if len(self._deferred_wgrads) == 4:
+                self._flush_wgrads()
+        else:
+            K.gemm_fp8_wgrad_multi([wg])
+        if bname is not None and bname in unit.gviews:
+            K.colsum_accum(dy, unit.gviews[bname], alpha)
+        return dx
+
     def _flush_wgrads(self) -> None:
         if not self._deferred_wgrads:
             return
+        # FP8 entries are ("fp8", (dyt, s_dy, xt, s_x, dw, alpha, accumulate)); a block mixing FP8 and bf16 linears (a width
+        # that is not a multiple of 16) gets one launch per kind
+        fp8 = [q[1] for q in self._deferred_wgrads if isinstance(q[0], str)]
+        bf16 = [q for q in self._deferred_wgrads if not isinstance(q[0], str)]
+
+        def launch():
+            if fp8:
+                K.gemm_fp8_wgrad_multi(fp8)
+            if bf16:
+                K.gemm_wgrad_multi(bf16)
+
         if self.overlap_wgrads and self.device.type == "cuda":
             if self._wgrad_stream is None:
                 self._wgrad_stream = torch.cuda.Stream(device=self.device)
             side, main = self._wgrad_stream, torch.cuda.current_stream()
-            side.wait_stream(main)  # every (dy, x) pair of the list has been produced on the main stream
+            side.wait_stream(main)  # every operand of the list has been produced on the main stream
             with torch.cuda.stream(side):
-                K.gemm_wgrad_multi(self._deferred_wgrads)
-            for dy, x, _, _, _ in self._deferred_wgrads:  # the allocator must not hand these blocks out before the launch has read them
-                dy.record_stream(side)
-                x.record_stream(side)
+                launch()
+            # the allocator must not hand these blocks out before the launch has read them
+            for t in [q[0] for q in bf16] + [q[1] for q in bf16] + [q[0] for q in fp8] + [q[2] for q in fp8]:
+                t.record_stream(side)
         else:
-            K.gemm_wgrad_multi(self._deferred_wgrads)
+            launch()
         self._deferred_wgrads.clear()
 
     def join_wgrad_stream(self, stream=None) -> None:
@@ -718,6 +825,8 @@ class DolomiteEngine:
         m_res = 1.0 if cfg.m_residual is None else float(cfg.m_residual)
         head_name = "transformer.wte.weight" if cfg.tie_word_embeddings else "lm_head.weight"
         self._dropout_now = s.get("dropout_seed")  # the masks of the forward being backpropagated
+        self._fp8_now = s.get("fp8", False)  # and its FP8 mode (recomputed blocks too)
+        self._fp8_wcache.clear()
         p_res = self._drop_p("resid_pdrop")
         if comm is not None:
             comm.pre_backward_unit(0)
@@ -806,6 +915,14 @@ class DolomiteEngine:
         if comm is not None:
             comm.post_backward_unit(0)
         self.join_wgrad_stream()  # optimizer / gradient norm / the next zero_grad run on the main stream
+        if self._fp8_now:
+            # DelayedScaling update of every slot.  TE updates the forward slots when the forward ends; nothing reads them
+            # between that point and here except this backward, which must see the forward's scales, so running both
+            # updates now gives the same scales to the next micro-step
+            # a sharded model's ranks run the same linears in lock step: their amaxes are reduced so the scales agree
+            self.fp8.update(all_reduce=self.comm is not None and self.world_size > 1)
+            self._fp8_now = False
+            self._fp8_wcache.clear()
         self._saved = None
 
     # ------------------------------------------------------------------------------------------

@@ -17,6 +17,8 @@ The tokenizer comes from `tokenizer_args.tokenizer_name` (or `model_args.model_n
 
 from __future__ import annotations
 
+from contextlib import nullcontext
+
 import time
 
 import torch.distributed as dist
@@ -94,7 +96,8 @@ def train(args: TrainingArgs, model, optimizer, scheduler, dataloader, rank: int
     for step in range(starting_iteration + 1, tp.num_training_steps + 1):
         loss, grad_norm = train_step(model, optimizer, scheduler, train_dataloader=dataloader,
                                      gradient_accumulation_steps=tp.gradient_accumulation_steps,
-                                     gradient_clipping=tp.gradient_clipping)
+                                     gradient_clipping=tp.gradient_clipping,
+                                     forward_context=getattr(model, "forward_context", nullcontext))
         losses.append(loss)
         if rank == 0 and step % args.logging_args.log_interval == 0:
             dt = (time.perf_counter() - t0) / (step - starting_iteration)
@@ -120,6 +123,9 @@ def main() -> None:
     if wrapper.tokenizer is None:
         raise ValueError("finetuning needs a tokenizer: set tokenizer_args.tokenizer_name (or model_args.model_name) to a local directory")
     model = wrap_model_for_distributed_training(args, wrapper)
+    from .fp8 import setup_training
+
+    model.forward_context = setup_training(args, wrapper)
     optimizer = get_optimizer(args.optimizer_args.class_name, args.optimizer_args.class_args, model,
                               args.optimizer_args.params_group_method)
     ls = args.lr_scheduler_args

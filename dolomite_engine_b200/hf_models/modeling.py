@@ -186,7 +186,7 @@ class DolomitePreTrainedModel(nn.Module):
             drop = (cu_seqlens[1:-1] - 1).long()
             shift_labels[drop] = -100
         input_ids, position_ids, cu_seqlens, shift_labels, T_real = _pad_packed_stream(input_ids, position_ids, cu_seqlens,
-                                                                                       shift_labels)
+                                                                                       shift_labels, self._token_multiple())
         out = _EngineFunction.apply(self._anchor, self, input_ids, position_ids, cu_seqlens, int(max_seqlen), shift_labels, -100, torch.is_grad_enabled())
         if shift_labels is not None:
             result = CausalLMOutputWithPast(loss=out, logits=None)
@@ -195,6 +195,12 @@ class DolomitePreTrainedModel(nn.Module):
         if not return_dict:
             return tuple(v for v in (result.loss, result.logits) if v is not None)
         return result
+
+    def _token_multiple(self) -> int:
+        """FP8 training forward: the token count is also the row length of the transposed fp8 operands of the weight
+        gradients, which the FP8 GEMM wants in multiples of 16.  Evaluation and generation run bf16 and pack as bf16 does."""
+        e = self.engine
+        return 16 if e.fp8 is not None and e.fp8_autocast and e.training and torch.is_grad_enabled() else 8
 
     def _forward_padded(self, input_ids, attention_mask, position_ids, labels, return_dict, past_key_values, use_cache,
                         inputs_embeds, token_type_ids, cu_seqlens):
@@ -237,7 +243,7 @@ class DolomitePreTrainedModel(nn.Module):
             nxt_valid[:, :-1] = mask[:, 1:]
             nxt = torch.where(nxt_valid & mask, nxt, torch.full_like(nxt, -100))
             shift_labels = nxt.reshape(-1)[keep].contiguous()
-        ids_p, pos_p, cu, shift_labels, T_real = _pad_packed_stream(ids_p, pos_p, cu, shift_labels)
+        ids_p, pos_p, cu, shift_labels, T_real = _pad_packed_stream(ids_p, pos_p, cu, shift_labels, self._token_multiple())
         out = _EngineFunction.apply(self._anchor, self, ids_p, pos_p, cu, int(max(max_seqlen, 1)), shift_labels, -100, torch.is_grad_enabled())
         if shift_labels is not None:
             result = CausalLMOutputWithPast(loss=out, logits=None)

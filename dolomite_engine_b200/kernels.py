@@ -391,6 +391,101 @@ def gemm_wgrad_multi(problems: list[tuple], n_rows: int | None = None) -> None:
 
 
 # ------------------------------------------------------------------------------------------------
+# FP8 (te.Linear under te.fp8_autocast with DelayedScaling, HYBRID: e4m3 forward, e5m2 output gradients)
+# ------------------------------------------------------------------------------------------------
+E4M3, E5M2 = 0, 1
+FP8_MAX = {E4M3: 448.0, E5M2: 57344.0}
+_U8 = torch.uint8
+
+
+def fp8_cast(x, fmt: int, scale, *, plain: bool = True, transpose: bool = False, amax=None, out=None, out_t=None):
+    """x bf16 [rows, cols] -> (q [rows, cols] or None, q_t [cols, rows] or None), uint8 storage of fp8 `fmt`;
+    q = satfinite_rne(fp32(x) * scale).  `scale`: fp32 device scalar (a 1-element view); `amax`: 1-element fp32 view that
+    receives max(amax, max|x|)."""
+    _req(x, _BF16, "x"), _req(scale, torch.float32, "scale")
+    assert x.dim() == 2 and x.stride(1) == 1 and (plain or transpose)
+    rows, cols = x.shape
+    if plain and out is None:
+        out = torch.empty(rows, cols, dtype=_U8, device=x.device)
+    if transpose and out_t is None:
+        out_t = torch.empty(cols, rows, dtype=_U8, device=x.device)
+    if amax is not None:
+        _req(amax, torch.float32, "amax")
+    _lib.call("dolomite_b200_fp8_cast", x.data_ptr(), x.stride(0), rows, cols, fmt, scale.data_ptr(),
+              _ptr(out) if plain else None, _ptr(out_t) if transpose else None, _ptr(amax), _stream())
+    return (out if plain else None), (out_t if transpose else None)
+
+
+def fp8_scaling_update(amax_history, scale, scale_inv, fmt: int) -> None:
+    """DelayedScaling update of every slot of one format: amax_history fp32 [len, n], scale / scale_inv fp32 [n]"""
+    _req(amax_history, torch.float32, "amax_history"), _req(scale, torch.float32, "scale")
+    _req(scale_inv, torch.float32, "scale_inv")
+    L, n = amax_history.shape
+    assert amax_history.is_contiguous() and scale.numel() == n and scale_inv.numel() == n
+    _lib.call("dolomite_b200_fp8_scaling_update", amax_history.data_ptr(), L, n, scale.data_ptr(), scale_inv.data_ptr(),
+              FP8_MAX[fmt], _stream())
+
+
+def gemm_fp8(a, a_fmt: int, a_scale_inv, b, b_fmt: int, b_scale_inv, *, out=None, out_dtype=_BF16, c=None, alpha=1.0,
+             beta=0.0, bias=None, split_accumulate: bool = False):
+    """D[M,N] = alpha * (a_scale_inv * b_scale_inv * A·Bᵀ + bias) + beta*C with A fp8 [M,K], B fp8 [N,K] (uint8 storage)"""
+    _req(a, _U8, "a"), _req(b, _U8, "b"), _req(a_scale_inv, torch.float32, "a_scale_inv")
+    _req(b_scale_inv, torch.float32, "b_scale_inv")
+    assert a.dim() == 2 and b.dim() == 2 and a.stride(1) == 1 and b.stride(1) == 1
+    M, K = a.shape
+    N, Kb = b.shape
+    if K != Kb:
+        raise _lib.DolomiteB200Error(f"gemm_fp8: contraction mismatch {K} vs {Kb}")
+    if out is None:
+        out = torch.empty(M, N, dtype=out_dtype, device=a.device)
+    assert out.stride(1) == 1 and out.shape == (M, N)
+    if c is not None:
+        assert c.dtype == out.dtype and c.stride(1) == 1
+    if gemm_timer is not None:
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+    _lib.call(
+        "dolomite_b200_gemm_fp8", a.data_ptr(), a.stride(0), a_fmt, b.data_ptr(), b.stride(0), b_fmt, a_scale_inv.data_ptr(),
+        b_scale_inv.data_ptr(), out.data_ptr(), out.stride(0), int(out.dtype == torch.float32), _ptr(c),
+        0 if c is None else c.stride(0), alpha, beta, _ptr(bias), M, N, K, int(split_accumulate), _stream(),
+    )
+    if gemm_timer is not None:
+        e1.record()
+        gemm_timer.append((2.0 * M * N * K, e0, e1))
+    return out
+
+
+def gemm_fp8_wgrad_multi(problems: list[tuple], dy_fmt: int = E5M2, x_fmt: int = E4M3, split_accumulate: bool = True):
+    """problems: up to 4 tuples (dyt fp8 [M, K], dy_scale_inv, xt fp8 [N, K], x_scale_inv, dw fp32 [M, N], alpha,
+    accumulate) -> ONE launch computing dw (+)= alpha * s_dy * s_x * dyt · xtᵀ for all of them"""
+    import ctypes
+
+    n = len(problems)
+    assert 1 <= n <= 4
+    K = problems[0][0].shape[1]
+    P, L, F, I = ctypes.c_void_p * n, ctypes.c_int64 * n, ctypes.c_float * n, ctypes.c_int * n
+    for dyt, sdy, xt, sx, dw, _, _ in problems:
+        _req(dyt, _U8, "dyt"), _req(xt, _U8, "xt"), _req(dw, torch.float32, "dw")
+        assert dyt.shape[1] == K and xt.shape[1] == K and dyt.stride(1) == 1 and xt.stride(1) == 1 and dw.stride(1) == 1
+        assert dw.shape == (dyt.shape[0], xt.shape[0])
+    if gemm_timer is not None:
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+    _lib.call(
+        "dolomite_b200_gemm_fp8_wgrad_multi", n, P(*[q[0].data_ptr() for q in problems]), L(*[q[0].stride(0) for q in problems]),
+        P(*[q[2].data_ptr() for q in problems]), L(*[q[2].stride(0) for q in problems]),
+        P(*[q[1].data_ptr() for q in problems]), P(*[q[3].data_ptr() for q in problems]),
+        P(*[q[4].data_ptr() for q in problems]), L(*[q[4].stride(0) for q in problems]),
+        L(*[q[0].shape[0] for q in problems]), L(*[q[2].shape[0] for q in problems]), K,
+        F(*[float(q[5]) for q in problems]), I(*[int(bool(q[6])) for q in problems]), dy_fmt, x_fmt, int(split_accumulate),
+        _stream(),
+    )
+    if gemm_timer is not None:
+        e1.record()
+        gemm_timer.append((sum(2.0 * K * q[0].shape[0] * q[2].shape[0] for q in problems), e0, e1))
+
+
+# ------------------------------------------------------------------------------------------------
 # packed var-len causal attention (attention/padding_free.py:51-62)
 # ------------------------------------------------------------------------------------------------
 def attn_varlen_fwd(qkv, cu_seqlens, max_seqlen: int, n_groups: int, q_per_group: int, head_dim: int, scale: float, out=None,

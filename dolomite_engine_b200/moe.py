@@ -25,8 +25,7 @@ def forward(engine, unit, p: str, x, residual, m_res: float, layer: int = 0):
     k = cfg.num_experts_per_tok
     if (p + "mlp.c_fc.bias") in unit.views:
         raise NotImplementedError("expert biases are not supported by the grouped-GEMM MoE path (moe/scatter.py:22)")
-    gate = unit.views[p + "mlp.gate.weight"]
-    logits = K.gemm(x, gate, flags=0)  # [T, E] bf16 (tiny N: direct-store epilogue)
+    logits = engine._linear(unit, p + "mlp.gate.weight", x, flags=0)  # [T, E] bf16 (tiny N: direct-store epilogue)
     plan = K.moe_route(logits, k)
     if FUSED_GATHER:
         # scattermoe `parallel_linear(grouped_in=False, grouped_out=True)`: the expert GEMM reads the token rows straight
@@ -68,6 +67,8 @@ def backward(engine, unit, p: str, x, dh, m_res: float, saved, layer: int = 0):
     dx = K.moe_token_sum(dxg, plan)
     # router path: softmax-over-k backward -> dense dlogits -> gate wgrad and dx contribution
     dlogits = K.moe_router_bwd(plan, dw)
+    if engine._is_fp8(p + "mlp.gate.weight"):  # the router as te.Linear (num_experts % 16 == 0)
+        return engine._linear_bwd_fp8(unit, p + "mlp.gate.weight", None, x, dlogits, dx_add=dx)
     gate = unit.views[p + "mlp.gate.weight"]
     ggate = unit.gviews[p + "mlp.gate.weight"]
     # dGate[E, H] += dlogits^T x: E rows are one row of output tiles with the whole token stream as contraction.  Not split

@@ -9,6 +9,8 @@ section 8f rank 2); `class_name: SyntheticPackedDataset` fabricates batches with
 
 from __future__ import annotations
 
+from contextlib import nullcontext
+
 import os
 import time
 
@@ -90,6 +92,9 @@ def build(args: TrainingArgs):
     shard_world, shard_rank = shard_world_and_rank(args, world, rank)
     wrapper = get_model(args, device=device, world_size=shard_world, rank=shard_rank)
     model = wrap_model_for_distributed_training(args, wrapper)
+    from .fp8 import setup_training
+
+    model.forward_context = setup_training(args, wrapper)
     optimizer = get_optimizer(args.optimizer_args.class_name, args.optimizer_args.class_args, model,
                               args.optimizer_args.params_group_method)
     ls = args.lr_scheduler_args
@@ -262,7 +267,8 @@ def train(args: TrainingArgs, model, optimizer, scheduler, dataloader, rank: int
     for step in range(starting_iteration + 1, tp.num_training_steps + 1):
         loss, grad_norm = train_step(model, optimizer, scheduler, train_dataloader=dataloader,
                                      gradient_accumulation_steps=tp.gradient_accumulation_steps,
-                                     gradient_clipping=tp.gradient_clipping)
+                                     gradient_clipping=tp.gradient_clipping,
+                                     forward_context=getattr(model, "forward_context", nullcontext))
         losses.append(loss)
         if profiler is not None:
             profiler.step()

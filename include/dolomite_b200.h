@@ -233,6 +233,43 @@ int dolomite_b200_gemm_bf16_wgrad_multi(int n_problems, const void* const* dY, c
                                         void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * FP8 linear layers with delayed scaling: what TransformerEngine's te.Linear computes inside
+ * te.fp8_autocast(DelayedScaling(Format.HYBRID, amax_history_len=16, amax_compute_algo="max")) -- the nn.Linear swap of
+ * distributed/fp8/nv_te.py:15-42 and the training forward context of pretrain.py:126-134 / finetune.py:90-98.
+ * Formats: 0 = e4m3 (max 448; inputs and weights), 1 = e5m2 (max 57344; output gradients).  fp8 tensors are uint8 storage.
+ *
+ * gemm_fp8:  D[M,N] = alpha * (a_scale_inv * b_scale_inv * sum_k A[m,k] * B[n,k] + bias[n]) + beta * C[m,n]
+ *   A fp8 row-major [M,K] (lda), B fp8 row-major [N,K] (ldb): both K-major (fp8 wgmma reads no other layout).
+ *   a_scale_inv / b_scale_inv: DEVICE fp32 scalars (no host sync).  D/C/bias as in gemm_bf16.
+ *   K % 16 == 0, N % 16 == 0, lda / ldb % 16 == 0, 16-byte aligned bases.
+ *   split_accumulate != 0: the tensor-core accumulator is added into a separate fp32 sum once per 128-deep k-block (TE's
+ *   split accumulator, dgrad / wgrad); 0 = one accumulator over the whole contraction (TE's fprop fast accumulation).
+ * gemm_fp8_wgrad_multi: up to 4 weight gradients in one launch, dW_i (+)= alpha_i * dYt_i . Xt_i^T with dYt_i fp8
+ *   [M_i, K] and Xt_i fp8 [N_i, K] (the transposed casts; K = token rows, K % 16 == 0), dW_i fp32.
+ * ------------------------------------------------------------------------------------------------ */
+int dolomite_b200_gemm_fp8(const void* A, int64_t lda, int a_fmt, const void* B, int64_t ldb, int b_fmt,
+                           const float* a_scale_inv, const float* b_scale_inv, void* D, int64_t ldd, int d_is_f32,
+                           const void* C, int64_t ldc, float alpha, float beta, const void* bias, int64_t M, int64_t N,
+                           int64_t K, int split_accumulate, void* stream);
+int dolomite_b200_gemm_fp8_wgrad_multi(int n_problems, const void* const* dYt, const int64_t* ld_dyt, const void* const* Xt,
+                                       const int64_t* ld_xt, const float* const* dy_scale_inv,
+                                       const float* const* x_scale_inv, float* const* dW, const int64_t* ld_dw,
+                                       const int64_t* M, const int64_t* N, int64_t K, const float* alpha,
+                                       const int* accumulate, int dy_fmt, int x_fmt, int split_accumulate, void* stream);
+/* fp8_cast: x bf16 [rows, cols] (ldx) -> q = satfinite_rne(fp32(x) * scale[0]) as fp8 `fmt`:
+ *   out   [rows, cols] contiguous (may be NULL), out_t [cols, rows] contiguous, the transpose (may be NULL; needs
+ *   rows % 16 == 0); amax (may be NULL): *amax = max(*amax, max|x|) -- the amax-history row 0 entry of the tensor's slot.
+ *   cols % 16 == 0, ldx % 8 == 0, 16-byte aligned pointers. */
+int dolomite_b200_fp8_cast(const void* x, int64_t ldx, int64_t rows, int64_t cols, int fmt, const float* scale, void* out,
+                           void* out_t, float* amax, void* stream);
+/* fp8_scaling_update: DelayedScaling's amax / scale update for n_slots tensors of one format in one launch.
+ *   amax_history fp32 [history_len, n_slots] (row 0 = current), scale / scale_inv fp32 [n_slots]:
+ *   amax = max over the history (NaN propagates); scale = fp8_max / amax if amax is finite and > 0, else kept;
+ *   scale_inv = 1 / scale; the history rolls by -1 along rows and row 0 is zeroed.  history_len <= 64. */
+int dolomite_b200_fp8_scaling_update(float* amax_history, int history_len, int64_t n_slots, float* scale, float* scale_inv,
+                                     float fp8_max, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Grouped GEMM for MoE experts (replaces scattermoe `parallel_linear`, moe_dolomite/moe/scatter.py:38-49, and the
  * per-expert F.linear loop of moe/base.py:12-50).  Token rows are grouped by expert, each segment padded to a
  * multiple of 256 rows (scattermoe `padded_block_indices`); m_tile_group[i] = expert of 128-row tile i (-1: unused).

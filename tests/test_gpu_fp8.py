@@ -1,0 +1,539 @@
+"""GPU: the FP8 kernels (cast / cast-transpose + amax, DelayedScaling update, FP8 GEMM) against the reference arithmetic of
+test_fp8.py, and the FP8 path of the engine."""
+
+import pytest
+import torch
+
+from test_fp8 import E4M3, E5M2, FP8_MAX, dequantize_ref, quantize_ref, recipe_update_ref
+
+pytestmark = pytest.mark.gpu
+
+
+@pytest.fixture(scope="module")
+def K():
+    from dolomite_engine_b200 import build
+    from dolomite_engine_b200 import kernels
+
+    build.build()
+    return kernels
+
+
+def _dev_scalar(v):
+    return torch.tensor([v], dtype=torch.float32, device="cuda")
+
+
+def _special_input(rows, cols, fmt, scale, ld=None, seed=0):
+    g = torch.Generator().manual_seed(seed)
+    x = torch.randn(rows, cols, generator=g) * 3.0
+    mx, tiny = FP8_MAX[fmt], (2.0 ** -9 if fmt == E4M3 else 2.0 ** -16)
+    flat = x.view(-1)
+    n = flat.numel()
+    idx = torch.randperm(n, generator=g)
+    flat[idx[:50]] = mx / scale * (1.0 + torch.rand(50, generator=g))  # above max after scaling: saturates
+    flat[idx[50:100]] = -mx / scale * (1.0 + torch.rand(50, generator=g))
+    flat[idx[100:200]] = tiny / scale * torch.randint(-12, 12, (100,), generator=g).float() / 2  # subnormals and ties
+    flat[idx[200]] = float("inf")
+    flat[idx[201]] = 0.0
+    xb = x.to(torch.bfloat16)
+    if ld is None:
+        return xb, xb.cuda()
+    buf = torch.zeros(rows, ld, dtype=torch.bfloat16)
+    buf[:, :cols] = xb
+    return xb, buf.cuda()[:, :cols]
+
+
+@pytest.mark.parametrize("fmt", [E4M3, E5M2])
+@pytest.mark.parametrize("shape", [(80, 208, None), (256, 64, 72), (16, 4096, None)])
+def test_cast_bit_exact(K, fmt, shape):
+    rows, cols, ld = shape
+    scale = 0.75
+    x_cpu, x = _special_input(rows, cols, fmt, scale, ld)
+    s = _dev_scalar(scale)
+    amax = torch.zeros(1, dtype=torch.float32, device="cuda")
+    q, qt = K.fp8_cast(x, fmt, s, transpose=True, amax=amax)
+    ref = quantize_ref(x_cpu, scale, fmt)
+    assert torch.equal(q.cpu(), ref)
+    assert torch.equal(qt.cpu(), ref.t().contiguous())
+    assert amax.item() == x_cpu.float().abs().max().item()  # inf included
+    # plain-only and transpose-only launches give the same bits; a finite input gives the exact finite amax
+    x_fin = torch.nan_to_num(x_cpu.float(), posinf=1.0).to(torch.bfloat16).cuda()
+    amax.fill_(0.0)
+    q2, none = K.fp8_cast(x_fin, fmt, s, amax=amax)
+    none2, qt2 = K.fp8_cast(x_fin, fmt, s, plain=False, transpose=True)
+    assert none is None and none2 is None
+    assert torch.equal(q2.cpu(), quantize_ref(x_fin.cpu(), scale, fmt)) and torch.equal(qt2, q2.t())
+    assert amax.item() == x_fin.float().abs().max().item()
+
+
+def test_cast_rejects_bad_shapes(K):
+    from dolomite_engine_b200._lib import DolomiteB200Error
+
+    s = _dev_scalar(1.0)
+    with pytest.raises(DolomiteB200Error, match="multiple of 16"):
+        K.fp8_cast(torch.zeros(16, 24, dtype=torch.bfloat16, device="cuda"), E4M3, s)
+    with pytest.raises(DolomiteB200Error, match="rows % 16"):
+        K.fp8_cast(torch.zeros(24, 32, dtype=torch.bfloat16, device="cuda"), E4M3, s, transpose=True)
+
+
+@pytest.mark.parametrize("fmt", [E4M3, E5M2])
+def test_scaling_update_bit_exact(K, fmt):
+    n, L = 37, 16
+    g = torch.Generator().manual_seed(3)
+    hist = torch.zeros(L, n, dtype=torch.float32)
+    scale = torch.ones(n, dtype=torch.float32)
+    d_hist, d_scale, d_sinv = hist.cuda(), scale.cuda(), torch.ones(n, dtype=torch.float32, device="cuda")
+    for step in range(40):  # > 2 wraps of the 16-row history
+        a = torch.exp(torch.randn(n, generator=g) * 4.0)
+        kind = torch.randint(0, 12, (n,), generator=g)
+        a[kind == 0] = 0.0
+        a[kind == 1] = float("inf")
+        a[kind == 2] = float("nan")
+        a[kind == 3] = 1e-42  # subnormal amax: 448 / amax overflows to inf
+        hist[0] = torch.maximum(hist[0], a) if step % 3 else a
+        d_hist[0].copy_(hist[0])
+        hist, scale, sinv = recipe_update_ref(hist, scale, FP8_MAX[fmt])
+        K.fp8_scaling_update(d_hist, d_scale, d_sinv, fmt)
+        assert torch.equal(d_hist.cpu().view(torch.int32), hist.view(torch.int32)), step
+        assert torch.equal(d_scale.cpu().view(torch.int32), scale.view(torch.int32)), step
+        assert torch.equal(d_sinv.cpu().view(torch.int32), sinv.view(torch.int32)), step
+
+
+def _fp8_operand(rows, cols, fmt, seed):
+    g = torch.Generator().manual_seed(seed)
+    x = (torch.randn(rows, cols, generator=g) * (1.0 + seed % 3)).to(torch.bfloat16)
+    amax = x.float().abs().max().item()
+    scale = FP8_MAX[fmt] / amax
+    q = quantize_ref(x, scale, fmt)
+    return q, dequantize_ref(q, fmt), float(torch.tensor(1.0 / scale, dtype=torch.float32))
+
+
+# Measured on an H100 80GB HBM3 (700 W): with split accumulation the fp32 result of the fp8 GEMM differs from the fp64 sum
+# of the same dequantised products by rel-L2 0.76e-4 .. 1.28e-4, at the small test shapes and at the C2 shapes alike.  That
+# error is made inside the tensor core's k32 step (its products are summed with fewer than 24 mantissa bits), which the
+# split accumulator cannot remove, so the 1e-5 first proposed for it is out of reach.  Bound: 4x the largest measured value.
+# Fast accumulation also keeps the tensor core's accumulator across k-blocks: 1.2e-4 .. 1.8e-4 at K = 208, 8.5e-4 at
+# K = 2048 and 2.0e-3 at K = 8192 (C2 shapes), bounded at 2.5x the largest.
+FP8_MMA_BOUND = 5e-4
+FP8_FAST_BOUND_C2 = 5e-3
+
+
+def rel_l2(a, b):
+    a, b = a.double().cpu(), b.double().cpu()
+    return ((a - b).norm() / (b.norm() + 1e-300)).item()
+
+
+@pytest.mark.parametrize("fa,fb", [(E4M3, E4M3), (E5M2, E4M3), (E4M3, E5M2), (E5M2, E5M2)])
+@pytest.mark.parametrize("split", [True, False])
+def test_gemm_against_fp64(K, fa, fb, split):
+    # M and N tails (not multiples of 128), K a multiple of 16 but not of 128
+    M, N, Kd = 200, 272, 208
+    qa, da, sa = _fp8_operand(M, Kd, fa, 1)
+    qb, db, sb = _fp8_operand(N, Kd, fb, 2)
+    ref = (da @ db.t()) * sa * sb
+    g = torch.Generator().manual_seed(5)
+    bias = (torch.randn(N, generator=g) * 0.5).to(torch.bfloat16)
+    c32 = torch.randn(M, N, generator=g)
+    A, B, SA, SB = qa.cuda(), qb.cuda(), _dev_scalar(sa), _dev_scalar(sb)
+    # fp32 output: the accumulator itself
+    d = K.gemm_fp8(A, fa, SA, B, fb, SB, out_dtype=torch.float32, split_accumulate=split)
+    err = rel_l2(d, ref)
+    print(f"fp8 gemm {fa}{fb} split={split}: rel-L2 {err:.3e}")
+    assert err <= FP8_MMA_BOUND
+    # alpha * (s * acc + bias) + beta * C, fp32 D accumulating into itself (wgrad)
+    d2 = c32.cuda()
+    K.gemm_fp8(A, fa, SA, B, fb, SB, out=d2, c=d2, alpha=0.5, beta=1.0, bias=bias.cuda(), split_accumulate=split)
+    ref2 = 0.5 * (ref + bias.double()) + c32.double()
+    assert rel_l2(d2, ref2) <= FP8_MMA_BOUND
+    # bf16 output with a bf16 residual: one bf16 rounding of the fp32 result
+    c16 = c32.to(torch.bfloat16)
+    d3 = K.gemm_fp8(A, fa, SA, B, fb, SB, c=c16.cuda(), alpha=2.0, beta=1.0, split_accumulate=split)
+    ref3 = 2.0 * ref + c16.double()
+    assert rel_l2(d3, ref3) <= 4e-3
+
+
+def test_gemm_wgrad_multi_matches_single(K):
+    probs, refs = [], []
+    T = 336  # token rows: the contraction
+    for q, (M, N) in enumerate([(256, 128), (128, 384), (384, 256), (144, 128)]):
+        qa, da, sa = _fp8_operand(M, T, E5M2, 10 + q)
+        qb, db, sb = _fp8_operand(N, T, E4M3, 20 + q)
+        dw = torch.randn(M, N).cuda()
+        ref = (da @ db.t()) * sa * sb * 0.25 + (dw.double().cpu() if q % 2 else 0)
+        probs.append((qa.cuda(), _dev_scalar(sa), qb.cuda(), _dev_scalar(sb), dw, 0.25, q % 2 == 1))
+        refs.append(ref)
+    K.gemm_fp8_wgrad_multi(probs)
+    for (_, _, _, _, dw, _, _), ref in zip(probs, refs):
+        assert rel_l2(dw, ref) <= FP8_MMA_BOUND
+
+
+def test_gemm_rejects_bad_shapes(K):
+    from dolomite_engine_b200._lib import DolomiteB200Error
+
+    a = torch.zeros(64, 40, dtype=torch.uint8, device="cuda")
+    s = _dev_scalar(1.0)
+    with pytest.raises(DolomiteB200Error, match="multiples of 16"):
+        K.gemm_fp8(a, E4M3, s, torch.zeros(64, 40, dtype=torch.uint8, device="cuda"), E4M3, s)
+
+
+C2_SHAPES = {  # (M = tokens, N = out features, K = in features) of the four block GEMMs of C2, one 4096-token sequence
+    "c_attn": (4096, 3072, 2048), "attn.c_proj": (4096, 2048, 2048), "c_fc": (4096, 16384, 2048),
+    "mlp.c_proj": (4096, 2048, 8192),
+}
+
+
+@pytest.mark.parametrize("name", list(C2_SHAPES))
+def test_gemm_fast_accumulation_error_at_c2_shapes(K, name):
+    """Fast accumulation (fprop) keeps one tensor-core accumulator over the whole contraction, split accumulation promotes
+    it once per 128-deep k-block (measured values at FP8_MMA_BOUND)."""
+    M, N, Kd = C2_SHAPES[name]
+    qa, da, sa = _fp8_operand(M // 4, Kd, E4M3, 31)  # a quarter of the rows keeps the fp64 reference affordable
+    qb, db, sb = _fp8_operand(N, Kd, E4M3, 32)
+    ref = (da.cuda() @ db.cuda().t()) * sa * sb
+    A, B, SA, SB = qa.cuda(), qb.cuda(), _dev_scalar(sa), _dev_scalar(sb)
+    fast = rel_l2(K.gemm_fp8(A, E4M3, SA, B, E4M3, SB, out_dtype=torch.float32), ref)
+    split = rel_l2(K.gemm_fp8(A, E4M3, SA, B, E4M3, SB, out_dtype=torch.float32, split_accumulate=True), ref)
+    print(f"{name} M={M // 4} N={N} K={Kd}: rel-L2 fast {fast:.3e} split {split:.3e}")
+    assert split <= FP8_MMA_BOUND
+    assert fast <= FP8_FAST_BOUND_C2
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the engine under fp8_autocast
+# ---------------------------------------------------------------------------------------------------------------------
+def _engine(untied=True, seed=42, **kw):
+    from test_fp8 import _cfg
+
+    from dolomite_engine_b200.engine import DolomiteEngine
+
+    cfg = _cfg(num_key_value_heads=2, tie_word_embeddings=not untied, vocab_size=1024, n_layer=2, **kw)
+    return DolomiteEngine(cfg, "cuda", seed=seed)
+
+
+def _batch(V, T=512, seed=0):
+    g = torch.Generator().manual_seed(seed)
+    ids = torch.randint(0, V, (T + 1,), generator=g)
+    inp, labels = ids[:-1].cuda(), ids[1:].cuda()
+    pos = torch.cat([torch.arange(200), torch.arange(T - 200)]).cuda()
+    cu = torch.tensor([0, 200, T], dtype=torch.int32).cuda()
+    return inp, pos, cu, 312, labels
+
+
+def _step(eng, batch, fp8: bool, lr=None):
+    from dolomite_engine_b200.fp8 import fp8_autocast
+    from contextlib import nullcontext
+
+    eng.zero_grad()
+    with fp8_autocast(eng) if fp8 else nullcontext():
+        _, loss = eng.forward(*batch, fuse_head_loss=True)
+    eng.backward()
+    if lr is not None:  # plain SGD on the fp32 masters
+        for u in eng.units:
+            u.master.data.add_(u.master.grad, alpha=-lr)
+        eng.refresh_compute_from_master()
+    return loss.item()
+
+
+def _grads(eng):
+    return {n: u.gviews[n].clone() for n, u, _ in eng.named_views()}
+
+
+def test_engine_fp8_linear_backward_matches_its_quantised_operands():
+    """The loss of an FP8 step is within 1e-2 of the BF16 loss (measured 1e-4 .. 3e-4 here), and every FP8 weight gradient
+    equals the fp64 product of its own e5m2 output gradient and e4m3 input, quantised with the engine's scales (measured
+    on an H100: rel-L2 0.8e-4 .. 1.5e-4 for the block weights, 9e-4 for the head, whose contraction holds the few large
+    one-hot terms of the loss gradient next to many small ones; bound 3e-3).
+
+    Whole-model gradients are not compared with the BF16 run: at initialisation the softmax is almost uniform and the
+    FP8 forward's rounding moves p - 1/V by a large fraction of itself, so the gradients of the two runs differ by rel-L2
+    0.6 .. 0.9 (measured) although each FP8 linear computes its backward as specified."""
+    ref, eng = _engine(), _engine()
+    eng.enable_fp8()
+    assert len(eng.fp8.names) == 9  # 4 per block + the untied head
+    b = _batch(1024)
+    l_ref = _step(ref, b, False)
+    _step(eng, b, True)  # step 0: scale 1
+    stash = {}
+    orig = eng._linear_bwd_fp8
+
+    def spy(unit, wname, bname, x, dy, *a, **k):
+        xs, gs = eng.fp8.input_slot(wname)[0].item(), eng.fp8.grad_slot(wname)[0].item()
+        stash[wname] = (x.float().cpu(), dy.float().cpu(), xs, gs, k.get("alpha", a[0] if a else 1.0))
+        return orig(unit, wname, bname, x, dy, *a, **k)
+
+    eng._linear_bwd_fp8 = spy
+    l8 = _step(eng, b, True)  # scales from the amaxes of step 0
+    print(f"loss bf16 {l_ref:.6f} fp8 {l8:.6f}")
+    assert abs(l8 - l_ref) / l_ref <= 1e-2
+    assert set(stash) == set(eng.fp8.names)
+    for name, (x, dy, xs, gs, alpha) in stash.items():
+        qx = dequantize_ref(quantize_ref(x.to(torch.bfloat16), xs, E4M3), E4M3) / xs
+        qdy = dequantize_ref(quantize_ref(dy.to(torch.bfloat16), gs, E5M2), E5M2) / gs
+        want = alpha * (qdy.t() @ qx)
+        _, unit, _ = next(v for v in eng.named_views() if v[0] == name)
+        err = rel_l2(unit.gviews[name], want)
+        print(f"{name}: rel-L2 against its quantised operands {err:.3e}")
+        assert err <= 3e-3
+    assert torch.all(eng.fp8.fwd_scale != 1.0) and torch.all(eng.fp8.bwd_scale != 1.0)
+
+
+def test_engine_fp8_training_deterministic_and_tracks_bf16():
+    runs = []
+    for _ in range(2):
+        eng = _engine()
+        eng.enable_fp8()
+        losses = [_step(eng, _batch(1024, seed=s % 4), True, lr=0.05) for s in range(30)]
+        runs.append((losses, _grads(eng), [u.master.detach().clone() for u in eng.units], eng.fp8.state_dict()))
+    ref = _engine()
+    ref_losses = [_step(ref, _batch(1024, seed=s % 4), False, lr=0.05) for s in range(30)]
+    (l1, g1, p1, r1), (l2, g2, p2, r2) = runs
+    assert l1 == l2
+    assert all(torch.equal(g1[n], g2[n]) for n in g1)
+    assert all(torch.equal(a, b) for a, b in zip(p1, p2))
+    assert all(torch.equal(r1[k], r2[k]) for k in r1 if k != "names")
+    print(f"fp8 loss {l1[0]:.4f} -> {l1[-1]:.4f}; bf16 {ref_losses[0]:.4f} -> {ref_losses[-1]:.4f}")
+    assert l1[-1] < l1[0] - 0.5
+    assert abs(l1[-1] - ref_losses[-1]) / ref_losses[-1] <= 2e-2
+
+
+def test_engine_fp8_checkpointing_bit_identical():
+    a, b = _engine(), _engine()
+    a.enable_fp8()
+    b.enable_fp8()
+    b.checkpoint_every = 1
+    for s in range(3):
+        assert _step(a, _batch(1024, seed=s), True) == _step(b, _batch(1024, seed=s), True)
+    ga, gb = _grads(a), _grads(b)
+    assert all(torch.equal(ga[n], gb[n]) for n in ga)
+    assert torch.equal(a.fp8.fwd_scale, b.fp8.fwd_scale) and torch.equal(a.fp8.bwd_history, b.fp8.bwd_history)
+
+
+def test_engine_fp8_eval_and_bf16_steps_unchanged():
+    """outside fp8_autocast an FP8-configured engine computes what the BF16 engine does (evaluate, generate)"""
+    a, b = _engine(), _engine()
+    a.enable_fp8()
+    _step(a, _batch(1024), True)  # non-trivial scales (no parameter update: both keep the same weights)
+    inp, pos, cu, ms, labels = _batch(1024, seed=5)
+    for eng in (a, b):
+        eng.training = False
+    la, _ = a.forward(inp, pos, cu, ms, save_for_backward=False)
+    lb, _ = b.forward(inp, pos, cu, ms, save_for_backward=False)
+    assert torch.equal(la, lb)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# model level: the engine against the CPU oracle whose linears are the FP8 linear below, given the engine's own scales
+# ---------------------------------------------------------------------------------------------------------------------
+class _Fp8LinearRef(torch.autograd.Function):
+    """te.Linear restated: e4m3 input and weight, fp32 product of the dequantised operands, e5m2 output gradient"""
+
+    @staticmethod
+    def forward(ctx, x, w, b, s):
+        (xs, xsi), (ws, wsi), (gs, gsi) = s
+        # te.Linear under bf16 autocast quantises bf16 tensors: round the oracle's fp32 activations (and gradients) first
+        qx = dequantize_ref(quantize_ref(x.detach().bfloat16(), xs, E4M3), E4M3).float() * xsi
+        qw = dequantize_ref(quantize_ref(w.detach(), ws, E4M3), E4M3).float() * wsi
+        ctx.save_for_backward(qx, qw)
+        ctx.g = (gs, gsi)
+        ctx.has_bias = b is not None
+        y = qx @ qw.t()
+        return y + b if b is not None else y
+
+    @staticmethod
+    def backward(ctx, dy):
+        qx, qw = ctx.saved_tensors
+        gs, gsi = ctx.g
+        qdy = dequantize_ref(quantize_ref(dy.bfloat16(), gs, E5M2), E5M2).float() * gsi
+        return qdy @ qw, qdy.t() @ qx, (dy.sum(0) if ctx.has_bias else None), None
+
+
+def _oracle_cfgs():
+    from oracle.validate_against_reference import CONFIGS
+
+    return {
+        # dense RMSNorm + SwiGLU + GQA, untied head (FP8 head), biases and muP multipliers
+        "gqa_untied": dict(CONFIGS["gqa_bias_mup"]),
+        # bigcode: LayerNorm + tanh-GELU + learned positions + MQA + biases
+        "bigcode": dict(CONFIGS["bigcode"]),
+        # an MLP width that is not a multiple of 16: c_fc / c_proj stay bf16 next to FP8 attention linears (mixed launch)
+        "bigcode_mixed": dict(CONFIGS["bigcode"], n_inner=520),
+        # MoE with 32 experts: the router gate is an FP8 linear, the experts stay bf16
+        "moe32": dict(vocab_size=512, n_positions=256, n_embd=128, n_layer=2, n_head=8, n_inner=192,
+                      attention_head_type="mha", add_bias=False, num_experts=32, num_experts_per_tok=2),
+    }
+
+
+def _engine_and_oracle(name):
+    import oracle.dolomite_oracle as O
+
+    from dolomite_engine_b200.engine import DolomiteEngine
+    from dolomite_engine_b200.hf_models import GPTDolomiteConfig, MoEDolomiteConfig
+
+    kw = _oracle_cfgs()[name]
+    ocfg = O.OracleConfig(**kw)
+    params = O.init_params(ocfg, seed=42)
+    g = torch.Generator().manual_seed(7)
+    for k in params:
+        if k.endswith(".bias") and not k.startswith("transformer.ln") and ".ln_" not in k:
+            params[k] = torch.randn(params[k].shape, generator=g) * 0.02
+    params = {k: v.bfloat16().float() for k, v in params.items()}  # the engine computes with bf16 weights
+    cls = MoEDolomiteConfig if kw.get("num_experts") else GPTDolomiteConfig
+    d = dict(position_embedding_type="rope", normalization_function="rmsnorm", activation_function="swiglu",
+             resid_pdrop=0, embd_pdrop=0, attn_pdrop=0, eos_token_id=7)
+    d.update(kw)
+    eng = DolomiteEngine(cls(**d), "cuda", seed=None)
+    eng.load_state_dict(params)
+    eng.enable_fp8()
+    return eng, ocfg, params
+
+
+@pytest.mark.parametrize("name", ["gqa_untied", "bigcode", "bigcode_mixed", "moe32"])
+def test_engine_fp8_matches_fp8_oracle(name):
+    """Logits, loss and every parameter gradient of an FP8 step against the oracle model whose FP8 linears are
+    _Fp8LinearRef with the engine's scales.  The oracle computes in fp32 from the bf16 weights; the engine rounds its
+    activations to bf16 between kernels, so where the two straddle an fp8 rounding boundary they quantise one fp8 step
+    (6-12 % for e4m3, 12-25 % for e5m2) apart, and these flips compound towards the first block.  Measured on an H100:
+    loss 1.4e-5 .. 5.2e-5, logits 6.7e-3 .. 2.2e-2, worst parameter gradient 6.2e-2 .. 1.13e-1 (block 0's c_attn / ln_1;
+    later blocks and the head stay within 3e-2).  Bars: loss 1e-3 (the bf16 parity bar), logits 5e-2, gradients 2e-1,
+    about 2x the largest measured value; each FP8 linear alone is pinned to 3e-3 by the test above."""
+    import numpy as np
+
+    import oracle.dolomite_oracle as O
+    from dolomite_engine_b200.fp8 import fp8_autocast
+
+    eng, ocfg, params = _engine_and_oracle(name)
+    T = 256
+    rng = np.random.default_rng(11)
+    ids = torch.from_numpy(rng.integers(0, ocfg.vocab_size, size=T, dtype=np.int64))
+    labels = torch.from_numpy(rng.integers(0, ocfg.vocab_size, size=T, dtype=np.int64))
+    cu_np = np.array([0, 100, T], dtype=np.int32)
+    pos = torch.cat([torch.arange(100), torch.arange(T - 100)])
+    args = (ids.cuda(), pos.cuda(), torch.from_numpy(cu_np).cuda(), 156)
+    # step 0 sets the scales (scale 1 before it); step 1 is compared
+    eng.zero_grad()
+    with fp8_autocast(eng):
+        eng.forward(*args, labels=labels.cuda(), fuse_head_loss=True)
+    eng.backward()
+    fs, fsi = eng.fp8.fwd_scale.cpu().tolist(), eng.fp8.fwd_scale_inv.cpu().tolist()
+    bs, bsi = eng.fp8.bwd_scale.cpu().tolist(), eng.fp8.bwd_scale_inv.cpu().tolist()
+    assert all(s != 1.0 for s in fs + bs)
+    eng.zero_grad()
+    with fp8_autocast(eng):
+        logits, _ = eng.forward(*args)  # logits kept: the loss gradient is handed to backward
+    routing = {}
+    if eng.is_moe:
+        routing = {f"transformer.h.{i}.mlp.": layer[-1][0].sel_idx.long().cpu() for i, layer in enumerate(eng._saved["layers"])}
+    lg = logits.float()
+    loss = torch.nn.functional.cross_entropy(lg, labels.cuda())
+    dl = (torch.softmax(lg, -1) - torch.nn.functional.one_hot(labels.cuda(), lg.shape[1]).float()) / T
+    eng.backward(dlogits=dl.to(torch.bfloat16))
+
+    p_req = {k: v.clone().requires_grad_(True) for k, v in params.items()}
+    slots = {}
+    for n in eng.fp8.names:
+        j = eng.fp8.index[n]
+        slots[id(p_req[n])] = ((fs[2 * j], fsi[2 * j]), (fs[2 * j + 1], fsi[2 * j + 1]), (bs[j], bsi[j]))
+    orig = O.linear
+
+    def linear(x, w, b, bf16=False):
+        s = slots.get(id(w))
+        return orig(x, w, b, bf16) if s is None else _Fp8LinearRef.apply(x, w, b, s)
+
+    O.linear = linear
+    O.FORCED_ROUTING.update(routing)
+    try:
+        logits_ref = O.forward_logits(p_req, ocfg, ids.numpy(), pos.numpy(), cu_np)
+        loss_ref = torch.nn.functional.cross_entropy(logits_ref, labels)
+        loss_ref.backward()
+    finally:
+        O.linear = orig
+        O.FORCED_ROUTING.clear()
+    e_logits = rel_l2(logits, logits_ref.detach())
+    e_loss = abs(loss.item() - loss_ref.item()) / loss_ref.item()
+    errs = {n: rel_l2(u.gviews[n], p_req[n].grad) for n, u, _ in eng.named_views() if p_req[n].grad is not None}
+    worst = max(errs, key=errs.get)
+    print(f"{name}: logits {e_logits:.2e} loss {e_loss:.2e} worst gradient {worst} {errs[worst]:.2e}; "
+          f"fp8 linears {len(eng.fp8.names)}")
+    assert e_logits <= 5e-2 and e_loss <= 1e-3
+    assert errs[worst] <= 2e-1, sorted(errs.items(), key=lambda kv: -kv[1])[:5]
+
+
+def test_engine_fp8_gradient_accumulation_updates_once_per_micro_step():
+    """three micro-steps without zero_grad: every backward rolls the history once and sets the scales from it"""
+    eng = _engine()
+    eng.enable_fp8()
+    eng.zero_grad()
+    from dolomite_engine_b200.fp8 import fp8_autocast
+
+    prev = (eng.fp8.fwd_history.cpu(), eng.fp8.fwd_scale.cpu(), eng.fp8.bwd_history.cpu(), eng.fp8.bwd_scale.cpu())
+    for m in range(3):
+        with fp8_autocast(eng):
+            eng.forward(*_batch(1024, seed=m), fuse_head_loss=True)
+        eng.backward()
+        cur = (eng.fp8.fwd_history.cpu(), eng.fp8.fwd_scale.cpu(), eng.fp8.bwd_history.cpu(), eng.fp8.bwd_scale.cpu())
+        for (h0, s0, fmt), (h1, s1) in zip([(prev[0], prev[1], E4M3), (prev[2], prev[3], E5M2)],
+                                          [(cur[0], cur[1]), (cur[2], cur[3])]):
+            # this micro-step's amaxes now sit in the last row; one update of the previous state with them gives the new state
+            before = h0.clone()
+            before[0] = h1[-1]
+            want_h, want_s, _ = recipe_update_ref(before, s0, FP8_MAX[fmt])
+            assert torch.equal(h1, want_h) and torch.equal(s1, want_s), m
+        prev = cur
+
+
+def test_engine_fp8_resume_is_bit_identical(tmp_path):
+    """save_checkpoint after 3 steps, load_checkpoint_for_training into a differently initialised engine: the next 3 steps
+    and the recipe state equal those of the uninterrupted run"""
+    import types
+
+    from dolomite_engine_b200 import checkpointing as C
+
+    ns = types.SimpleNamespace
+    path = str(tmp_path / "ckpt")
+    save_args = ns(save_args=ns(save_path=path, save_optimizer=False), distributed_args=ns(fsdp_algorithm=1),
+                   model_dump=lambda mode="json": {})
+    load_args = ns(load_args=ns(load_path=path, iteration=None, load_optimizer=False, load_lr_scheduler=False,
+                                resume_learning_rate=False, load_rng_state=True))
+    a = _engine()
+    a.enable_fp8()
+    for s in range(3):
+        _step(a, _batch(1024, seed=s), True, lr=0.05)
+    C.save_checkpoint(save_args, ns(engine=a), None, None, None, None, 3)
+    b = _engine(seed=7)
+    b.enable_fp8()
+    C.load_checkpoint_for_training(load_args, ns(engine=b), None, None, None)
+    assert torch.equal(a.fp8.fwd_scale, b.fp8.fwd_scale) and torch.equal(a.fp8.bwd_history, b.fp8.bwd_history)
+    la = [_step(a, _batch(1024, seed=s), True, lr=0.05) for s in range(3, 6)]
+    lb = [_step(b, _batch(1024, seed=s), True, lr=0.05) for s in range(3, 6)]
+    assert la == lb
+    assert all(torch.equal(u.master, v.master) for u, v in zip(a.units, b.units))
+    ra, rb = a.fp8.state_dict(), b.fp8.state_dict()
+    assert all(torch.equal(ra[k], rb[k]) for k in ra if k != "names")
+
+
+def test_engine_fp8_overlapped_weight_gradients_equal():
+    """DOLO_OVERLAP_WGRADS: the FP8 weight gradients of a block on the side stream give the same bits"""
+    a, b = _engine(), _engine()
+    a.enable_fp8()
+    b.enable_fp8()
+    b.overlap_wgrads = True
+    for s in range(2):
+        assert _step(a, _batch(1024, seed=s), True) == _step(b, _batch(1024, seed=s), True)
+    ga, gb = _grads(a), _grads(b)
+    assert all(torch.equal(ga[n], gb[n]) for n in ga)
+
+
+def test_fp8_ddp_parity_over_nccl():
+    """tools/ddp_parity.py FP8=1 on two GPUs: sharded == unsharded, and both ranks hold identical scales"""
+    import os
+    import subprocess
+    import sys
+
+    if torch.cuda.device_count() < 2:
+        pytest.skip(f"needs 2 GPUs, this box has {torch.cuda.device_count()}")
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    env = dict(os.environ, FP8="1", COMM_DTYPE="fp32", RESHARD="0")
+    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--master-addr", "127.0.0.1",
+           "--master-port", str(29950 + os.getpid() % 40), os.path.join(root, "tools", "ddp_parity.py")]
+    proc = subprocess.run(cmd, env=env, capture_output=True, text=True, timeout=600)
+    tail = (proc.stdout + proc.stderr)[-3000:]
+    assert proc.returncode == 0 and "DDP_PARITY OK" in proc.stdout, tail

@@ -5,7 +5,9 @@
 env: COMM_DTYPE=fp32|bf16 (wire dtype of the reduce-scatter), ACCUM=k (micro-steps per optimizer step, the first k-1
 under no_sync()), RESHARD=1 (what `stage: 3` means: block units share two parameter / gradient buffers, parameters are
 re-gathered in backward, gradients reduce-scattered per micro-step), CKPT=k (block activation checkpointing),
-SHARD=S (HSDP: S consecutive ranks per shard group), MOE=1 (MoEDolomite blocks instead of dense ones).
+SHARD=S (HSDP: S consecutive ranks per shard group), MOE=1 (MoEDolomite blocks instead of dense ones), FP8=1 (the linears
+in FP8 with delayed scaling, ACCUM=1: the ranks all-reduce their amaxes, so every rank must hold the same scales; the
+unsharded copy runs every rank's micro-batch with the scales the ranks used in that step).
 
 Every rank r feeds its own micro-batches to the sharded model (world_size = N); rank 0 additionally runs an unsharded
 copy of the same model over ALL micro-batches of all ranks.  Checks per step: (1) mean loss over ranks == mean loss
@@ -20,7 +22,10 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
+from contextlib import nullcontext
+
 from dolomite_engine_b200.distributed import ShardedDataParallel, build_data_parallel_groups, configure_comm_ctas
+from dolomite_engine_b200.fp8 import fp8_autocast
 from dolomite_engine_b200.model_wrapper import ModelWrapperForPretraining
 from dolomite_engine_b200.optimization import get_optimizer
 
@@ -59,9 +64,21 @@ def main():
         ref = ModelWrapperForPretraining(pretrained_config=dict(CFG), micro_batch_size=mbs, sequence_length=seq, device=dev)
         ref_sdp = ShardedDataParallel(ref, None, reshard_after_forward=False)
         ref_opt = get_optimizer("DolomiteFusedAdamW", OPT, ref_sdp)
+    fp8 = os.environ.get("FP8", "0") == "1"
+    eng = w.model.engine
+    ref_eng = ref.model.engine if rank == 0 else None
+    if fp8:
+        assert accum == 1, "FP8=1 runs with ACCUM=1"
+        eng.enable_fp8()
+        if rank == 0:
+            ref_eng.enable_fp8()
+            ref_eng.fp8.update = lambda all_reduce=False: None  # takes the ranks' scales before every step instead
+    ctx = (lambda e: fp8_autocast(e)) if fp8 else (lambda e: nullcontext())
     rng = np.random.default_rng(0)
     ok = True
     for step in range(4):
+        if fp8 and rank == 0:
+            ref_eng.fp8.load_state_dict(eng.fp8.state_dict())
         # tokens[m][r]: micro-step m, rank r
         tokens = [[torch.from_numpy(rng.integers(0, 1024, size=(mbs, seq + 1), dtype=np.int64)) for _ in range(world)]
                   for _ in range(accum)]
@@ -72,19 +89,29 @@ def main():
                 l = sdp({"text": tokens[m][rank]})
                 l.backward()
                 lsum += l.detach()
-        l = sdp({"text": tokens[accum - 1][rank]})
+        with ctx(eng):
+            l = sdp({"text": tokens[accum - 1][rank]})
         l.backward()
         lsum += l.detach()
         torch.cuda.synchronize()
         lsum /= accum
         dist.all_reduce(lsum, op=dist.ReduceOp.AVG)
         fulls = [w.model.engine.full_master(u) for u in w.model.engine.units]  # collective: every rank
+        if fp8:  # the amax all-reduce gives every rank the same scales
+            st = torch.cat([eng.fp8.fwd_scale, eng.fp8.bwd_scale, eng.fp8.fwd_history.flatten()])
+            every = [torch.empty_like(st) for _ in range(world)]
+            dist.all_gather(every, st)
+            same = all(torch.equal(every[0], x) for x in every)
+            if rank == 0 and not same:
+                print(f"step {step}: FP8 scales differ between ranks", flush=True)
+            ok = ok and same
         if rank == 0:
             ref_sdp.zero_grad()
             rl = 0.0
             for m in range(accum):
                 for t in tokens[m]:
-                    x = ref_sdp({"text": t})
+                    with ctx(ref_eng):
+                        x = ref_sdp({"text": t})
                     x.backward()
                     rl += x.item()
             rl /= world * accum
@@ -123,7 +150,7 @@ def main():
     dist.destroy_process_group()
     if rank == 0:
         print("DDP_PARITY", "OK" if ok else "FAILED", f"(world {world}, wire {os.environ.get('COMM_DTYPE', 'fp32')}, accum {accum}, "
-              f"reshard {int(reshard)}, moe {os.environ.get('MOE', '0')})", flush=True)
+              f"reshard {int(reshard)}, moe {os.environ.get('MOE', '0')}, fp8 {int(fp8)})", flush=True)
     sys.exit(0 if flag.item() == 1.0 else 1)
 
 
