@@ -40,8 +40,15 @@ static int g_gemm_l2_hints = 1;
 int dolo_option_gemm_l2_hints() { return g_gemm_l2_hints; }
 static int g_gemm_dynamic = 1;
 static int g_gemm_f32_tma_epilogue = 0;
+static int g_gemm_tile_n = 0;
+int dolo_option_gemm_tile_n() { return g_gemm_tile_n; }
 
 extern "C" int dolomite_b200_set_option(const char* key, int value) {
+    if (key != nullptr && strcmp(key, "gemm_tile_n") == 0) {
+        DOLO_REQUIRE(value == 0 || value == 128 || value == 256, "gemm_tile_n must be 0 (automatic), 128 or 256");
+        g_gemm_tile_n = value;
+        return DOLO_OK;
+    }
     if (key != nullptr && strcmp(key, "gemm_sm_margin") == 0) {
         DOLO_REQUIRE(value >= 0 && value <= 64, "gemm_sm_margin must be in [0, 64]");
         g_gemm_sm_margin = value;
@@ -95,6 +102,7 @@ extern "C" int dolomite_b200_get_option(const char* key, int* value) {
     else if (strcmp(key, "gemm_f32_tma_epilogue") == 0) *value = g_gemm_f32_tma_epilogue;
     else if (strcmp(key, "gemm_dynamic") == 0) *value = g_gemm_dynamic;
     else if (strcmp(key, "gemm_cta_pair") == 0) *value = g_gemm_cta_pair;
+    else if (strcmp(key, "gemm_tile_n") == 0) *value = g_gemm_tile_n;
     else return dolo_set_error("unknown option '%s'", key);
     return DOLO_OK;
 }

@@ -44,6 +44,7 @@ int dolo_option_gemm_sm_margin();
 // longest tiles of a document first, so that the last wave holds short tiles only); 0 = tiles fastest
 int dolo_option_attn_head_fastest();
 int dolo_option_gemm_l2_hints();  // 1 (default) = evict-first / evict-last operand loads for long-contraction GEMMs
+int dolo_option_gemm_tile_n();    // 0 (default) = tile width of dense bf16 GEMMs chosen per launch; 128 | 256 = forced
 
 // TMA descriptor encode through the driver entry point (no link-time libcuda dependency).
 // rank-2 / rank-3 fp8 (elem_bytes 1) / bf16 / f32 tiled maps.  dims/strides innermost first; strides in BYTES for dims >= 1.
@@ -237,6 +238,17 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 template <int N>
 __device__ __forceinline__ void wgmma_wait() {
     asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// Warpgroup register reallocation: a warp-specialised kernel moves the registers its producer warpgroup does not need to
+// its consumer warpgroups.  .sync.aligned per warpgroup: all four warps of the warpgroup execute the same instruction.
+// N is a multiple of 8 in [24, 256].
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
 }
 // Compile-time only: ties accumulator registers to the asm stream, so that no read of them is scheduled above a
 // wgmma_wait (the asm of the MMA and of the wait do not name them together).

@@ -1,8 +1,11 @@
-// bf16 GEMM for sm_90a (H100):  TMA (cp.async.bulk.tensor) -> 128B-swizzled smem ring -> wgmma (m64n128k16 per consumer
-// warpgroup, fp32 accumulators in registers) -> epilogue straight from the registers (alpha / bias / beta*C, bf16 | fp32).
+// bf16 GEMM for sm_90a (H100):  TMA (cp.async.bulk.tensor) -> 128B-swizzled smem ring -> wgmma (m64n128k16 or
+// m64n256k16 per consumer warpgroup, fp32 accumulators in registers) -> epilogue straight from the registers
+// (alpha / bias / beta*C, bf16 | fp32).
 //
 // Persistent, warp-specialised: warpgroup 0 = producer (one elected thread issues the TMA loads; the whole first warp for
-// gather-on-load), warpgroups 1 and 2 = consumers, each owning 64 rows of the 128 x 128 output tile.
+// gather-on-load), warpgroups 1 and 2 = consumers, each owning 64 rows of the output tile.  The tile is 128 x 128 (six
+// 32 KB stages) or, for dense launches, 128 x 256 (four 48 KB stages; setmaxnreg moves registers from the producer to
+// the consumers, which hold 128 accumulators each).  choose_tile_n picks the width per launch from the tile counts.
 // Both operands may be K-major (row-major [rows, K]) or MN-major (stored [K, rows]); the latter is what dgrad / wgrad
 // need, so no transposes are ever materialised:
 //     fwd   Y[T,N]  = X[T,K]  . W[N,K]^T          A K-major,  B K-major
@@ -19,8 +22,8 @@ using namespace dolo;
 namespace {
 
 constexpr int BM = 128;
-constexpr int BN = 128;
-constexpr int BK = 64;  // 64 bf16 = 128 bytes = one swizzle span
+constexpr int BN = 128;  // tile width of the grouped, gather-on-load and split-K modes and of the fp8 kernel
+constexpr int BK = 64;   // 64 bf16 = 128 bytes = one swizzle span
 constexpr int STAGES = 6;
 constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KB
 constexpr int B_STAGE_BYTES = BN * BK * 2;  // 16 KB
@@ -28,6 +31,29 @@ constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
 constexpr int GEMM_THREADS = 384;  // warpgroup 0 producer, 1..2 consumers
 constexpr int SMEM_BYTES = 1024 /*align slack*/ + STAGES * STAGE_BYTES + 256 /*barriers*/;
 static_assert(SMEM_BYTES <= 232448, "shared memory budget exceeded (227 KB per block on sm_90)");
+
+// Stage ring of the bf16 kernel per output tile width TN: 128 x 128 keeps six 32 KB stages, 128 x 256 four 48 KB stages.
+template <int TN>
+struct Ring {
+    static_assert(TN == 128 || TN == 256, "tile width 128 or 256");
+    static constexpr int STAGES = TN == 256 ? 4 : 6;
+    static constexpr int B_BYTES = TN * BK * 2;
+    static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_BYTES;
+    static constexpr int SMEM_BYTES = 1024 /*align slack*/ + STAGES * STAGE_BYTES + 256 /*barriers*/;
+    static_assert(SMEM_BYTES <= 232448, "shared memory budget exceeded (227 KB per block on sm_90)");
+};
+
+// Registers per thread of the 128 x 256 kernel after setmaxnreg: the producer warpgroup only issues TMA loads, the
+// consumers hold 128 fp32 accumulators each.  40 * 128 + 2 * 232 * 128 <= 65536 registers per SM.
+constexpr int PRODUCER_REGS = 40;
+constexpr int CONSUMER_REGS = 232;
+static_assert(PRODUCER_REGS * 128 + 2 * CONSUMER_REGS * 128 <= 65536, "register file exceeded");
+
+// Time of one 128 x 256 tile over one 128 x 128 tile of the same K (see choose_tile_n): the median over the twelve bf16
+// GEMM launches of a C2 training step, measured by tools/bench_gemm.py on an H100 80GB HBM3 at a 700 W power limit
+// (per launch 1.47 .. 1.87; the launches that fill their waves at both widths give 1.63 .. 1.87).  Every value in
+// (5/3, 1.875) makes the same choices at C2: 128 for the 4096 x 2560 outputs, 256 for all the others.
+constexpr double TILE256_COST = 1.81;
 
 constexpr int MAXP = 4;  // problems per launch (the four weight gradients of a transformer block share one launch)
 
@@ -127,9 +153,14 @@ __device__ __forceinline__ TileInfo tile_info(int t, const GemmParams& p) {
     return ti;
 }
 
-template <bool A_MN, bool B_MN>
+// TN: output tile width.  The 128 x 256 tile runs dense launches only (grouped == 0, no gather), because the grouped
+// modes' tile tables are per 128 x 128 tile.
+template <bool A_MN, bool B_MN, int TN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
     gemm_bf16_kernel(const __grid_constant__ GemmMaps maps, const __grid_constant__ GemmParams p) {
+    constexpr int STAGES = Ring<TN>::STAGES;
+    constexpr int B_STAGE_BYTES = Ring<TN>::B_BYTES;
+    constexpr int STAGE_BYTES = Ring<TN>::STAGE_BYTES;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_align_1024(smem_raw);
     uint8_t* smem_a = smem;
@@ -142,7 +173,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     const int num_tiles = p.num_tiles;
-    const bool gather = !A_MN && p.a_row_index != nullptr;
+    const bool gather = TN == 128 && !A_MN && p.a_row_index != nullptr;
 
     if (threadIdx.x == 0) {
         for (int q = 0; q < p.n_prob; ++q) {
@@ -160,6 +191,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 
     if (wg == 0) {
         // ================= producer =================
+        if constexpr (TN == 256) setmaxnreg_dec<PRODUCER_REGS>();  // all four warps, before warps 1..3 leave
         if (warp != 0) return;
         if (gather) {
             // Gather-on-load (grouped expert GEMM reading the UNGROUPED activations): lane l copies rows 4l .. 4l+3 of the
@@ -230,11 +262,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
                             tma_load_2d_hint(sa + i * (BK * 128), tmap_a, &full_bar[stage], m_blk * BM + i * 64, kb * BK, ha);
                     }
                     if (!B_MN) {
-                        tma_load_2d_hint(sb, tmap_b, &full_bar[stage], kb * BK, b_outer + n_blk * BN, hb);
+                        tma_load_2d_hint(sb, tmap_b, &full_bar[stage], kb * BK, b_outer + n_blk * TN, hb);
                     } else {
 #pragma unroll
-                        for (int i = 0; i < BN / 64; ++i)
-                            tma_load_2d_hint(sb + i * (BK * 128), tmap_b, &full_bar[stage], n_blk * BN + i * 64,
+                        for (int i = 0; i < TN / 64; ++i)
+                            tma_load_2d_hint(sb + i * (BK * 128), tmap_b, &full_bar[stage], n_blk * TN + i * 64,
                                              b_outer + kb * BK, hb);
                     }
                     if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -245,17 +277,18 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     }
 
     // ================= consumers: warpgroup cw owns rows [64 cw, 64 cw + 64) of the tile =================
+    if constexpr (TN == 256) setmaxnreg_inc<CONSUMER_REGS>();
     const int cw = wg - 1;
     const int wr = (warp & 3) * 16 + (lane >> 2);  // accumulator row of this thread inside the warpgroup (and +8)
     const int wc = 2 * (lane & 3);                 // first accumulator column inside each n8 block
     int stage = 0;
     uint32_t phase = 0;
-    float acc[BN / 2];
+    float acc[TN / 2];
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
         const TileInfo ti = tile_info(t, p);
         const Problem& pr = p.pr[ti.q];
         const int64_t row0 = int64_t(ti.m_blk) * BM + cw * 64 + wr;
-        const int col0 = ti.n_blk * BN + wc;
+        const int col0 = ti.n_blk * TN + wc;
         if (!ti.valid) {
             // K-grouped launch (expert weight gradients) and this expert received NO rows: its product is zero.  A launch
             // that OVERWRITES (beta = 0, no C) must still write the tile -- the caller did not clear the buffer.
@@ -265,7 +298,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
                 for (int h = 0; h < 2; ++h) {
                     const int64_t row = row0 + 8 * h;
                     if (row >= pr.M) continue;
-                    for (int j = 0; j < BN / 8; ++j)
+                    for (int j = 0; j < TN / 8; ++j)
                         if (col0 + 8 * j < pr.N)
                             *reinterpret_cast<float2*>(D + row * pr.ldd + col0 + 8 * j) = make_float2(0.f, 0.f);
                 }
@@ -287,7 +320,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
                 const uint64_t adesc = A_MN ? gmma_desc(sa + cw * (BK * 128) + k * 2048, BK * 128, 1024, 1)
                                             : gmma_desc(sa + cw * (64 * 128) + k * 32, 16, 1024, 1);
                 const uint64_t bdesc = B_MN ? gmma_desc(sb + k * 2048, BK * 128, 1024, 1) : gmma_desc(sb + k * 32, 16, 1024, 1);
-                wgmma_ss<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc, bdesc, (kb != ti.kb0 || k != 0) ? 1u : 0u);
+                wgmma_ss<TN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc, bdesc, (kb != ti.kb0 || k != 0) ? 1u : 0u);
             }
             wgmma_commit();
             wgmma_wait<1>();  // the previous k-block's MMAs retired: its stage may be refilled
@@ -296,7 +329,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
         wgmma_wait<0>();
-        reg_fence<BN / 2>(acc);
+        reg_fence<TN / 2>(acc);
         if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
 
         // ---------------- epilogue: registers -> global ----------------
@@ -305,7 +338,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         const __nv_bfloat16* bias = pr.bias;
         const int N = pr.N;
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
+        for (int j = 0; j < TN / 8; ++j) {
             const int col = col0 + 8 * j;
             if (col >= N) continue;  // N % 8 == 0: the column pair is either wholly in range or wholly out
             float b0 = 0.f, b1 = 0.f;
@@ -347,21 +380,46 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     }
 }
 
-template <bool A_MN, bool B_MN>
+// SMs of the static persistent schedule: worker w takes tiles w, w + W, ... on `SMs - gemm_sm_margin` SMs
+int gemm_workers() {
+    const int sms = dolo_num_sms() - dolo_option_gemm_sm_margin();
+    return sms < 1 ? 1 : sms;
+}
+
+template <bool A_MN, bool B_MN, int TN>
 int launch_gemm(const GemmMaps& maps, const GemmParams& p, cudaStream_t st) {
-    auto kern = gemm_bf16_kernel<A_MN, B_MN>;
+    auto kern = gemm_bf16_kernel<A_MN, B_MN, TN>;
+    constexpr int smem_bytes = Ring<TN>::SMEM_BYTES;
     static bool attr_set = false;  // per instantiation
     if (!attr_set) {
-        DOLO_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+        DOLO_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
         attr_set = true;
     }
-    // static persistent schedule: worker w takes tiles w, w + W, ... on `SMs - gemm_sm_margin` SMs
-    int sms = dolo_num_sms() - dolo_option_gemm_sm_margin();
-    if (sms < 1) sms = 1;
+    const int sms = gemm_workers();
     const int grid = p.num_tiles < sms ? p.num_tiles : sms;
-    kern<<<grid, GEMM_THREADS, SMEM_BYTES, st>>>(maps, p);
+    kern<<<grid, GEMM_THREADS, smem_bytes, st>>>(maps, p);
     DOLO_LAUNCH_OK("gemm_bf16");
     return DOLO_OK;
+}
+
+// Tile width of a dense launch.  The static persistent schedule gives its busiest worker ceil(tiles / workers) tiles, so
+// a launch costs ceil(tiles_w / workers) * c_w.  The 128 x 256 tile moves 25 % fewer operand bytes per FLOP and runs
+// closer to the tensor-core peak (TILE256_COST < 2), but halves the tile count: where it leaves a partly filled last wave
+// that the 128 x 128 tiles fill (a 4096 x 2560 output: 4.85 waves of 128-wide tiles on 132 SMs, 2.42 of 256-wide ones)
+// the narrow tile can win.
+int choose_tile_n(int n, const int64_t* M, const int64_t* N) {
+    const int forced = dolo_option_gemm_tile_n();
+    if (forced != 0) return forced;
+    const int64_t w = gemm_workers();
+    int64_t t128 = 0, t256 = 0;
+    for (int q = 0; q < n; ++q) {
+        const int64_t mb = (M[q] + BM - 1) / BM;
+        t128 += mb * ((N[q] + 127) / 128);
+        t256 += mb * ((N[q] + 255) / 256);
+    }
+    const double c128 = double((t128 + w - 1) / w);
+    const double c256 = double((t256 + w - 1) / w) * TILE256_COST;
+    return c256 < c128 ? 256 : 128;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -577,9 +635,10 @@ struct GemmProblemArgs {
     int64_t M, N, K;
 };
 
-// Fills maps.{a,b}[q] and p.pr[q] for one problem.  All problems of a launch share the operand layouts and the output type.
+// Fills maps.{a,b}[q] and p.pr[q] for one problem.  All problems of a launch share the operand layouts, the output type
+// and the tile width tile_n (128 or 256).
 static int setup_problem(GemmMaps& maps, GemmParams& p, int q, const GemmProblemArgs& g, int a_mn_major, int b_mn_major,
-                         int d_is_f32, const GroupArgs& ga) {
+                         int d_is_f32, const GroupArgs& ga, int tile_n) {
     const int64_t M = g.M, N = g.N, K = g.K;
     DOLO_REQUIRE(K > 0, "gemm: K must be > 0");
     DOLO_REQUIRE(K % 8 == 0 && N % 8 == 0, "gemm: K=%lld and N=%lld must be multiples of 8", (long long)K, (long long)N);
@@ -588,7 +647,7 @@ static int setup_problem(GemmMaps& maps, GemmParams& p, int q, const GemmProblem
     DOLO_REQUIRE(!a_mn_major || M % 8 == 0, "gemm: MN-major A requires M %% 8 == 0");
     DOLO_REQUIRE(g.C == nullptr || g.ldc % (d_is_f32 ? 4 : 8) == 0, "gemm: ldc alignment");
     DOLO_REQUIRE(M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31), "gemm: dimension too large");
-    // K-major: dims {K, rows}, box {64, tile rows}.  MN-major: dims {rows, K}, box {64, 64}.
+    // K-major: dims {K, rows}, box {64, tile rows} (128 for A, tile_n for B).  MN-major: dims {rows, K}, box {64, 64}.
     uint64_t dims[2], strides[2];
     uint32_t box[2];
     int rc;
@@ -613,7 +672,7 @@ static int setup_problem(GemmMaps& maps, GemmParams& p, int q, const GemmProblem
     strides[0] = 2;
     if (!b_mn_major) {
         dims[0] = uint64_t(K); dims[1] = uint64_t(ga.mode == 1 ? ga.b_total_outer : N); strides[1] = uint64_t(g.ldb) * 2;
-        box[0] = BK; box[1] = BN;
+        box[0] = BK; box[1] = uint32_t(tile_n);
     } else {
         dims[0] = uint64_t(N); dims[1] = uint64_t(ga.mode == 1 ? ga.b_total_outer : K); strides[1] = uint64_t(g.ldb) * 2;
         box[0] = 64; box[1] = BK;
@@ -638,7 +697,7 @@ static int setup_problem(GemmMaps& maps, GemmParams& p, int q, const GemmProblem
         pr.hint_b = a_smaller ? TMA_HINT_EVICT_FIRST : TMA_HINT_EVICT_LAST;
     }
     pr.num_m = int((M + BM - 1) / BM);
-    pr.num_n = int((N + BN - 1) / BN);
+    pr.num_n = int((N + tile_n - 1) / tile_n);
     pr.num_kb = int((K + BK - 1) / BK);
     {
         // A panel of group_m x 128 rows x K bf16 should fit comfortably in the 50 MB L2 next to the streaming B tiles
@@ -651,12 +710,17 @@ static int setup_problem(GemmMaps& maps, GemmParams& p, int q, const GemmProblem
     return DOLO_OK;
 }
 
-template <typename... Ts>
-static int dispatch_layout(int a_mn_major, int b_mn_major, Ts&&... args) {
-    if (!a_mn_major && !b_mn_major) return launch_gemm<false, false>(args...);
-    if (!a_mn_major && b_mn_major) return launch_gemm<false, true>(args...);
-    if (a_mn_major && !b_mn_major) return launch_gemm<true, false>(args...);
-    return launch_gemm<true, true>(args...);
+template <int TN>
+static int dispatch_layout(int a_mn_major, int b_mn_major, const GemmMaps& maps, const GemmParams& p, cudaStream_t st) {
+    if (!a_mn_major && !b_mn_major) return launch_gemm<false, false, TN>(maps, p, st);
+    if (!a_mn_major && b_mn_major) return launch_gemm<false, true, TN>(maps, p, st);
+    if (a_mn_major && !b_mn_major) return launch_gemm<true, false, TN>(maps, p, st);
+    return launch_gemm<true, true, TN>(maps, p, st);
+}
+
+static int dispatch(int tile_n, int a_mn_major, int b_mn_major, const GemmMaps& maps, const GemmParams& p, cudaStream_t st) {
+    return tile_n == 256 ? dispatch_layout<256>(a_mn_major, b_mn_major, maps, p, st)
+                         : dispatch_layout<128>(a_mn_major, b_mn_major, maps, p, st);
 }
 
 static int gemm_impl(const void* A, int64_t lda, int a_mn_major, const void* B, int64_t ldb, int b_mn_major, void* D,
@@ -666,11 +730,12 @@ static int gemm_impl(const void* A, int64_t lda, int a_mn_major, const void* B, 
     if (M == 0 || N == 0) return DOLO_OK;
     const bool tma_store = (flags & DOLO_GEMM_FLAG_TMA_STORE) != 0;
     DOLO_REQUIRE(!tma_store || (!d_is_f32 && C == nullptr), "gemm: TMA-store epilogue needs bf16 D and no C");
+    const int tile_n = ga.mode == 0 ? choose_tile_n(1, &M, &N) : BN;
     GemmMaps maps;
     GemmParams p;
     memset(&p, 0, sizeof(p));
     GemmProblemArgs g{A, lda, B, ldb, D, ldd, C, ldc, bias, alpha, beta, M, N, K};
-    int rc = setup_problem(maps, p, 0, g, a_mn_major, b_mn_major, d_is_f32, ga);
+    int rc = setup_problem(maps, p, 0, g, a_mn_major, b_mn_major, d_is_f32, ga, tile_n);
     if (rc) return rc;
     p.n_prob = 1;
     p.pr[0].tile_start = 0;
@@ -683,7 +748,7 @@ static int gemm_impl(const void* A, int64_t lda, int a_mn_major, const void* B, 
     p.group_k_offsets = ga.group_k_offsets;
     p.num_groups = ga.num_groups;
     p.d_group_stride = ga.d_group_stride;
-    return dispatch_layout(a_mn_major, b_mn_major, maps, p, static_cast<cudaStream_t>(stream));
+    return dispatch(tile_n, a_mn_major, b_mn_major, maps, p, static_cast<cudaStream_t>(stream));
 }
 
 // The weight gradients of one transformer block in ONE persistent launch (autograd of linear.py:5-25 for c_attn, attention
@@ -695,15 +760,16 @@ extern "C" int dolomite_b200_gemm_bf16_wgrad_multi(int n_problems, const void* c
                                                    const int64_t* ld_dw, const int64_t* M, const int64_t* N, int64_t K,
                                                    const float* alpha, const int* accumulate, void* stream) {
     DOLO_REQUIRE(n_problems >= 1 && n_problems <= MAXP, "wgrad_multi: between 1 and %d problems per launch", MAXP);
+    for (int q = 0; q < n_problems; ++q) DOLO_REQUIRE(M[q] > 0 && N[q] > 0, "wgrad_multi: empty problem %d", q);
+    const int tile_n = choose_tile_n(n_problems, M, N);
     GemmMaps maps;
     GemmParams p;
     memset(&p, 0, sizeof(p));
     int tiles = 0;
     for (int q = 0; q < n_problems; ++q) {
-        DOLO_REQUIRE(M[q] > 0 && N[q] > 0, "wgrad_multi: empty problem %d", q);
         GemmProblemArgs g{dY[q], ld_dy[q], X[q], ld_x[q], dW[q], ld_dw[q], accumulate[q] ? dW[q] : nullptr, ld_dw[q], nullptr,
                           alpha[q], 1.f, M[q], N[q], K};
-        int rc = setup_problem(maps, p, q, g, 1, 1, 1, GroupArgs());
+        int rc = setup_problem(maps, p, q, g, 1, 1, 1, GroupArgs(), tile_n);
         if (rc) return rc;
         p.pr[q].tile_start = tiles;
         tiles += p.pr[q].num_m * p.pr[q].num_n;
@@ -713,7 +779,16 @@ extern "C" int dolomite_b200_gemm_bf16_wgrad_multi(int n_problems, const void* c
     p.d_is_f32 = 1;
     p.grouped = 0;
     p.num_groups = 1;
-    return launch_gemm<true, true>(maps, p, static_cast<cudaStream_t>(stream));
+    return dispatch(tile_n, 1, 1, maps, p, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int dolomite_b200_gemm_bf16_tile_n(int n_problems, const int64_t* M, const int64_t* N, int* tile_n,
+                                              float* cost_256_over_128) {
+    DOLO_REQUIRE(n_problems >= 1 && n_problems <= MAXP && M != nullptr && N != nullptr && tile_n != nullptr,
+                 "gemm_bf16_tile_n: between 1 and %d problems, non-null M, N and tile_n", MAXP);
+    *tile_n = choose_tile_n(n_problems, M, N);
+    if (cost_256_over_128 != nullptr) *cost_256_over_128 = float(TILE256_COST);
+    return DOLO_OK;
 }
 
 extern "C" int dolomite_b200_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const void* B, int64_t ldb,

@@ -14,6 +14,7 @@
 #define DOLO_F16(i) DOLO_F8(i), DOLO_F8(i + 8)
 #define DOLO_F32(i) DOLO_F16(i), DOLO_F16(i + 16)
 #define DOLO_F64(i) DOLO_F32(i), DOLO_F32(i + 32)
+#define DOLO_F128(i) DOLO_F64(i), DOLO_F64(i + 64)
 
 namespace dolo {
 
@@ -40,6 +41,14 @@ __device__ __forceinline__ void wgmma_ss_n128(float* d, uint64_t da, uint64_t db
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\twgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
                  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}\n"
                  : DOLO_F64(0) : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
+}
+// 128 accumulators per thread: a consumer warpgroup needs more than the 168 registers a 384-thread CTA gets by default
+// (see setmaxnreg_inc in common.cuh)
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_ss_n256(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\twgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, %131, %132;\n\t}\n"
+                 : DOLO_F128(0) : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
 }
 template <int TB>
 __device__ __forceinline__ void wgmma_rs_n16(float* d, const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
@@ -78,11 +87,12 @@ __device__ __forceinline__ void wgmma_fp8_n128(float* d, uint64_t da, uint64_t d
 // N-generic entry points (N must be one of the instantiated widths)
 template <int N, int TA, int TB>
 __device__ __forceinline__ void wgmma_ss(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
-    static_assert(N == 16 || N == 32 || N == 64 || N == 128, "wgmma_ss: unsupported N");
+    static_assert(N == 16 || N == 32 || N == 64 || N == 128 || N == 256, "wgmma_ss: unsupported N");
     if constexpr (N == 16) wgmma_ss_n16<TA, TB>(d, da, db, scale_d);
     else if constexpr (N == 32) wgmma_ss_n32<TA, TB>(d, da, db, scale_d);
     else if constexpr (N == 64) wgmma_ss_n64<TA, TB>(d, da, db, scale_d);
-    else wgmma_ss_n128<TA, TB>(d, da, db, scale_d);
+    else if constexpr (N == 128) wgmma_ss_n128<TA, TB>(d, da, db, scale_d);
+    else wgmma_ss_n256<TA, TB>(d, da, db, scale_d);
 }
 template <int N, int TB>
 __device__ __forceinline__ void wgmma_rs(float* d, const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {

@@ -390,6 +390,18 @@ def gemm_wgrad_multi(problems: list[tuple], n_rows: int | None = None) -> None:
         gemm_timer.append((sum(2.0 * K * q[0].shape[1] * q[1].shape[1] for q in problems), e0, e1))
 
 
+def gemm_tile_n(shapes: list[tuple[int, int]]) -> tuple[int, float]:
+    """output tile width (128 | 256) of a dense gemm / gemm_wgrad_multi launch over these (M, N) outputs on the current
+    device, and the per-tile cost ratio c_256 / c_128 of the automatic choice"""
+    import ctypes
+
+    n = len(shapes)
+    tile_n, cost = ctypes.c_int(0), ctypes.c_float(0.0)
+    _lib.call("dolomite_b200_gemm_bf16_tile_n", n, (ctypes.c_int64 * n)(*[s[0] for s in shapes]),
+              (ctypes.c_int64 * n)(*[s[1] for s in shapes]), ctypes.addressof(tile_n), ctypes.addressof(cost))
+    return int(tile_n.value), float(cost.value)
+
+
 # ------------------------------------------------------------------------------------------------
 # FP8 (te.Linear under te.fp8_autocast with DelayedScaling, HYBRID: e4m3 forward, e5m2 output gradients)
 # ------------------------------------------------------------------------------------------------

@@ -43,6 +43,9 @@ int dolomite_b200_device_info(int* sm_count, int* cc_major, int* cc_minor);
  *   "attn_head_fastest" heads per chunk of the attention CTA order (default 8: inside a chunk heads fastest + longest tiles
  *                      first, so that the last wave is short tiles; 0 = tiles fastest)
  *   "gemm_l2_hints"    1 | 0 (long-contraction GEMMs load the streamed operand evict-first and the re-used one evict-last)
+ *   "gemm_tile_n"      0 (default) | 128 | 256: output tile width of the dense bf16 GEMMs (gemm_bf16 without split-K and
+ *                      gemm_bf16_wgrad_multi); 0 chooses per launch (dolomite_b200_gemm_bf16_tile_n), 128 / 256 force a
+ *                      width (diagnostics and tests; both widths give bit-identical results)
  * Accepted and reported back, but without effect on sm_90 (one kernel per job): "gemm_cta_pair", "gemm_dynamic",
  * "gemm_f32_tma_epilogue", "attn_fwd_split", "attn_bwd_variant", "attn_bwd_ablate". */
 int dolomite_b200_set_option(const char* key, int value);
@@ -231,6 +234,14 @@ int dolomite_b200_gemm_bf16_wgrad_multi(int n_problems, const void* const* dY, c
                                         const int64_t* ld_x, float* const* dW, const int64_t* ld_dw, const int64_t* M,
                                         const int64_t* N, int64_t K, const float* alpha, const int* accumulate,
                                         void* stream);
+
+/* Output tile width (128 or 256 columns, 128 rows) that a dense launch of gemm_bf16 (without split-K) or
+ * gemm_bf16_wgrad_multi over these problems takes on the current device, under the current gemm_tile_n and
+ * gemm_sm_margin options.  Automatic choice: the wider tile unless its last, partly filled wave makes the launch slower,
+ * i.e. 256 iff ceil(tiles_256 / SMs) * cost_256_over_128 < ceil(tiles_128 / SMs), tiles summed over the problems.
+ * *cost_256_over_128 (may be NULL) receives the constant of that rule: the time of one 128x256 tile over one 128x128 tile. */
+int dolomite_b200_gemm_bf16_tile_n(int n_problems, const int64_t* M, const int64_t* N, int* tile_n,
+                                   float* cost_256_over_128);
 
 /* ------------------------------------------------------------------------------------------------
  * FP8 linear layers with delayed scaling: what TransformerEngine's te.Linear computes inside

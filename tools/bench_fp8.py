@@ -22,11 +22,21 @@ from contextlib import nullcontext
 
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))  # the repository root (bench.py)
 
 from dolomite_engine_b200 import kernels as K  # noqa: E402
 
-C2 = {"c_attn": (3072, 2048), "attn.c_proj": (2048, 2048), "c_fc": (16384, 2048), "mlp.c_proj": (2048, 8192)}  # (N, K)
+
+
+def c2_block_shapes() -> dict:
+    """{linear: (N, K)} of a C2 block, from the flagship benchmark's model configuration"""
+    import bench
+
+    cfg = bench.model_config("c2")
+    H, F, nh = cfg["n_embd"], cfg["n_inner"], cfg["n_head"]
+    kv = {"mha": nh, "mqa": 1}.get(cfg["attention_head_type"], cfg.get("num_key_value_heads") or nh)
+    fc = 2 * F if cfg["activation_function"].endswith("glu") else F
+    return {"c_attn": (H + 2 * kv * (H // nh), H), "attn.c_proj": (H, H), "c_fc": (fc, H), "mlp.c_proj": (H, F)}
 
 
 def _card() -> dict:
@@ -114,7 +124,7 @@ def main() -> None:
     if a.train_steps:
         res["train_step_c2"] = train_steps(a.train_steps, a.rounds)
     res["shapes"] = {}
-    for name, (N, Kd) in C2.items():
+    for name, (N, Kd) in c2_block_shapes().items():
         x = torch.randn(T, Kd, device="cuda", generator=g).to(torch.bfloat16)
         w = (torch.randn(N, Kd, device="cuda", generator=g) * 0.02).to(torch.bfloat16)
         dy = (torch.randn(T, N, device="cuda", generator=g) * 1e-3).to(torch.bfloat16)
