@@ -133,6 +133,20 @@ __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
+// ---------------- 8x8 b16 matrix moves (the register layout of an m64nNk16 accumulator's bf16 pairs) ----------------
+// Lane t names row t % 8 of matrix t / 8; register i holds, for matrix i, row lane / 4, columns 2 (lane % 4) and +1.
+__device__ __forceinline__ void stmatrix_x4(uint32_t saddr, const uint32_t (&r)[4]) {
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(r[0]), "r"(r[1]),
+                 "r"(r[2]), "r"(r[3])
+                 : "memory");
+}
+__device__ __forceinline__ void ldmatrix_x4(uint32_t saddr, uint32_t (&r)[4]) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+                 : "r"(saddr)
+                 : "memory");
+}
+
 // ---------------- TMA ----------------
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");

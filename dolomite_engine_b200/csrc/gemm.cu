@@ -1,6 +1,6 @@
 // bf16 GEMM for sm_90a (H100):  TMA (cp.async.bulk.tensor) -> 128B-swizzled smem ring -> wgmma (m64n128k16 or
-// m64n256k16 per consumer warpgroup, fp32 accumulators in registers) -> epilogue straight from the registers
-// (alpha / bias / beta*C, bf16 | fp32).
+// m64n256k16 per consumer warpgroup, fp32 accumulators in registers) -> epilogue (alpha / bias / beta*C, bf16 | fp32)
+// through double-buffered shared-memory slabs -> asynchronous TMA stores.
 //
 // Persistent, warp-specialised: warpgroup 0 = producer (one elected thread issues the TMA loads; the whole first warp for
 // gather-on-load), warpgroups 1 and 2 = consumers, each owning 64 rows of the output tile.  The tile is 128 x 128 (six
@@ -32,14 +32,26 @@ constexpr int GEMM_THREADS = 384;  // warpgroup 0 producer, 1..2 consumers
 constexpr int SMEM_BYTES = 1024 /*align slack*/ + STAGES * STAGE_BYTES + 256 /*barriers*/;
 static_assert(SMEM_BYTES <= 232448, "shared memory budget exceeded (227 KB per block on sm_90)");
 
-// Stage ring of the bf16 kernel per output tile width TN: 128 x 128 keeps six 32 KB stages, 128 x 256 four 48 KB stages.
+// Epilogue staging of the bf16 kernel: each consumer warpgroup owns two slabs of 64 rows x 128 B (64 bf16 or 32 fp32
+// columns, 128B-swizzled like the D / C tensor maps) and a copy of the tile's bias slice (up to 256 bf16).
+constexpr int EPI_SLAB_BYTES = 64 * 128;
+constexpr int EPI_BYTES = 2 /*warpgroups*/ * 2 /*slabs*/ * EPI_SLAB_BYTES;
+constexpr int EPI_BIAS_BYTES = 2 /*warpgroups*/ * 256 * 2;
+
+// Shared memory of the bf16 kernel per output tile width TN: the stage ring (128 x 128 keeps six 32 KB stages, 128 x 256
+// four 48 KB stages), then the epilogue slabs, the bias slices and the barriers.
 template <int TN>
 struct Ring {
     static_assert(TN == 128 || TN == 256, "tile width 128 or 256");
     static constexpr int STAGES = TN == 256 ? 4 : 6;
     static constexpr int B_BYTES = TN * BK * 2;
     static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_BYTES;
-    static constexpr int SMEM_BYTES = 1024 /*align slack*/ + STAGES * STAGE_BYTES + 256 /*barriers*/;
+    static constexpr int EPI_OFFSET = STAGES * STAGE_BYTES;  // a multiple of 1024: the slabs keep the swizzle alignment
+    static constexpr int BIAS_OFFSET = EPI_OFFSET + EPI_BYTES;
+    static constexpr int BAR_OFFSET = BIAS_OFFSET + EPI_BIAS_BYTES;
+    static constexpr int SMEM_BYTES = 1024 /*align slack*/ + BAR_OFFSET + 256 /*barriers*/;
+    static_assert(EPI_OFFSET % 1024 == 0, "epilogue slabs must stay 1024-byte aligned");
+    static_assert((2 * STAGES + 4) * 8 <= 256, "barrier area");
     static_assert(SMEM_BYTES <= 232448, "shared memory budget exceeded (227 KB per block on sm_90)");
 };
 
@@ -50,15 +62,18 @@ constexpr int CONSUMER_REGS = 232;
 static_assert(PRODUCER_REGS * 128 + 2 * CONSUMER_REGS * 128 <= 65536, "register file exceeded");
 
 // Time of one 128 x 256 tile over one 128 x 128 tile of the same K (see choose_tile_n): the median over the twelve bf16
-// GEMM launches of a C2 training step, measured by tools/bench_gemm.py on an H100 80GB HBM3 at a 700 W power limit
-// (per launch 1.47 .. 1.87; the launches that fill their waves at both widths give 1.63 .. 1.87).  Every value in
-// (5/3, 1.875) makes the same choices at C2: 128 for the 4096 x 2560 outputs, 256 for all the others.
-constexpr double TILE256_COST = 1.81;
+// GEMM launches of a C2 training step in two passes of tools/bench_gemm.py on an H100 80GB HBM3 at a 400 W power limit
+// (per launch 1.26 .. 1.85).  The shared-memory epilogue removed most of the fixed cost per tile, which weighed more on
+// the 128 x 256 tile, so the ratio fell from 1.81.  Every value below 5/3 makes the same choice at C2: 256 for every
+// launch, including the 4096 x 2560 outputs (3 waves against 5); a whole C2 step confirms that choice.
+constexpr double TILE256_COST = 1.65;
 
 constexpr int MAXP = 4;  // problems per launch (the four weight gradients of a transformer block share one launch)
 
+// d / c: rank-3 maps {N, M, groups} of D and C with a box of one epilogue slab {128 B of columns, 64 rows, 1} (bf16 kernel
+// only; the group dimension is 1 except for the K-grouped expert weight gradients)
 struct GemmMaps {
-    CUtensorMap a[MAXP], b[MAXP];
+    CUtensorMap a[MAXP], b[MAXP], d[MAXP], c[MAXP];
 };
 
 struct Problem {
@@ -83,7 +98,7 @@ struct GemmParams {
     //   1 = M-grouped: every 128-row tile of A/D belongs to one group (m_tile_group[m_blk], -1 = unused tile); B's outer
     //       TMA coordinate is offset by group * b_group_rows (fwd / dgrad of the expert linears)
     //   2 = K-grouped: tile index also enumerates the group; the contraction runs over rows
-    //       [group_k_offsets[g], group_k_offsets[g+1]) and D/C are offset by g * d_group_stride (expert wgrad)
+    //       [group_k_offsets[g], group_k_offsets[g+1]) and D/C are slice g of their rank-3 maps (expert wgrad)
     int grouped;
     const int* m_tile_group;
     const int* a_row_index;  // gather-on-load: source row of A for every (grouped) row of the problem, or NULL
@@ -93,7 +108,6 @@ struct GemmParams {
     int b_group_rows;
     const int* group_k_offsets;
     int num_groups;
-    int64_t d_group_stride;
 };
 
 struct TileInfo {
@@ -128,7 +142,7 @@ __device__ __forceinline__ TileInfo tile_info(int t, const GemmParams& p) {
     ti.kb1 = pr.num_kb;
     ti.valid = true;
     if (p.grouped == 3) {
-        // split-K: tile index also enumerates the K split; partial products are reduced with fp32 atomics
+        // split-K: tile index also enumerates the K split; partial products are reduce-added (TMA, fp32)
         const int per = pr.num_m * pr.num_n;
         const int split = t / per;
         tile_coords(t - split * per, pr.num_m, pr.num_n, pr.group_m, ti.m_blk, ti.n_blk);
@@ -153,6 +167,162 @@ __device__ __forceinline__ TileInfo tile_info(int t, const GemmParams& p) {
     return ti;
 }
 
+// Epilogue state of one consumer warpgroup.  Its 64 rows of the tile leave in chunks of one slab (64 bf16 or 32 fp32
+// columns), alternating between its two slabs.  A slab is rewritten only after the store that last read it has finished
+// reading.  Chunks 0 and 1 of a tile reuse slabs whose stores were issued before the tile's mainloop (begin_tile), so
+// they never wait; chunks 2 and up (128 x 256 bf16, fp32) wait for the store of the chunk two back, while the previous
+// chunk's store stays in flight.  The stores of a tile's last chunks run on during the next tile's mainloop.  C, when
+// present, is TMA-loaded into the slab that then receives the result: chunks 0 and 1 during the mainloop
+// (load_c_prefetch), later ones when their slab comes free.
+struct Epilogue {
+    uint8_t* slabs;         // [2][EPI_SLAB_BYTES]
+    uint32_t* bias;         // [TN / 2] bf16 pairs of the tile's bias slice
+    uint64_t* c_bar;        // [2] C arrival per slab
+    int slab = 0;           // slab of the next chunk
+    uint32_t c_phase = 0;   // bit s: parity of the next wait on c_bar[s]
+    int cw;                 // consumer warpgroup: named barrier 1 + cw
+    bool leader;            // thread 0 of the warpgroup: issues the TMA traffic and owns its bulk async-groups
+
+    // C of chunks 0 and 1 of the tile (row0, col0), once the previous tile's stores have read both slabs
+    __device__ __forceinline__ void load_c_prefetch(const CUtensorMap* cmap, int chunk_cols, int col0, int row0, int grp) {
+        tma_store_wait_read<0>();
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const int s = slab ^ i;
+            mbar_expect_tx(&c_bar[s], EPI_SLAB_BYTES);
+            tma_load_3d(slabs + s * EPI_SLAB_BYTES, cmap, &c_bar[s], col0 + i * chunk_cols, row0, grp);
+        }
+    }
+
+    // after the tile's mainloop: the previous tile's stores have read both slabs (they were issued a mainloop ago), and
+    // the barrier also publishes the tile's bias slice
+    __device__ __forceinline__ void begin_tile() {
+        if (leader) tma_store_wait_read<0>();
+        named_bar_sync(1 + cw, 128);
+    }
+
+    // chunk ch >= 2 goes to the slab of chunk ch - 2: wait until that chunk's store has read it (the store of chunk
+    // ch - 1 may stay in flight); the leader then TMA-loads the chunk's C into it if there is one
+    __device__ __forceinline__ void reuse_slab(bool has_c, const CUtensorMap* cmap, int col, int row0, int grp) {
+        if (leader) {
+            tma_store_wait_read<1>();
+            if (has_c) {
+                mbar_expect_tx(&c_bar[slab], EPI_SLAB_BYTES);
+                tma_load_3d(slabs + slab * EPI_SLAB_BYTES, cmap, &c_bar[slab], col, row0, grp);
+            }
+        }
+        named_bar_sync(1 + cw, 128);
+    }
+
+    // D tile (row0, col0) of group grp = (acc + bias) * alpha (+ beta * C), written (or reduce-added) through the slabs.
+    // The fp32 expression and its order are those of a plain register epilogue, so results do not depend on the path.
+    template <int TN, bool F32>
+    __device__ __forceinline__ void store(const float (&acc)[TN / 2], const CUtensorMap* dmap, const CUtensorMap* cmap,
+                                          int col0, int row0, int grp, float alpha, float beta, bool has_bias, bool has_c,
+                                          bool reduce) {
+        constexpr int CHUNK = F32 ? 32 : 64;  // columns of one slab
+        constexpr int NB = CHUNK / 8;         // n8 accumulator blocks per slab
+        const int lane = threadIdx.x & 31;
+        const int wrow = ((threadIdx.x >> 5) & 3) * 16;  // this warp's first row inside the warpgroup's 64
+#pragma unroll
+        for (int ch = 0; ch < TN / CHUNK; ++ch) {
+            uint8_t* sl = slabs + slab * EPI_SLAB_BYTES;
+            if (ch >= 2) reuse_slab(has_c, cmap, col0 + ch * CHUNK, row0, grp);
+            if (has_c) {
+                mbar_wait(&c_bar[slab], (c_phase >> slab) & 1u, 4);
+                c_phase ^= 1u << slab;
+            }
+            if constexpr (F32) {
+                // thread: rows lane / 4 (+8) of its warp, columns 2 (lane % 4) (+1) of each n8 block; 128B swizzle:
+                // 16-byte unit u of slab row r lives at unit u ^ (r % 8)
+#pragma unroll
+                for (int jj = 0; jj < NB; ++jj) {
+                    const int j = ch * NB + jj;
+                    float b0 = 0.f, b1 = 0.f;
+                    if (has_bias) {
+                        const uint32_t bv = bias[4 * j + (lane & 3)];
+                        b0 = bf16_lo(bv);
+                        b1 = bf16_hi(bv);
+                    }
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int r = wrow + 8 * h + (lane >> 2);
+                        const int byte = jj * 32 + (lane & 3) * 8;
+                        float2* s = reinterpret_cast<float2*>(sl + r * 128 + ((((byte >> 4) ^ (r & 7)) << 4) | (byte & 15)));
+                        float v0 = (acc[4 * j + 2 * h] + b0) * alpha;
+                        float v1 = (acc[4 * j + 2 * h + 1] + b1) * alpha;
+                        if (has_c) {
+                            const float2 c2 = *s;
+                            v0 += beta * c2.x;
+                            v1 += beta * c2.y;
+                        }
+                        *s = make_float2(v0, v1);
+                    }
+                }
+            } else {
+                // one x4 matrix move per pair of n8 blocks: matrix m = lane / 8 is n8 block jj + m / 2, rows 8 (m % 2) ..+7
+                const int m = lane >> 3;
+                const int r = wrow + 8 * (m & 1) + (lane & 7);
+#pragma unroll
+                for (int jj = 0; jj < NB; jj += 2) {
+                    const uint32_t addr = smem_u32(sl + r * 128 + (((jj + (m >> 1)) ^ (lane & 7)) << 4));
+                    uint32_t cv[4], out[4];
+                    if (has_c) ldmatrix_x4(addr, cv);
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        const int j = ch * NB + jj + (i >> 1), h = i & 1;
+                        float b0 = 0.f, b1 = 0.f;
+                        if (has_bias) {
+                            const uint32_t bv = bias[4 * j + (lane & 3)];
+                            b0 = bf16_lo(bv);
+                            b1 = bf16_hi(bv);
+                        }
+                        float v0 = (acc[4 * j + 2 * h] + b0) * alpha;
+                        float v1 = (acc[4 * j + 2 * h + 1] + b1) * alpha;
+                        if (has_c) {
+                            v0 += beta * bf16_lo(cv[i]);
+                            v1 += beta * bf16_hi(cv[i]);
+                        }
+                        out[i] = pack_bf16(v0, v1);
+                    }
+                    stmatrix_x4(addr, out);
+                }
+            }
+            issue(dmap, col0 + ch * CHUNK, row0, grp, reduce);
+        }
+    }
+
+    // zero D tile of an fp32 launch, stored from zeroed slabs
+    template <int TN>
+    __device__ __forceinline__ void store_zero_f32(const CUtensorMap* dmap, int col0, int row0, int grp) {
+        begin_tile();
+#pragma unroll 1
+        for (int ch = 0; ch < TN / 32; ++ch) {
+            if (ch >= 2) reuse_slab(false, nullptr, 0, 0, 0);
+            uint4* s = reinterpret_cast<uint4*>(slabs + slab * EPI_SLAB_BYTES);
+#pragma unroll
+            for (int i = 0; i < EPI_SLAB_BYTES / 16 / 128; ++i) s[(threadIdx.x & 127) + 128 * i] = make_uint4(0u, 0u, 0u, 0u);
+            issue(dmap, col0 + ch * 32, row0, grp, false);
+        }
+    }
+
+    // the current slab is written: the leader stores (or reduce-adds) it to the chunk at (col, row0) and moves on to
+    // the other slab.  D's tensor map clips the M and N tails.
+    __device__ __forceinline__ void issue(const CUtensorMap* dmap, int col, int row0, int grp, bool reduce) {
+        const uint8_t* sl = slabs + slab * EPI_SLAB_BYTES;
+        fence_proxy_async_smem();  // the slab's writes -> visible to the TMA store (async proxy)
+        named_bar_sync(1 + cw, 128);
+        if (leader) {
+            if (reduce)
+                tma_reduce_add_3d(dmap, sl, col, row0, grp);
+            else
+                tma_store_3d(dmap, sl, col, row0, grp);
+            tma_store_commit();
+        }
+        slab ^= 1;
+    }
+};
+
 // TN: output tile width.  The 128 x 256 tile runs dense launches only (grouped == 0, no gather), because the grouped
 // modes' tile tables are per 128 x 128 tile.
 template <bool A_MN, bool B_MN, int TN>
@@ -165,9 +335,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     uint8_t* smem = smem_align_1024(smem_raw);
     uint8_t* smem_a = smem;
     uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
-    uint64_t* full_bar = bars;            // [STAGES]
-    uint64_t* empty_bar = bars + STAGES;  // [STAGES]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Ring<TN>::BAR_OFFSET);
+    uint64_t* full_bar = bars;                 // [STAGES]
+    uint64_t* empty_bar = bars + STAGES;       // [STAGES]
+    uint64_t* c_bar = bars + 2 * STAGES;       // [2 consumer warpgroups][2 slabs]
 
     const int wg = threadIdx.x >> 7;
     const int warp = threadIdx.x >> 5;
@@ -185,6 +356,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
             mbar_init(&full_bar[i], gather ? 33 : 1);
             mbar_init(&empty_bar[i], 8);  // one arrive per consumer warp
         }
+        for (int i = 0; i < 4; ++i) mbar_init(&c_bar[i], 1);
         mbar_fence_init();
     }
     __syncthreads();
@@ -279,32 +451,35 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     // ================= consumers: warpgroup cw owns rows [64 cw, 64 cw + 64) of the tile =================
     if constexpr (TN == 256) setmaxnreg_inc<CONSUMER_REGS>();
     const int cw = wg - 1;
-    const int wr = (warp & 3) * 16 + (lane >> 2);  // accumulator row of this thread inside the warpgroup (and +8)
-    const int wc = 2 * (lane & 3);                 // first accumulator column inside each n8 block
+    const int wt = threadIdx.x & 127;  // thread inside the warpgroup
+    Epilogue epi;
+    epi.slabs = smem + Ring<TN>::EPI_OFFSET + cw * 2 * EPI_SLAB_BYTES;
+    epi.bias = reinterpret_cast<uint32_t*>(smem + Ring<TN>::BIAS_OFFSET + cw * (EPI_BIAS_BYTES / 2));
+    epi.c_bar = c_bar + 2 * cw;
+    epi.cw = cw;
+    epi.leader = wt == 0;
+    const int chunk_cols = p.d_is_f32 ? 32 : 64;
     int stage = 0;
     uint32_t phase = 0;
     float acc[TN / 2];
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
         const TileInfo ti = tile_info(t, p);
         const Problem& pr = p.pr[ti.q];
-        const int64_t row0 = int64_t(ti.m_blk) * BM + cw * 64 + wr;
-        const int col0 = ti.n_blk * TN + wc;
+        const int row0 = ti.m_blk * BM + cw * 64;  // first row of this warpgroup's 64
+        const int col0 = ti.n_blk * TN;
+        const int dgrp = p.grouped == 2 ? ti.grp : 0;
+        // K-grouped launch (expert weight gradients) and this expert received NO rows: its product is zero.  A launch that
+        // OVERWRITES (beta = 0, no C) must still write the tile -- the caller did not clear the buffer.
         if (!ti.valid) {
-            // K-grouped launch (expert weight gradients) and this expert received NO rows: its product is zero.  A launch
-            // that OVERWRITES (beta = 0, no C) must still write the tile -- the caller did not clear the buffer.
-            if (p.grouped == 2 && p.d_is_f32 && pr.C == nullptr) {
-                float* D = static_cast<float*>(pr.D) + int64_t(ti.grp) * p.d_group_stride;
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int64_t row = row0 + 8 * h;
-                    if (row >= pr.M) continue;
-                    for (int j = 0; j < TN / 8; ++j)
-                        if (col0 + 8 * j < pr.N)
-                            *reinterpret_cast<float2*>(D + row * pr.ldd + col0 + 8 * j) = make_float2(0.f, 0.f);
-                }
-            }
+            if (p.grouped == 2 && p.d_is_f32 && pr.C == nullptr) epi.store_zero_f32<TN>(&maps.d[ti.q], col0, row0, dgrp);
             continue;
         }
+        const bool has_bias = pr.bias != nullptr;
+        const bool has_c = pr.C != nullptr;
+        // the tile's bias slice: loaded now, kept in shared memory for the epilogue
+        uint32_t bias_v = 0;
+        if (has_bias && wt < TN / 2 && col0 + 2 * wt < pr.N)
+            bias_v = __ldg(reinterpret_cast<const uint32_t*>(pr.bias + col0 + 2 * wt));
         int prev_stage = -1;
         for (int kb = ti.kb0; kb < ti.kb1; ++kb) {
             mbar_wait(&full_bar[stage], phase, 3);
@@ -319,10 +494,14 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
                 // this warpgroup's 64 rows are the cw-th chunk.
                 const uint64_t adesc = A_MN ? gmma_desc(sa + cw * (BK * 128) + k * 2048, BK * 128, 1024, 1)
                                             : gmma_desc(sa + cw * (64 * 128) + k * 32, 16, 1024, 1);
-                const uint64_t bdesc = B_MN ? gmma_desc(sb + k * 2048, BK * 128, 1024, 1) : gmma_desc(sb + k * 32, 16, 1024, 1);
+                const uint64_t bdesc = B_MN ? gmma_desc(sb + k * 2048, BK * 128, 1024, 1)
+                                            : gmma_desc(sb + k * 32, 16, 1024, 1);
                 wgmma_ss<TN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc, bdesc, (kb != ti.kb0 || k != 0) ? 1u : 0u);
             }
             wgmma_commit();
+            // C of the tile's first two chunks: the load overlaps the rest of the mainloop.  Two k-blocks in, the
+            // previous tile's last stores have long read their slabs, so the leader does not hold up the MMAs.
+            if (kb == min(ti.kb0 + 2, ti.kb1 - 1) && has_c && epi.leader) epi.load_c_prefetch(&maps.c[ti.q], chunk_cols, col0, row0, dgrp);
             wgmma_wait<1>();  // the previous k-block's MMAs retired: its stage may be refilled
             if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
             prev_stage = stage;
@@ -331,53 +510,19 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         wgmma_wait<0>();
         reg_fence<TN / 2>(acc);
         if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+        // the previous tile's epilogue has finished reading the bias slice: its last chunk ended in a barrier
+        if (has_bias && wt < TN / 2) epi.bias[wt] = bias_v;
+        epi.begin_tile();
 
-        // ---------------- epilogue: registers -> global ----------------
-        const int64_t d_off = (p.grouped == 2) ? int64_t(ti.grp) * p.d_group_stride : 0;
-        const float alpha = pr.alpha, beta = pr.beta;
-        const __nv_bfloat16* bias = pr.bias;
-        const int N = pr.N;
-#pragma unroll
-        for (int j = 0; j < TN / 8; ++j) {
-            const int col = col0 + 8 * j;
-            if (col >= N) continue;  // N % 8 == 0: the column pair is either wholly in range or wholly out
-            float b0 = 0.f, b1 = 0.f;
-            if (bias != nullptr) {
-                const uint32_t bv = *reinterpret_cast<const uint32_t*>(bias + col);
-                b0 = bf16_lo(bv);
-                b1 = bf16_hi(bv);
-            }
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int64_t row = row0 + 8 * h;
-                if (row >= pr.M) continue;
-                float v0 = (acc[4 * j + 2 * h] + b0) * alpha;
-                float v1 = (acc[4 * j + 2 * h + 1] + b1) * alpha;
-                if (p.d_is_f32) {
-                    float* d = static_cast<float*>(pr.D) + d_off + row * pr.ldd + col;
-                    if (p.grouped == 3) {  // split-K partial: D += v
-                        asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(d), "f"(v0), "f"(v1) : "memory");
-                        continue;
-                    }
-                    if (pr.C) {
-                        const float2 c2 = *reinterpret_cast<const float2*>(static_cast<const float*>(pr.C) + d_off + row * pr.ldc + col);
-                        v0 += beta * c2.x;
-                        v1 += beta * c2.y;
-                    }
-                    *reinterpret_cast<float2*>(d) = make_float2(v0, v1);
-                } else {
-                    __nv_bfloat16* d = static_cast<__nv_bfloat16*>(pr.D) + d_off + row * pr.ldd + col;
-                    if (pr.C) {
-                        const uint32_t cv =
-                            *reinterpret_cast<const uint32_t*>(static_cast<const __nv_bfloat16*>(pr.C) + d_off + row * pr.ldc + col);
-                        v0 += beta * bf16_lo(cv);
-                        v1 += beta * bf16_hi(cv);
-                    }
-                    *reinterpret_cast<uint32_t*>(d) = pack_bf16(v0, v1);
-                }
-            }
-        }
+        // ---------------- epilogue: registers -> shared-memory slabs -> TMA ----------------
+        if (p.d_is_f32)
+            epi.store<TN, true>(acc, &maps.d[ti.q], &maps.c[ti.q], col0, row0, dgrp, pr.alpha, pr.beta, has_bias, has_c,
+                                p.grouped == 3);
+        else
+            epi.store<TN, false>(acc, &maps.d[ti.q], &maps.c[ti.q], col0, row0, dgrp, pr.alpha, pr.beta, has_bias, has_c,
+                                 false);
     }
+    if (epi.leader) tma_store_wait_all<0>();  // the slabs must outlive the stores that read them
 }
 
 // SMs of the static persistent schedule: worker w takes tiles w, w + W, ... on `SMs - gemm_sm_margin` SMs
@@ -405,8 +550,8 @@ int launch_gemm(const GemmMaps& maps, const GemmParams& p, cudaStream_t st) {
 // Tile width of a dense launch.  The static persistent schedule gives its busiest worker ceil(tiles / workers) tiles, so
 // a launch costs ceil(tiles_w / workers) * c_w.  The 128 x 256 tile moves 25 % fewer operand bytes per FLOP and runs
 // closer to the tensor-core peak (TILE256_COST < 2), but halves the tile count: where it leaves a partly filled last wave
-// that the 128 x 128 tiles fill (a 4096 x 2560 output: 4.85 waves of 128-wide tiles on 132 SMs, 2.42 of 256-wide ones)
-// the narrow tile can win.
+// that the 128 x 128 tiles fill, the narrow tile can win (a 4096 x 2560 output: 4.85 waves of 128-wide tiles on 132 SMs,
+// 2.42 of 256-wide ones, so 128 wins iff TILE256_COST > 5/3).
 int choose_tile_n(int n, const int64_t* M, const int64_t* N) {
     const int forced = dolo_option_gemm_tile_n();
     if (forced != 0) return forced;
@@ -679,6 +824,24 @@ static int setup_problem(GemmMaps& maps, GemmParams& p, int q, const GemmProblem
     }
     rc = dolo_make_tmap(&maps.b[q], g.B, 2, 2, dims, strides, box, DOLO_SW_128);
     if (rc) return rc;
+    {
+        // D and C: dims {N, M, groups}, box = one epilogue slab {128 B of columns, 64 rows, 1}
+        const uint64_t eb = d_is_f32 ? 4 : 2;
+        const int64_t groups = ga.mode == 2 ? ga.num_groups : 1;
+        const int64_t group_stride = ga.mode == 2 ? ga.d_group_stride : M * g.ldd;
+        uint64_t ddims[3] = {uint64_t(N), uint64_t(M), uint64_t(groups)};
+        uint64_t dstrides[3] = {eb, uint64_t(g.ldd) * eb, uint64_t(group_stride) * eb};
+        const uint32_t dbox[3] = {uint32_t(128 / eb), 64, 1};
+        rc = dolo_make_tmap(&maps.d[q], g.D, int(eb), 3, ddims, dstrides, dbox, DOLO_SW_128);
+        if (rc) return rc;
+        if (g.C != nullptr) {
+            // C: D's dims with C's row stride (the K-grouped mode passes C == D)
+            dstrides[1] = uint64_t(g.ldc) * eb;
+            if (ga.mode != 2) dstrides[2] = uint64_t(M * g.ldc) * eb;
+            rc = dolo_make_tmap(&maps.c[q], g.C, int(eb), 3, ddims, dstrides, dbox, DOLO_SW_128);
+            if (rc) return rc;
+        }
+    }
     Problem& pr = p.pr[q];
     pr.D = g.D;
     pr.C = g.C;
@@ -747,7 +910,6 @@ static int gemm_impl(const void* A, int64_t lda, int a_mn_major, const void* B, 
     p.b_group_rows = int(ga.b_group_rows);
     p.group_k_offsets = ga.group_k_offsets;
     p.num_groups = ga.num_groups;
-    p.d_group_stride = ga.d_group_stride;
     return dispatch(tile_n, a_mn_major, b_mn_major, maps, p, static_cast<cudaStream_t>(stream));
 }
 
@@ -796,7 +958,7 @@ extern "C" int dolomite_b200_gemm_bf16(const void* A, int64_t lda, int a_mn_majo
                                        float alpha, float beta, const void* bias, int64_t M, int64_t N, int64_t K,
                                        int flags, void* stream) {
     if (flags & DOLO_GEMM_FLAG_SPLITK_ACCUMULATE) {
-        // D(fp32) += alpha * A B^T with the contraction split over several CTAs (fp32 vector atomics): removes the
+        // D(fp32) += alpha * A B^T with the contraction split over several CTAs (TMA fp32 reduce-adds): removes the
         // wave-quantisation tail of weight-gradient GEMMs (few output tiles, long K) and the read of C
         DOLO_REQUIRE(d_is_f32 && bias == nullptr && (C == nullptr || (C == D && beta == 1.f)),
                      "gemm: split-K accumulate needs fp32 D, no bias and C == D with beta == 1");

@@ -210,17 +210,19 @@ int dolomite_b200_attn_decode(const void* qkv, int64_t row_stride, const void* k
  *   B is logical [N,K]: b_mn_major == 0 -> stored row-major [N,K] (ld = ldb);  1 -> stored [K,N] (ld = ldb).
  *   D/C: row-major [M,N]; d_is_f32 selects fp32 (else bf16) for BOTH D and C.  C may be NULL (beta ignored)
  *   or alias D.  bias: bf16 [N] or NULL.   K % 8 == 0, lds % 8 == 0, 16-byte aligned bases.
- *   flags: bit0 = the caller promises bf16 D and no C (checked); the epilogue always stores from the registers.
+ *   flags: bit0 = the caller promises bf16 D and no C (checked).  With or without it, every launch stages its output
+ *   tiles in shared memory and writes them with TMA stores (reduce-adds for split-K), so D and C need 16-byte aligned
+ *   bases and row strides.
  * ------------------------------------------------------------------------------------------------ */
 #define DOLO_GEMM_FLAG_TMA_STORE 1
-/* bit1: D(fp32) += alpha*A.B^T with split-K + fp32 vector atomics (weight gradients); C must be NULL or alias D with
+/* bit1: D(fp32) += alpha*A.B^T with split-K + TMA fp32 reduce-adds (weight gradients); C must be NULL or alias D with
  * beta == 1, bias NULL.  Summation order over K splits is not deterministic (like FSDP's own reduce order). */
 #define DOLO_GEMM_FLAG_SPLITK_ACCUMULATE 2
 /* bit2 / bit3: force / forbid a CTA-pair kernel: accepted, no effect on sm_90 (no paired MMA). */
 #define DOLO_GEMM_FLAG_CTA_PAIR 4
 #define DOLO_GEMM_FLAG_NO_CTA_PAIR 8
-/* bit4 / bit5: epilogue selection of other GPU generations: accepted, no effect on sm_90 (fp32 D is stored from the
- * registers). */
+/* bit4 / bit5: epilogue selection of other GPU generations: accepted, no effect on sm_90 (bf16 and fp32 D both take
+ * the shared-memory + TMA-store epilogue). */
 #define DOLO_GEMM_FLAG_DIRECT_EPILOGUE 16
 #define DOLO_GEMM_FLAG_F32_TMA_EPILOGUE 32
 int dolomite_b200_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const void* B, int64_t ldb, int b_mn_major,

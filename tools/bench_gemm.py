@@ -9,8 +9,14 @@ the head's weight gradient.  Each launch is warmed up at every width, then timed
 each round a window of back-to-back launches of at least --window-ms; the best round of each width is kept.  Per shape
 it reports TFLOP/s at each width, the width the automatic choice takes, and c_256 / c_128, the time of one 128 x 256
 tile over one 128 x 128 tile: time / ceil(tiles / SMs) at each width.  The median of that ratio over the shapes is the
-constant of the automatic choice (TILE256_COST in csrc/gemm.cu).  Prints one JSON line with the card name and power
-limit.
+constant of the automatic choice (TILE256_COST in csrc/gemm.cu).
+
+The launches carry the engine's epilogue operands: a bias on every block linear's forward, the residual as C on the
+two c_proj forwards, and weight gradients that overwrite their output (one micro-step per optimizer step).
+
+A K sweep times the forward of a 4096 x 2560 output at K = 2560 .. 20480 at both widths and fits the time of one tile,
+t = n_kb * a + f (n_kb 64-deep k-blocks): `a` is the mainloop's cost per k-block and `f` the fixed cost per tile
+(epilogue, pipeline fill and drain).  Prints one JSON line with the card name and power limit.
 """
 
 from __future__ import annotations
@@ -64,18 +70,20 @@ def _launches(T: int, block: dict, head: list, g) -> list[dict]:
     for name, (N, Kd) in list(block.items()) + head:
         x, w, dy = _bf16(T, Kd, g=g), _bf16(N, Kd, g=g, scale=0.02), _bf16(T, N, g=g, scale=1e-3)
         y, dx = torch.empty(T, N, dtype=torch.bfloat16, device="cuda"), torch.empty(T, Kd, dtype=torch.bfloat16, device="cuda")
+        bias = None if name == "head" else _bf16(N, g=g, scale=0.02)
+        res = _bf16(T, N, g=g) if name.endswith("c_proj") else None  # the residual stream, added by the c_proj forwards
         out.append(dict(name=f"{name}.fwd", outputs=[(T, N)], flops=2.0 * T * N * Kd,
-                        fn=lambda x=x, w=w, y=y: K.gemm(x, w, out=y)))
+                        fn=lambda x=x, w=w, y=y, b=bias, c=res: K.gemm(x, w, out=y, bias=b, c=c, beta=1.0)))
         out.append(dict(name=f"{name}.dgrad", outputs=[(T, Kd)], flops=2.0 * T * N * Kd,
                         fn=lambda dy=dy, w=w, dx=dx: K.gemm(dy, w, b_mn=True, out=dx)))
         if name == "head":
             dw = torch.zeros(N, Kd, dtype=torch.float32, device="cuda")
             out.append(dict(name="head.wgrad", outputs=[(N, Kd)], flops=2.0 * T * N * Kd,
-                            fn=lambda dy=dy, x=x, dw=dw: K.gemm(dy, x, a_mn=True, b_mn=True, out=dw, c=dw, beta=1.0)))
+                            fn=lambda dy=dy, x=x, dw=dw: K.gemm(dy, x, a_mn=True, b_mn=True, out=dw)))
     probs, outputs, flops = [], [], 0.0
     for N, Kd in block.values():
         probs.append((_bf16(T, N, g=g, scale=1e-3), _bf16(T, Kd, g=g), torch.zeros(N, Kd, dtype=torch.float32, device="cuda"),
-                      1.0, True))
+                      1.0, False))
         outputs.append((N, Kd))
         flops += 2.0 * T * N * Kd
     out.append(dict(name="block.wgrad_multi", outputs=outputs, flops=flops, fn=lambda probs=probs: K.gemm_wgrad_multi(probs)))
@@ -91,6 +99,33 @@ def _time(fn, iters: int) -> float:
     e1.record()
     torch.cuda.synchronize()
     return e0.elapsed_time(e1) / iters * 1e-3
+
+
+def k_sweep(T: int, N: int, g, window_ms: float, rounds: int, workers: int) -> dict:
+    """forward of a T x N output at K = 2560 .. 20480 at both widths; least-squares fit of the per-tile time
+    t = n_kb * a + f, where t = launch time / ceil(tiles / workers)"""
+    res = {}
+    for width in (128, 256):
+        K.set_option("gemm_tile_n", width)
+        waves = math.ceil(math.ceil(T / 128) * math.ceil(N / width) / workers)
+        pts = []
+        for Kd in (2560, 5120, 10240, 20480):
+            x, w = _bf16(T, Kd, g=g), _bf16(N, Kd, g=g, scale=0.02)
+            y = torch.empty(T, N, dtype=torch.bfloat16, device="cuda")
+            fn = lambda x=x, w=w, y=y: K.gemm(x, w, out=y)  # noqa: E731
+            fn()
+            torch.cuda.synchronize()
+            iters = max(5, math.ceil(window_ms * 1e-3 / _time(fn, 3)))
+            best = min(_time(fn, iters) for _ in range(rounds))
+            pts.append((Kd // 64, best / waves, 2.0 * T * N * Kd / best / 1e12))
+        n = len(pts)
+        mx, my = sum(p[0] for p in pts) / n, sum(p[1] for p in pts) / n
+        a = sum((p[0] - mx) * (p[1] - my) for p in pts) / sum((p[0] - mx) ** 2 for p in pts)
+        f = my - a * mx
+        res[str(width)] = {"waves": waves, "tile_us": {p[0] * 64: round(p[1] * 1e6, 3) for p in pts},
+                           "tflops": {p[0] * 64: round(p[2], 1) for p in pts},
+                           "a_us_per_kblock": round(a * 1e6, 4), "f_us_per_tile": round(f * 1e6, 3)}
+    return res
 
 
 def main() -> None:
@@ -134,6 +169,7 @@ def main() -> None:
             r.update(outputs=L["outputs"], auto_tile_n=auto_n, waves_128=waves[128], waves_256=waves[256],
                      tile_cost_256_over_128=round(ratio, 3), auto_over_128=round(best["auto"] / best["128"], 4))
             res["shapes"][L["name"]] = r
+        res["k_sweep_4096x2560"] = k_sweep(T, 2560, g, a.window_ms, a.rounds, workers)
     finally:
         K.set_option("gemm_tile_n", default)
     res["tile_cost_256_over_128_median"] = round(statistics.median(ratios), 3)
