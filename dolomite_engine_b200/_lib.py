@@ -39,6 +39,8 @@ SIGNATURES: dict[str, tuple] = {
     "dolomite_b200_layernorm_fwd": (_I, [_P, _P, _P, _P, _P, _P, _L, _I, _F, _P]),
     "dolomite_b200_layernorm_bwd_workspace_bytes": (_L, [_I]),
     "dolomite_b200_layernorm_bwd": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _L, _I, _P]),
+    "dolomite_b200_act_fwd": (_I, [_I, _I, _P, _P, _L, _L, _P]),
+    "dolomite_b200_act_bwd": (_I, [_I, _I, _P, _P, _P, _P, _L, _L, _P]),
     "dolomite_b200_gelu_fwd": (_I, [_P, _P, _L, _P]),
     "dolomite_b200_gelu_bwd": (_I, [_P, _P, _P, _P, _L, _L, _P]),
     "dolomite_b200_swiglu_fwd": (_I, [_P, _P, _L, _L, _P]),
@@ -143,6 +145,7 @@ KERNELS_PER_CALL = {
     "dolomite_b200_rmsnorm_fwd": 1, "dolomite_b200_rmsnorm_bwd": 2, "dolomite_b200_rope_qk_inplace": 1,
     "dolomite_b200_layernorm_fwd": 1, "dolomite_b200_layernorm_bwd": 3, "dolomite_b200_gelu_fwd": 1,
     "dolomite_b200_gelu_bwd": 1, "dolomite_b200_swiglu_fwd": 1, "dolomite_b200_swiglu_bwd": 1, "dolomite_b200_swiglu_bwd_bias": 1,
+    "dolomite_b200_act_fwd": 1, "dolomite_b200_act_bwd": 1,
     "dolomite_b200_embedding_fwd": 1,
     "dolomite_b200_embedding_bwd": 1, "dolomite_b200_cross_entropy_fwd_bwd": 3, "dolomite_b200_colsum_accum": 1,
     "dolomite_b200_scale_bf16_by_device_scalar": 1, "dolomite_b200_add_scaled": 1, "dolomite_b200_sumsq_accum": 2,

@@ -1,6 +1,8 @@
-// HBM-bound kernels of the GPTDolomite training step: RMSNorm, RoPE, SwiGLU, embedding, cross-entropy,
+// HBM-bound kernels of the GPTDolomite training step: RMSNorm, RoPE, MLP activations, embedding, cross-entropy,
 // bias-gradient column sums, residual adds and the flat-shard optimizer kernels.
 // All are coalesced 16-byte vector kernels with warp-shuffle reductions; fp32 math, bf16 storage.
+#include <type_traits>
+
 #include "common.cuh"
 #include "../../include/dolomite_b200.h"
 
@@ -347,178 +349,253 @@ __global__ void __launch_bounds__(MAX_THREADS)
 }
 
 // ------------------------------------------------------------------------------------------
-// SwiGLU
+// MLP activations (hf_models/modeling_utils/activations/{base,glu}.py): one functor per function with its value f and
+// its derivative d, used by one forward and one backward template in three forms (DOLO_ACT_PLAIN / _GLU /
+// _SIGMOID_GLU, include/dolomite_b200.h).  fp32 math on bf16 storage.  Where torch's eager module rounds to bf16 more
+// than once, f rounds at the same points (laplace, softsign, tanhshrink); d is the fp32 derivative with torch
+// autograd's value at the non-differentiable points (bf16 inputs land on them often).
 // ------------------------------------------------------------------------------------------
 // MUFU ex2 + MUFU rcp (2 ulp fp32; the result is rounded to bf16 right after) instead of the ~10-instruction IEEE divide:
-// the kernel is otherwise issue-bound next to its HBM time (168 M elements per layer).
+// the SwiGLU kernel is otherwise issue-bound next to its HBM time (168 M elements per layer).
 __device__ __forceinline__ float sigmoidf_(float x) { return __fdividef(1.f, 1.f + __expf(-x)); }
-
-__global__ void __launch_bounds__(kThreads)
-    swiglu_fwd_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, int64_t T, int64_t F8) {
-    const int64_t total = T * F8;
-    for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += int64_t(gridDim.x) * blockDim.x) {
-        const int64_t t = i / F8, c = i - t * F8;
-        float u[8], g[8], o[8];
-        unpack8(__ldg(x + t * 2 * F8 + c), u);
-        unpack8(__ldg(x + t * 2 * F8 + F8 + c), g);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) o[j] = u[j] * bf16_round(g[j] * sigmoidf_(g[j]));
-        y[i] = pack8(o);
-    }
-}
-
-__global__ void __launch_bounds__(kThreads) swiglu_bwd_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x,
-                                                              uint4* __restrict__ dx, int64_t T, int64_t F8) {
-    const int64_t total = T * F8;
-    for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += int64_t(gridDim.x) * blockDim.x) {
-        const int64_t t = i / F8, c = i - t * F8;
-        float u[8], g[8], d[8], du[8], dg[8];
-        unpack8(__ldg(x + t * 2 * F8 + c), u);
-        unpack8(__ldg(x + t * 2 * F8 + F8 + c), g);
-        unpack8(__ldg(dy + i), d);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const float sg = sigmoidf_(g[j]);
-            const float silu = g[j] * sg;
-            du[j] = d[j] * silu;
-            dg[j] = d[j] * u[j] * (sg * (1.f + g[j] * (1.f - sg)));
-        }
-        dx[t * 2 * F8 + c] = pack8(du);
-        dx[t * 2 * F8 + F8 + c] = pack8(dg);
-    }
-}
-
-// SwiGLU backward that also accumulates the bias gradient of the producing linear layer (column sums of the bf16 dx it
-// writes): saves the separate pass that re-read the whole [T, 2F] tensor.  Block = 32 column vectors (256 up + 256 gate
-// columns) x 8 row lanes over `rows_per_block` rows; per-thread fp32 column sums, smem combine, and the row splits of a
-// column tile (one cluster) combined in a fixed order (cluster_colsum_apply).
-__global__ void __launch_bounds__(kThreads)
-    swiglu_bwd_bias_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x, uint4* __restrict__ dx,
-                           float* __restrict__ dbias, int64_t T, int64_t F8, int rows_per_block) {
-    __shared__ float sm[8][2][256];
-    const int lane = threadIdx.x & 31, rl = threadIdx.x >> 5;
-    const int64_t c = int64_t(blockIdx.x) * 32 + lane;
-    const int64_t r0 = int64_t(blockIdx.y) * rows_per_block;
-    const int64_t r1 = min(T, r0 + rows_per_block);
-    float su[8], sg[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) su[j] = sg[j] = 0.f;
-    if (c < F8) {
-        for (int64_t t = r0 + rl; t < r1; t += 8) {
-            float u[8], g[8], d[8], du[8], dg[8];
-            unpack8(__ldg(x + t * 2 * F8 + c), u);
-            unpack8(__ldg(x + t * 2 * F8 + F8 + c), g);
-            unpack8(__ldg(dy + t * F8 + c), d);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const float sgm = sigmoidf_(g[j]);
-                du[j] = d[j] * (g[j] * sgm);
-                dg[j] = d[j] * u[j] * (sgm * (1.f + g[j] * (1.f - sgm)));
-            }
-            const uint4 pu = pack8(du), pg = pack8(dg);
-            dx[t * 2 * F8 + c] = pu;
-            dx[t * 2 * F8 + F8 + c] = pg;
-            unpack8(pu, du);  // the bias gradient sums the bf16 values autograd would see
-            unpack8(pg, dg);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                su[j] += du[j];
-                sg[j] += dg[j];
-            }
-        }
-    }
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-        sm[rl][0][lane * 8 + j] = su[j];
-        sm[rl][1][lane * 8 + j] = sg[j];
-    }
-    __syncthreads();
-    __shared__ float part[2][256];
-    const int col = threadIdx.x;
-    float a = 0.f, b = 0.f;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) {
-        a += sm[w][0][col];
-        b += sm[w][1][col];
-    }
-    part[0][col] = a;
-    part[1][col] = b;
-    const int64_t gc = int64_t(blockIdx.x) * 256 + col;
-    const bool ok = gc < F8 * 8;
-    cluster_colsum_apply(&part[0][col], dbias + (ok ? gc : 0), ok, 1.f);
-    cluster_colsum_apply(&part[1][col], dbias + (ok ? F8 * 8 + gc : 0), ok, 1.f);
-}
-
-// ------------------------------------------------------------------------------------------
-// tanh-GELU (activation_function gelu_pytorch_tanh, non-GLU MLP of the StarCoder / bigcode shape)
-//   y = 0.5 x (1 + tanh(k (x + c x^3))),  k = sqrt(2/pi), c = 0.044715
-// ------------------------------------------------------------------------------------------
 __device__ __forceinline__ float tanh_fast(float z) {
     // tanh(z) = 1 - 2 / (1 + e^{2z}); MUFU ex2 + MUFU rcp, saturates cleanly for |z| large
     return 1.f - __fdividef(2.f, 1.f + __expf(2.f * z));
 }
-__device__ __forceinline__ float gelu_tanh_f(float x) {
-    const float z = 0.7978845608028654f * (x + 0.044715f * x * x * x);
-    return 0.5f * x * (1.f + tanh_fast(z));
-}
-__device__ __forceinline__ float gelu_tanh_grad(float x) {
-    const float z = 0.7978845608028654f * (x + 0.044715f * x * x * x);
-    const float t = tanh_fast(z);
-    const float dz = 0.7978845608028654f * (1.f + 3.f * 0.044715f * x * x);
-    return 0.5f * (1.f + t) + 0.5f * x * (1.f - t * t) * dz;
-}
 
-__global__ void __launch_bounds__(kThreads) gelu_fwd_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, int64_t n8) {
-    for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n8; i += int64_t(gridDim.x) * blockDim.x) {
-        float f[8];
-        unpack8(__ldg(x + i), f);
+namespace act {
+// elu / celu (alpha 1; CELU with alpha 1 is ELU) and selu: torch's elu kernel, x <= 0 ? expm1(x) * a * s : x * s
+template <int kSelu>
+struct EluT {
+    static constexpr float s = kSelu ? 1.0507009873554804934193349852946f : 1.f;
+    static constexpr float as = kSelu ? 1.0507009873554804934193349852946f * 1.6732632423543772848170429916717f : 1.f;
+    __device__ static float f(float x) { return x <= 0.f ? expm1f(x) * as : x * s; }
+    __device__ static float d(float x) { return x <= 0.f ? as * expf(x) : s; }
+};
+using Elu = EluT<0>;
+using Selu = EluT<1>;
+struct Gelu {  // exact erf
+    __device__ static float f(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
+    __device__ static float d(float x) {
+        return 0.5f * (1.f + erff(x * 0.70710678118654752f)) + x * 0.39894228040143268f * expf(-0.5f * x * x);
+    }
+};
+// tanh-GELU (gelu_pytorch_tanh): y = 0.5 x (1 + tanh(k (x + c x^3))),  k = sqrt(2/pi), c = 0.044715
+struct GeluTanh {
+    __device__ static float f(float x) {
+        const float z = 0.7978845608028654f * (x + 0.044715f * x * x * x);
+        return 0.5f * x * (1.f + tanh_fast(z));
+    }
+    __device__ static float d(float x) {
+        const float z = 0.7978845608028654f * (x + 0.044715f * x * x * x);
+        const float t = tanh_fast(z);
+        const float dz = 0.7978845608028654f * (1.f + 3.f * 0.044715f * x * x);
+        return 0.5f * (1.f + t) + 0.5f * x * (1.f - t * t) * dz;
+    }
+};
+struct HardShrink {  // lambda 0.5; zero on [-0.5, 0.5], ends included (value and gradient)
+    __device__ static float f(float x) { return (x >= -0.5f && x <= 0.5f) ? 0.f : x; }
+    __device__ static float d(float x) { return (x >= -0.5f && x <= 0.5f) ? 0.f : 1.f; }
+};
+struct HardSigmoid {
+    __device__ static float f(float x) { return fminf(fmaxf(x + 3.f, 0.f), 6.f) / 6.f; }
+    __device__ static float d(float x) { return (x > -3.f && x < 3.f) ? 1.f / 6.f : 0.f; }
+};
+struct HardSwish {  // gradient x/3 + 1/2 inside (-3, 3); 0 at -3 and 1 at 3, as torch autograd gives
+    __device__ static float f(float x) { return x * fminf(fmaxf(x + 3.f, 0.f), 6.f) / 6.f; }
+    __device__ static float d(float x) { return x <= -3.f ? 0.f : (x < 3.f ? x / 3.f + 0.5f : 1.f); }
+};
+struct HardTanh {  // [-1, 1]; gradient 0 at the bounds
+    __device__ static float f(float x) { return fminf(fmaxf(x, -1.f), 1.f); }
+    __device__ static float d(float x) { return (x > -1.f && x < 1.f) ? 1.f : 0.f; }
+};
+// transformers' LaplaceActivation, mu 0.707107, sigma 0.282095: 0.5 * (1 + erf((x - mu) / (sigma sqrt 2))), every eager
+// op rounded to bf16 (the 0.5 * is exact).  torch's bf16 `x - mu` rounds the scalar mu to bf16 first (0.70703125): near
+// erf = -1 the sum 1 + erf cancels, so that choice is visible in the result.
+struct Laplace {
+    static constexpr float mu = 0.70703125f;
+    static constexpr float den = float(0.282095 * 1.4142135623730951);
+    __device__ static float f(float x) {
+        const float z = bf16_round(bf16_round(x - mu) / den);
+        return 0.5f * bf16_round(1.f + bf16_round(erff(z)));
+    }
+    __device__ static float d(float x) {
+        const float z = (x - 0.707107f) / den;
+        return 0.56418958354775629f / den * expf(-z * z);  // 0.5 * 2/sqrt(pi) * exp(-z^2) / den
+    }
+};
+struct LeakyRelu {  // slope 0.01; gradient 0.01 at 0
+    __device__ static float f(float x) { return x > 0.f ? x : x * 0.01f; }
+    __device__ static float d(float x) { return x > 0.f ? 1.f : 0.01f; }
+};
+struct LogSigmoid {
+    __device__ static float f(float x) { return fminf(x, 0.f) - log1pf(expf(-fabsf(x))); }
+    __device__ static float d(float x) {
+        const float z = expf(-fabsf(x));
+        return x < 0.f ? 1.f - z / (1.f + z) : z / (1.f + z);
+    }
+};
+struct Mish {
+    __device__ static float f(float x) { return x * tanhf(log1pf(expf(x))); }
+    __device__ static float d(float x) {
+        const float t = tanhf(log1pf(expf(x)));
+        return t + x * (1.f / (1.f + expf(-x))) * (1.f - t * t);
+    }
+};
+struct Relu {
+    __device__ static float f(float x) { return fmaxf(x, 0.f); }
+    __device__ static float d(float x) { return x > 0.f ? 1.f : 0.f; }
+};
+struct Relu2 {  // square(relu(x)): relu is exact, so one rounding
+    __device__ static float f(float x) { const float r = fmaxf(x, 0.f); return r * r; }
+    __device__ static float d(float x) { return x > 0.f ? 2.f * x : 0.f; }
+};
+struct Relu6 {  // hardtanh(0, 6): gradient 0 at both bounds
+    __device__ static float f(float x) { return fminf(fmaxf(x, 0.f), 6.f); }
+    __device__ static float d(float x) { return (x > 0.f && x < 6.f) ? 1.f : 0.f; }
+};
+struct Sigmoid {
+    __device__ static float f(float x) { return sigmoidf_(x); }
+    __device__ static float d(float x) { const float s = sigmoidf_(x); return s * (1.f - s); }
+};
+struct Silu {
+    __device__ static float f(float x) { return x * sigmoidf_(x); }
+    __device__ static float d(float x) { const float s = sigmoidf_(x); return s * (1.f + x * (1.f - s)); }
+};
+struct Softplus {  // beta 1, threshold 20: linear (gradient 1) above the threshold
+    __device__ static float f(float x) { return x > 20.f ? x : log1pf(expf(x)); }
+    __device__ static float d(float x) { const float z = expf(x); return x > 20.f ? 1.f : z / (z + 1.f); }
+};
+struct SoftShrink {  // lambda 0.5; zero gradient on [-0.5, 0.5], ends included
+    __device__ static float f(float x) { return x > 0.5f ? x - 0.5f : (x < -0.5f ? x + 0.5f : 0.f); }
+    __device__ static float d(float x) { return (x >= -0.5f && x <= 0.5f) ? 0.f : 1.f; }
+};
+struct SoftSign {  // x / (|x| + 1), the sum rounded first
+    __device__ static float f(float x) { return x / bf16_round(fabsf(x) + 1.f); }
+    __device__ static float d(float x) { const float a = 1.f + fabsf(x); return 1.f / (a * a); }
+};
+struct Tanh {
+    __device__ static float f(float x) { return tanhf(x); }
+    __device__ static float d(float x) { const float t = tanhf(x); return 1.f - t * t; }
+};
+struct TanhShrink {  // x - tanh(x), tanh rounded first
+    __device__ static float f(float x) { return x - bf16_round(tanhf(x)); }
+    __device__ static float d(float x) { const float t = tanhf(x); return t * t; }
+};
+}  // namespace act
+
+// forward: plain y = f(x);  GLU x = [u | g], y = u * bf16(f(g));  sigmoid-GLU (torch's fused glu) y = u * f(g) rounded
+// once.  Grid-stride over 16-byte vectors of y.
+template <class Op, int Form>
+__global__ void __launch_bounds__(kThreads) act_fwd_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, int64_t T,
+                                                           int64_t F8) {
+    const int64_t total = T * F8;
+    for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += int64_t(gridDim.x) * blockDim.x) {
+        float o[8];
+        if constexpr (Form == DOLO_ACT_PLAIN) {
+            unpack8(__ldg(x + i), o);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) f[j] = gelu_tanh_f(f[j]);
-        y[i] = pack8(f);
+            for (int j = 0; j < 8; ++j) o[j] = Op::f(o[j]);
+        } else {
+            const int64_t t = i / F8, c = i - t * F8;
+            float u[8], g[8];
+            unpack8(__ldg(x + t * 2 * F8 + c), u);
+            unpack8(__ldg(x + t * 2 * F8 + F8 + c), g);
+#pragma unroll
+            for (int j = 0; j < 8; ++j) o[j] = Form == DOLO_ACT_GLU ? u[j] * bf16_round(Op::f(g[j])) : u[j] * Op::f(g[j]);
+        }
+        y[i] = pack8(o);
     }
 }
 
-// dx = dy * gelu'(x); optionally accumulates the bias gradient of the producing linear (column sums of the bf16 dx).
-// Same block shape as swiglu_bwd_bias_kernel: 32 column vectors x 8 row lanes.
+// dx of one row vector: plain dx = dy * f'(x);  GLU (both forms) du = dy * f(g), dg = dy * u * f'(g)
+template <class Op, bool Glu>
+__device__ __forceinline__ void act_bwd_vec(const uint4* __restrict__ dy, const uint4* __restrict__ x, int64_t t,
+                                            int64_t c, int64_t F8, float (&o)[Glu ? 2 : 1][8]) {
+    float d[8];
+    unpack8(__ldg(dy + t * F8 + c), d);
+    if constexpr (Glu) {
+        float u[8], g[8];
+        unpack8(__ldg(x + t * 2 * F8 + c), u);
+        unpack8(__ldg(x + t * 2 * F8 + F8 + c), g);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            o[0][j] = d[j] * Op::f(g[j]);
+            o[1][j] = d[j] * u[j] * Op::d(g[j]);
+        }
+    } else {
+        float xf[8];
+        unpack8(__ldg(x + t * F8 + c), xf);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) o[0][j] = d[j] * Op::d(xf[j]);
+    }
+}
+
+template <class Op, bool Glu>
+__global__ void __launch_bounds__(kThreads) act_bwd_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x,
+                                                           uint4* __restrict__ dx, int64_t T, int64_t F8) {
+    constexpr int NP = Glu ? 2 : 1;
+    const int64_t total = T * F8;
+    for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += int64_t(gridDim.x) * blockDim.x) {
+        const int64_t t = i / F8, c = i - t * F8;
+        float o[NP][8];
+        act_bwd_vec<Op, Glu>(dy, x, t, c, F8, o);
+#pragma unroll
+        for (int p = 0; p < NP; ++p) dx[t * NP * F8 + p * F8 + c] = pack8(o[p]);
+    }
+}
+
+// Backward that also accumulates the bias gradient of the producing linear layer (column sums of the bf16 dx it
+// writes): saves the separate pass that re-read the whole dx.  Block = 32 column vectors (256 columns of each half)
+// x 8 row lanes over `rows_per_block` rows; per-thread fp32 column sums, smem combine, and the row splits of a column
+// tile (one cluster) combined in a fixed order (cluster_colsum_apply).
+template <class Op, bool Glu>
 __global__ void __launch_bounds__(kThreads)
-    gelu_bwd_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x, uint4* __restrict__ dx,
-                    float* __restrict__ dbias, int64_t T, int64_t F8, int rows_per_block) {
-    __shared__ float sm[8][256];
+    act_bwd_bias_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x, uint4* __restrict__ dx,
+                        float* __restrict__ dbias, int64_t T, int64_t F8, int rows_per_block) {
+    constexpr int NP = Glu ? 2 : 1;
+    __shared__ float sm[8][NP][256];
     const int lane = threadIdx.x & 31, rl = threadIdx.x >> 5;
     const int64_t c = int64_t(blockIdx.x) * 32 + lane;
     const int64_t r0 = int64_t(blockIdx.y) * rows_per_block;
     const int64_t r1 = min(T, r0 + rows_per_block);
-    float s[8];
+    float s[NP][8];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) s[j] = 0.f;
+    for (int p = 0; p < NP; ++p)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) s[p][j] = 0.f;
     if (c < F8) {
         for (int64_t t = r0 + rl; t < r1; t += 8) {
-            float xf[8], d[8];
-            unpack8(__ldg(x + t * F8 + c), xf);
-            unpack8(__ldg(dy + t * F8 + c), d);
+            float o[NP][8];
+            act_bwd_vec<Op, Glu>(dy, x, t, c, F8, o);
 #pragma unroll
-            for (int j = 0; j < 8; ++j) d[j] *= gelu_tanh_grad(xf[j]);
-            const uint4 pk = pack8(d);
-            dx[t * F8 + c] = pk;
-            if (dbias != nullptr) {
-                unpack8(pk, d);
+            for (int p = 0; p < NP; ++p) {
+                const uint4 pk = pack8(o[p]);
+                dx[t * NP * F8 + p * F8 + c] = pk;
+                unpack8(pk, o[p]);  // the bias gradient sums the bf16 values autograd would see
 #pragma unroll
-                for (int j = 0; j < 8; ++j) s[j] += d[j];
+                for (int j = 0; j < 8; ++j) s[p][j] += o[p][j];
             }
         }
     }
-    if (dbias == nullptr) return;  // uniform over the cluster
 #pragma unroll
-    for (int j = 0; j < 8; ++j) sm[rl][lane * 8 + j] = s[j];
+    for (int p = 0; p < NP; ++p)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) sm[rl][p][lane * 8 + j] = s[p][j];
     __syncthreads();
-    __shared__ float part[256];
-    float a = 0.f;
+    __shared__ float part[NP][256];
+    const int col = threadIdx.x;
 #pragma unroll
-    for (int w = 0; w < 8; ++w) a += sm[w][threadIdx.x];
-    part[threadIdx.x] = a;
-    const int64_t gc = int64_t(blockIdx.x) * 256 + threadIdx.x;
+    for (int p = 0; p < NP; ++p) {
+        float a = 0.f;
+#pragma unroll
+        for (int w = 0; w < 8; ++w) a += sm[w][p][col];
+        part[p][col] = a;
+    }
+    const int64_t gc = int64_t(blockIdx.x) * 256 + col;
     const bool ok = gc < F8 * 8;
-    cluster_colsum_apply(&part[threadIdx.x], dbias + (ok ? gc : 0), ok, 1.f);
+#pragma unroll
+    for (int p = 0; p < NP; ++p) cluster_colsum_apply(&part[p][col], dbias + (ok ? p * F8 * 8 + gc : 0), ok, 1.f);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1227,29 +1304,6 @@ extern "C" int dolomite_b200_layernorm_bwd(const void* dy, const void* x, const 
     return DOLO_OK;
 }
 
-extern "C" int dolomite_b200_gelu_fwd(const void* x, void* y, int64_t n, void* stream) {
-    DOLO_REQUIRE(n % 8 == 0 && aligned16(x) && aligned16(y), "gelu: n must be a multiple of 8 and pointers 16-byte aligned");
-    if (n == 0) return DOLO_OK;
-    gelu_fwd_kernel<<<grid_for(n / 8, kThreads), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-        static_cast<const uint4*>(x), static_cast<uint4*>(y), n / 8);
-    DOLO_LAUNCH_OK("gelu_fwd");
-    return DOLO_OK;
-}
-
-extern "C" int dolomite_b200_gelu_bwd(const void* dy, const void* x, void* dx, float* dbias_accum, int64_t T, int64_t F,
-                                      void* stream) {
-    DOLO_REQUIRE(F > 0 && F % 8 == 0, "gelu_bwd: F=%lld must be a positive multiple of 8", (long long)F);
-    DOLO_REQUIRE(aligned16(x) && aligned16(dy) && aligned16(dx), "gelu_bwd: pointers must be 16-byte aligned");
-    if (T == 0) return DOLO_OK;
-    const int64_t F8 = F / 8;
-    const int col_tiles = int((F8 + 31) / 32);
-    const int rows_per_block = int((T + kColsumCluster - 1) / kColsumCluster);  // one cluster of row splits per column tile
-    DOLO_CUDA_OK(cudaError_t(launch_row_cluster(gelu_bwd_kernel, col_tiles, static_cast<cudaStream_t>(stream),
-                                                static_cast<const uint4*>(dy), static_cast<const uint4*>(x),
-                                                static_cast<uint4*>(dx), dbias_accum, T, F8, rows_per_block)));
-    return DOLO_OK;
-}
-
 extern "C" int dolomite_b200_rope_qk_inplace(void* qkv, int64_t row_stride, int64_t T, int n_groups, int q_per_group,
                                              int head_dim, const void* cos_table, const void* sin_table,
                                              const void* position_ids, int position_ids_is_int64, int64_t n_positions,
@@ -1286,41 +1340,132 @@ extern "C" int dolomite_b200_rope_qk_inplace(void* qkv, int64_t row_stride, int6
     return DOLO_OK;
 }
 
-extern "C" int dolomite_b200_swiglu_fwd(const void* x, void* y, int64_t T, int64_t F, void* stream) {
-    DOLO_REQUIRE(F > 0 && F % 8 == 0, "swiglu: F=%lld must be a positive multiple of 8", (long long)F);
-    DOLO_REQUIRE(aligned16(x) && aligned16(y), "swiglu: pointers must be 16-byte aligned");
-    if (T == 0) return DOLO_OK;
-    const int64_t F8 = F / 8;
-    swiglu_fwd_kernel<<<grid_for(T * F8, kThreads), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-        static_cast<const uint4*>(x), static_cast<uint4*>(y), T, F8);
-    DOLO_LAUNCH_OK("swiglu_fwd");
+namespace {
+
+// fn(Op{}) with the functor of activation `id`; false for an unknown id
+template <class Fn>
+bool visit_act(int id, Fn&& fn) {
+    switch (id) {
+        case DOLO_ACT_CELU:
+        case DOLO_ACT_ELU: fn(act::Elu{}); return true;
+        case DOLO_ACT_GELU: fn(act::Gelu{}); return true;
+        case DOLO_ACT_GELU_TANH: fn(act::GeluTanh{}); return true;
+        case DOLO_ACT_SELU: fn(act::Selu{}); return true;
+        case DOLO_ACT_HARDSHRINK: fn(act::HardShrink{}); return true;
+        case DOLO_ACT_HARDSIGMOID: fn(act::HardSigmoid{}); return true;
+        case DOLO_ACT_HARDSWISH: fn(act::HardSwish{}); return true;
+        case DOLO_ACT_HARDTANH: fn(act::HardTanh{}); return true;
+        case DOLO_ACT_LAPLACE: fn(act::Laplace{}); return true;
+        case DOLO_ACT_LEAKY_RELU: fn(act::LeakyRelu{}); return true;
+        case DOLO_ACT_LOG_SIGMOID: fn(act::LogSigmoid{}); return true;
+        case DOLO_ACT_MISH: fn(act::Mish{}); return true;
+        case DOLO_ACT_RELU: fn(act::Relu{}); return true;
+        case DOLO_ACT_RELU2: fn(act::Relu2{}); return true;
+        case DOLO_ACT_RELU6: fn(act::Relu6{}); return true;
+        case DOLO_ACT_SIGMOID: fn(act::Sigmoid{}); return true;
+        case DOLO_ACT_SILU: fn(act::Silu{}); return true;
+        case DOLO_ACT_SOFTPLUS: fn(act::Softplus{}); return true;
+        case DOLO_ACT_SOFTSHRINK: fn(act::SoftShrink{}); return true;
+        case DOLO_ACT_SOFTSIGN: fn(act::SoftSign{}); return true;
+        case DOLO_ACT_TANH: fn(act::Tanh{}); return true;
+        case DOLO_ACT_TANHSHRINK: fn(act::TanhShrink{}); return true;
+        default: return false;
+    }
+}
+
+template <class Op>
+void launch_act_fwd(int form, const void* x, void* y, int64_t T, int64_t F8, cudaStream_t st) {
+    auto X = static_cast<const uint4*>(x);
+    auto Y = static_cast<uint4*>(y);
+    const int grid = grid_for(T * F8, kThreads);
+    if (form == DOLO_ACT_PLAIN) {
+        act_fwd_kernel<Op, DOLO_ACT_PLAIN><<<grid, kThreads, 0, st>>>(X, Y, T, F8);
+    } else if (form == DOLO_ACT_GLU) {
+        act_fwd_kernel<Op, DOLO_ACT_GLU><<<grid, kThreads, 0, st>>>(X, Y, T, F8);
+    } else if constexpr (std::is_same_v<Op, act::Sigmoid>) {  // torch's fused glu exists for the sigmoid only
+        act_fwd_kernel<Op, DOLO_ACT_SIGMOID_GLU><<<grid, kThreads, 0, st>>>(X, Y, T, F8);
+    }
+}
+
+template <class Op, bool Glu>
+cudaError_t launch_act_bwd_form(const void* dy, const void* x, void* dx, float* dbias, int64_t T, int64_t F8,
+                                cudaStream_t st) {
+    auto DY = static_cast<const uint4*>(dy);
+    auto X = static_cast<const uint4*>(x);
+    auto DX = static_cast<uint4*>(dx);
+    if (dbias == nullptr) {
+        act_bwd_kernel<Op, Glu><<<grid_for(T * F8, kThreads), kThreads, 0, st>>>(DY, X, DX, T, F8);
+        return cudaGetLastError();
+    }
+    const int col_tiles = int((F8 + 31) / 32);
+    const int rows_per_block = int((T + kColsumCluster - 1) / kColsumCluster);  // one cluster of row splits per column tile
+    return cudaError_t(launch_row_cluster(act_bwd_bias_kernel<Op, Glu>, col_tiles, st, DY, X, DX, dbias, T, F8,
+                                          rows_per_block));
+}
+
+int check_act(const char* what, int act_id, int form, int64_t F) {
+    DOLO_REQUIRE(act_id >= 0 && act_id < DOLO_ACT_COUNT, "%s: unknown activation id %d", what, act_id);
+    DOLO_REQUIRE(form == DOLO_ACT_PLAIN || form == DOLO_ACT_GLU || (form == DOLO_ACT_SIGMOID_GLU && act_id == DOLO_ACT_SIGMOID),
+                 "%s: form %d is not defined for activation id %d", what, form, act_id);
+    DOLO_REQUIRE(F > 0 && F % 8 == 0, "%s: F=%lld must be a positive multiple of 8", what, (long long)F);
     return DOLO_OK;
 }
 
-extern "C" int dolomite_b200_swiglu_bwd(const void* dy, const void* x, void* dx, int64_t T, int64_t F, void* stream) {
-    DOLO_REQUIRE(F > 0 && F % 8 == 0, "swiglu_bwd: F=%lld must be a positive multiple of 8", (long long)F);
-    DOLO_REQUIRE(aligned16(x) && aligned16(dy) && aligned16(dx), "swiglu_bwd: pointers must be 16-byte aligned");
+}  // namespace
+
+extern "C" int dolomite_b200_act_fwd(int act_id, int form, const void* x, void* y, int64_t T, int64_t F, void* stream) {
+    if (const int rc = check_act("act_fwd", act_id, form, F)) return rc;
+    DOLO_REQUIRE(aligned16(x) && aligned16(y), "act_fwd: pointers must be 16-byte aligned");
     if (T == 0) return DOLO_OK;
-    const int64_t F8 = F / 8;
-    swiglu_bwd_kernel<<<grid_for(T * F8, kThreads), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-        static_cast<const uint4*>(dy), static_cast<const uint4*>(x), static_cast<uint4*>(dx), T, F8);
-    DOLO_LAUNCH_OK("swiglu_bwd");
+    visit_act(act_id, [&](auto op) {
+        launch_act_fwd<decltype(op)>(form, x, y, T, F / 8, static_cast<cudaStream_t>(stream));
+    });
+    DOLO_LAUNCH_OK("act_fwd");
     return DOLO_OK;
+}
+
+extern "C" int dolomite_b200_act_bwd(int act_id, int form, const void* dy, const void* x, void* dx, float* dbias_accum,
+                                     int64_t T, int64_t F, void* stream) {
+    if (const int rc = check_act("act_bwd", act_id, form, F)) return rc;
+    DOLO_REQUIRE(aligned16(x) && aligned16(dy) && aligned16(dx), "act_bwd: pointers must be 16-byte aligned");
+    if (T == 0) return DOLO_OK;
+    cudaError_t e = cudaSuccess;
+    visit_act(act_id, [&](auto op) {
+        using Op = decltype(op);
+        const cudaStream_t st = static_cast<cudaStream_t>(stream);
+        e = form == DOLO_ACT_PLAIN ? launch_act_bwd_form<Op, false>(dy, x, dx, dbias_accum, T, F / 8, st)
+                                   : launch_act_bwd_form<Op, true>(dy, x, dx, dbias_accum, T, F / 8, st);
+    });
+    DOLO_CUDA_OK(e);
+    return DOLO_OK;
+}
+
+// the SwiGLU / tanh-GELU entry points of ABI version 1
+extern "C" int dolomite_b200_gelu_fwd(const void* x, void* y, int64_t n, void* stream) {
+    DOLO_REQUIRE(n % 8 == 0 && aligned16(x) && aligned16(y), "gelu: n must be a multiple of 8 and pointers 16-byte aligned");
+    if (n == 0) return DOLO_OK;
+    launch_act_fwd<act::GeluTanh>(DOLO_ACT_PLAIN, x, y, n / 8, 1, static_cast<cudaStream_t>(stream));
+    DOLO_LAUNCH_OK("gelu_fwd");
+    return DOLO_OK;
+}
+
+extern "C" int dolomite_b200_gelu_bwd(const void* dy, const void* x, void* dx, float* dbias_accum, int64_t T, int64_t F,
+                                      void* stream) {
+    return dolomite_b200_act_bwd(DOLO_ACT_GELU_TANH, DOLO_ACT_PLAIN, dy, x, dx, dbias_accum, T, F, stream);
+}
+
+extern "C" int dolomite_b200_swiglu_fwd(const void* x, void* y, int64_t T, int64_t F, void* stream) {
+    return dolomite_b200_act_fwd(DOLO_ACT_SILU, DOLO_ACT_GLU, x, y, T, F, stream);
+}
+
+extern "C" int dolomite_b200_swiglu_bwd(const void* dy, const void* x, void* dx, int64_t T, int64_t F, void* stream) {
+    return dolomite_b200_act_bwd(DOLO_ACT_SILU, DOLO_ACT_GLU, dy, x, dx, nullptr, T, F, stream);
 }
 
 extern "C" int dolomite_b200_swiglu_bwd_bias(const void* dy, const void* x, void* dx, float* dbias_accum, int64_t T,
                                              int64_t F, void* stream) {
-    DOLO_REQUIRE(F > 0 && F % 8 == 0, "swiglu_bwd_bias: F=%lld must be a positive multiple of 8", (long long)F);
-    DOLO_REQUIRE(aligned16(x) && aligned16(dy) && aligned16(dx), "swiglu_bwd_bias: pointers must be 16-byte aligned");
     DOLO_REQUIRE(dbias_accum != nullptr, "swiglu_bwd_bias: bias gradient buffer is null");
-    if (T == 0) return DOLO_OK;
-    const int64_t F8 = F / 8;
-    const int col_tiles = int((F8 + 31) / 32);
-    const int rows_per_block = int((T + kColsumCluster - 1) / kColsumCluster);  // one cluster of row splits per column tile
-    DOLO_CUDA_OK(cudaError_t(launch_row_cluster(swiglu_bwd_bias_kernel, col_tiles, static_cast<cudaStream_t>(stream),
-                                                static_cast<const uint4*>(dy), static_cast<const uint4*>(x),
-                                                static_cast<uint4*>(dx), dbias_accum, T, F8, rows_per_block)));
-    return DOLO_OK;
+    return dolomite_b200_act_bwd(DOLO_ACT_SILU, DOLO_ACT_GLU, dy, x, dx, dbias_accum, T, F, stream);
 }
 
 extern "C" int dolomite_b200_embedding_fwd(const int64_t* ids, const void* wte, void* out, int64_t T, int H, int64_t V,

@@ -24,6 +24,7 @@ from typing import TYPE_CHECKING
 import torch
 
 from . import kernels as K
+from .activations import resolve as resolve_activation
 
 if TYPE_CHECKING:  # the config module lives in hf_models, which imports this module
     from .hf_models.config import CommonConfig
@@ -206,11 +207,9 @@ def check_supported(cfg: CommonConfig) -> None:
     if cfg.normalization_function not in ("rmsnorm", "layernorm"):
         raise NotImplementedError(
             f"normalization_function={cfg.normalization_function!r}: rmsnorm and layernorm are implemented in CUDA")
-    if cfg.activation_function not in ("swiglu", "gelu_pytorch_tanh"):
-        raise NotImplementedError(
-            f"activation_function={cfg.activation_function!r}: swiglu and gelu_pytorch_tanh are implemented in CUDA")
-    if cfg.model_type == "moe_dolomite" and (cfg.activation_function != "swiglu" or cfg.normalization_function != "rmsnorm"):
-        raise NotImplementedError("MoE blocks are implemented for swiglu + rmsnorm (the MoEDolomite / Granite-MoE shape)")
+    resolve_activation(cfg.activation_function)  # ValueError / NotImplementedError as the reference's lookup
+    if cfg.model_type == "moe_dolomite" and cfg.normalization_function != "rmsnorm":
+        raise NotImplementedError("MoE blocks are implemented with rmsnorm (the MoEDolomite / Granite-MoE shape)")
     # dropout > 0: identity in eval mode; in training mode the residual / embedding dropouts are elementwise kernels
     # (csrc/dropout.cu) and the attention-probability dropout lives inside the attention kernels
     hd = cfg.n_embd // cfg.n_head
@@ -242,6 +241,7 @@ class DolomiteEngine:
         self.qkv_dim = cfg.n_embd + 2 * cfg.num_key_value_heads * self.hd
         self.is_moe = cfg.model_type == "moe_dolomite"
         self.is_glu = cfg.activation_function.endswith("glu")
+        self.act = resolve_activation(cfg.activation_function)  # (CUDA function id, form) of the MLP activation
         self.is_layernorm = cfg.normalization_function == "layernorm"
         self.learned_positions = cfg.position_embedding_type == "learned_absolute"
         self.has_dropout = bool(cfg.resid_pdrop or cfg.embd_pdrop or cfg.attn_pdrop)
@@ -536,7 +536,7 @@ class DolomiteEngine:
             h, moe_saved = moe.forward(self, u, p, ln2, h_mid, m_res, layer=i)
             return h, (x_in, rstd1, ln1, qkv, attn, lse, h_mid, rstd2, ln2, moe_saved)
         fc = self._linear(u, p + "mlp.c_fc.weight", ln2, p + "mlp.c_fc.bias")
-        act = K.swiglu_fwd(fc) if self.is_glu else K.gelu_fwd(fc)
+        act = K.act_fwd(fc, *self.act)
         if p_res > 0:  # gpt_dolomite/mlp.py:45-50 then layer.py:82-86
             y = self._linear(u, p + "mlp.c_proj.weight", act, p + "mlp.c_proj.bias")
             h = K.dropout_fwd(y, p_res, self._drop_keys(4 * i + 2), residual=h_mid, post_mul=m_res, out=y)
@@ -705,7 +705,7 @@ class DolomiteEngine:
                 h, _ = moe.forward(self, u, p, ln2, h_mid, m_res)
             else:
                 fc = K.gemm(ln2, u.views[p + "mlp.c_fc.weight"], bias=u.views.get(p + "mlp.c_fc.bias"))
-                act = K.swiglu_fwd(fc) if self.is_glu else K.gelu_fwd(fc)
+                act = K.act_fwd(fc, *self.act)
                 h = K.gemm(act, u.views[p + "mlp.c_proj.weight"], bias=u.views.get(p + "mlp.c_proj.bias"), c=h_mid, alpha=m_res,
                            beta=1.0)
         hf, _ = self._norm_fwd(h, root, "transformer.ln_f.")
@@ -867,9 +867,8 @@ class DolomiteEngine:
                     del d_y
                 else:
                     d_act = self._linear_bwd(u, p + "mlp.c_proj.weight", p + "mlp.c_proj.bias", act, dh, alpha=m_res)
-                # the c_fc bias gradient (column sums of d_fc) is accumulated by the SwiGLU backward while it writes d_fc
-                act_bwd = K.swiglu_bwd if self.is_glu else K.gelu_bwd
-                d_fc = act_bwd(d_act, fc, bias_grad_accum=u.gviews.get(p + "mlp.c_fc.bias"))
+                # the c_fc bias gradient (column sums of d_fc) is accumulated by the activation backward while it writes d_fc
+                d_fc = K.act_bwd(d_act, fc, *self.act, bias_grad_accum=u.gviews.get(p + "mlp.c_fc.bias"))
                 del d_act
                 d_ln2 = self._linear_bwd(u, p + "mlp.c_fc.weight", None, ln2, d_fc)
                 del d_fc

@@ -97,7 +97,7 @@ def rope_qk_inplace(qkv, n_groups: int, q_per_group: int, head_dim: int, cos, si
 
 
 # ------------------------------------------------------------------------------------------------
-# SwiGLU (activations/glu.py:26-28)
+# LayerNorm and the MLP activations (activations/{base,glu}.py)
 # ------------------------------------------------------------------------------------------------
 def layernorm_fwd(x, w, b, eps: float, out=None):
     """y = bf16((x - mean) * rstd * w + b) -> (y, mean, rstd)"""
@@ -118,6 +118,29 @@ def layernorm_bwd(dy, x, w, mean, rstd, dw_accum, db_accum, dx_add=None, out=Non
     ws = _workspace(_lib.load().dolomite_b200_layernorm_bwd_workspace_bytes(H), x.device)
     _lib.call("dolomite_b200_layernorm_bwd", dy.data_ptr(), x.data_ptr(), w.data_ptr(), mean.data_ptr(), rstd.data_ptr(),
               _ptr(dx_add), dx.data_ptr(), _ptr(dw_accum), _ptr(db_accum), ws.data_ptr(), T, H, _stream())
+    return dx
+
+
+def act_fwd(x, act_id: int, form: int, out=None):
+    """MLP activation (activations.resolve gives `act_id`, `form`): plain [T, F] -> [T, F]; GLU forms [T, 2F] -> [T, F]"""
+    _req(x, _BF16, "x")
+    T, W = x.shape
+    F = W if form == 0 else W // 2
+    y = torch.empty(T, F, dtype=_BF16, device=x.device) if out is None else out
+    _lib.call("dolomite_b200_act_fwd", act_id, form, x.data_ptr(), y.data_ptr(), T, F, _stream())
+    return y
+
+
+def act_bwd(dy, x, act_id: int, form: int, out=None, bias_grad_accum=None):
+    """dx of act_fwd; with `bias_grad_accum` (fp32, one per column of x) also += column sums of dx (bias gradient of c_fc)"""
+    _req(dy, _BF16, "dy"), _req(x, _BF16, "x")
+    T, W = x.shape
+    dx = torch.empty_like(x) if out is None else out
+    if bias_grad_accum is not None:
+        _req(bias_grad_accum, torch.float32, "bias_grad_accum")
+        assert bias_grad_accum.numel() == W
+    _lib.call("dolomite_b200_act_bwd", act_id, form, dy.data_ptr(), x.data_ptr(), dx.data_ptr(), _ptr(bias_grad_accum), T,
+              W if form == 0 else W // 2, _stream())
     return dx
 
 

@@ -2,8 +2,13 @@
 ScatterMoE, moe_dolomite/layer.py:51-95 SparseMoEBlock).
 
     router logits = x gate^T -> top-k on raw logits -> fp32 softmax over the k selected -> bf16 weights
-    tokens grouped by expert (segments padded to 128 rows)  -> grouped wgmma GEMM c_fc -> SwiGLU
-    -> grouped GEMM c_proj -> gate-weighted combine (+ m_residual scale + residual add fused)
+    tokens grouped by expert (segments padded to 128 rows)  -> grouped wgmma GEMM c_fc -> activation (any name
+    activations.resolve accepts) -> grouped GEMM c_proj -> gate-weighted combine (+ m_residual scale + residual add fused)
+
+Padding rows of a segment are zeros in the gathered input (or a copy of token 0's row with the fused gather), so their
+`act` rows are finite but not zero for functions with f(0) != 0 (sigmoid, softplus, hard_sigmoid, laplace, log_sigmoid).
+They never reach a result: the combine reads only the rows of `row_of_slot`, and the combine backward writes zero `dyg`
+rows for them, so they add exact zeros to the c_proj weight gradient and give zero `d_fc` rows to the c_fc one.
 
 ScatterMoE forbids biases (moe/scatter.py:22); so does this path.  Activations stay grouped between the two expert
 GEMMs exactly like `parallel_linear(grouped_out=True)` -> `parallel_linear(grouped_in=True, gates=...)`.
@@ -33,7 +38,7 @@ def forward(engine, unit, p: str, x, residual, m_res: float, layer: int = 0):
         fc = K.gemm_grouped_m_gather(x, unit.views[p + "mlp.c_fc.weight"], plan)
     else:
         fc = K.gemm_grouped_m(K.moe_gather(x, plan), unit.views[p + "mlp.c_fc.weight"], plan, b_mn=False)
-    act = K.swiglu_fwd(fc)
+    act = K.act_fwd(fc, *engine.act)
     yg = K.gemm_grouped_m(act, unit.views[p + "mlp.c_proj.weight"], plan, b_mn=False)
     p_res = engine._drop_p("resid_pdrop")
     if p_res > 0:  # moe/base.py:106-120: dropout on the combined expert output, then layer.py's `* m_residual` / `+ residual`
@@ -59,7 +64,7 @@ def backward(engine, unit, p: str, x, dh, m_res: float, saved, layer: int = 0):
     beta_fc = 0.0 if engine.take_fresh(p + "mlp.c_fc.weight") else 1.0
     K.gemm_grouped_k(dyg, act, plan, unit.gviews[p + "mlp.c_proj.weight"], beta=beta_proj)  # dWproj[e] (+)= dY_e^T act_e
     d_act = K.gemm_grouped_m(dyg, w_proj, plan, b_mn=True)                            # [rows, F]
-    d_fc = K.swiglu_bwd(d_act, fc)
+    d_fc = K.act_bwd(d_act, fc, *engine.act)
     xg = K.moe_gather(x, plan)  # grouped (zero-padded) copy of the block input: the contraction operand of the c_fc wgrad
     K.gemm_grouped_k(d_fc, xg, plan, unit.gviews[p + "mlp.c_fc.weight"], beta=beta_fc)  # dWfc[e] (+)= dfc_e^T x_e
     del xg

@@ -91,9 +91,53 @@ int dolomite_b200_layernorm_bwd(const void* dy, const void* x, const void* w, co
                                 int H, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * MLP activations -- activation_function of gpt_dolomite/mlp.py:27-36 and moe_dolomite/moe/base.py:88-93, resolved by
+ * hf_models/modeling_utils/activations/{__init__,base,glu}.py (host side: dolomite_engine_b200/activations.py).
+ * Functions (torch's default constructor arguments): */
+enum {
+    DOLO_ACT_CELU = 0,     /* alpha 1 */
+    DOLO_ACT_ELU,          /* alpha 1 */
+    DOLO_ACT_GELU,         /* exact erf */
+    DOLO_ACT_GELU_TANH,    /* approximate="tanh" */
+    DOLO_ACT_SELU,
+    DOLO_ACT_HARDSHRINK,   /* lambda 0.5 */
+    DOLO_ACT_HARDSIGMOID,
+    DOLO_ACT_HARDSWISH,
+    DOLO_ACT_HARDTANH,     /* [-1, 1] */
+    DOLO_ACT_LAPLACE,      /* transformers' LaplaceActivation, mu 0.707107, sigma 0.282095 */
+    DOLO_ACT_LEAKY_RELU,   /* slope 0.01 */
+    DOLO_ACT_LOG_SIGMOID,
+    DOLO_ACT_MISH,
+    DOLO_ACT_RELU,
+    DOLO_ACT_RELU2,        /* relu(x)^2 */
+    DOLO_ACT_RELU6,
+    DOLO_ACT_SIGMOID,
+    DOLO_ACT_SILU,
+    DOLO_ACT_SOFTPLUS,     /* beta 1, threshold 20 */
+    DOLO_ACT_SOFTSHRINK,   /* lambda 0.5 */
+    DOLO_ACT_SOFTSIGN,
+    DOLO_ACT_TANH,
+    DOLO_ACT_TANHSHRINK,
+    DOLO_ACT_COUNT
+};
+/* Forms:
+ *   DOLO_ACT_PLAIN        x [T, F]:  y = f(x)
+ *   DOLO_ACT_GLU          x [T, 2F] = [u | g]:  y = u * bf16(f(g))     (GLUActivation, activations/glu.py)
+ *   DOLO_ACT_SIGMOID_GLU  x [T, 2F] = [u | g]:  y = u * sigmoid(g), rounded once (nn.GLU, names "glu" / "sigmoid_glu");
+ *                         DOLO_ACT_SIGMOID only
+ * Where the reference's eager module rounds to bf16 more than once (laplace, softsign, tanhshrink) f rounds at the same
+ * points.  bwd: plain dx = dy * f'(x); both GLU forms du = dy * f(g), dg = dy * u * f'(g); f' takes torch autograd's
+ * value at non-differentiable points.  dbias_accum (fp32 [F] or [2F], may be null) += column sums of the bf16 dx (bias
+ * gradient of c_fc), summed in a fixed order.  F is a positive multiple of 8, pointers 16-byte aligned. */
+enum { DOLO_ACT_PLAIN = 0, DOLO_ACT_GLU = 1, DOLO_ACT_SIGMOID_GLU = 2 };
+int dolomite_b200_act_fwd(int act_id, int form, const void* x, void* y, int64_t T, int64_t F, void* stream);
+int dolomite_b200_act_bwd(int act_id, int form, const void* dy, const void* x, void* dx, float* dbias_accum, int64_t T,
+                          int64_t F, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * tanh-GELU -- activation_function "gelu_pytorch_tanh" (hf_models/modeling_utils/activations/base.py), the non-GLU MLP
  * of gpt_dolomite/mlp.py:45-50.  bwd: dx = dy * gelu'(x); dbias_accum (fp32 [F], may be null) += column sums of the
- * bf16 dx (bias gradient of c_fc).
+ * bf16 dx (bias gradient of c_fc).  Same kernels as dolomite_b200_act_fwd / _bwd(DOLO_ACT_GELU_TANH, DOLO_ACT_PLAIN).
  * ------------------------------------------------------------------------------------------------ */
 int dolomite_b200_gelu_fwd(const void* x, void* y, int64_t n, void* stream);
 int dolomite_b200_gelu_bwd(const void* dy, const void* x, void* dx, float* dbias_accum, int64_t T, int64_t F, void* stream);
@@ -101,6 +145,7 @@ int dolomite_b200_gelu_bwd(const void* dy, const void* x, void* dx, float* dbias
 /* ------------------------------------------------------------------------------------------------
  * SwiGLU -- hf_models/modeling_utils/activations/glu.py:26-28 with gpt_dolomite/mlp.py:54-55 ordering:
  *   x = [up | gate] (first F columns up, last F gate);  y = up * silu(gate).
+ *   Same kernels as dolomite_b200_act_fwd / _bwd(DOLO_ACT_SILU, DOLO_ACT_GLU).
  * ------------------------------------------------------------------------------------------------ */
 int dolomite_b200_swiglu_fwd(const void* x, void* y, int64_t T, int64_t F, void* stream);
 int dolomite_b200_swiglu_bwd(const void* dy, const void* x, void* dx, int64_t T, int64_t F, void* stream);
