@@ -101,6 +101,12 @@ SIGNATURES: dict[str, tuple] = {
         _I,
         [_P, _P, _L, _P, _P, _P, _P, _I, _L, _I, _I, _I, _I, _F, _F, _U, _U, _P, _P],
     ),
+    "dolomite_b200_attn_varlen_fwd_alibi": (_I, [_P, _L, _P, _P, _P, _I, _L, _I, _I, _I, _I, _F, _F, _U, _U, _P, _P]),
+    "dolomite_b200_attn_varlen_bwd_alibi": (
+        _I,
+        [_P, _P, _L, _P, _P, _P, _P, _I, _L, _I, _I, _I, _I, _F, _F, _U, _U, _P, _P, _P],
+    ),
+    "dolomite_b200_attn_decode_alibi": (_I, [_P, _L, _P, _P, _P, _P, _I, _L, _I, _I, _I, _F, _P, _P]),
 }
 
 _lib = None
@@ -152,6 +158,7 @@ KERNELS_PER_CALL = {
     "dolomite_b200_clip_coef": 1, "dolomite_b200_adamw_step": 1, "dolomite_b200_cast_f32_to_bf16": 1,
     "dolomite_b200_accum_bf16_into_f32": 1, "dolomite_b200_gemm_bf16": 1, "dolomite_b200_attn_varlen_fwd": 1,
     "dolomite_b200_attn_varlen_bwd": 3, "dolomite_b200_attn_varlen_fwd_dropout": 1, "dolomite_b200_attn_varlen_bwd_dropout": 3,
+    "dolomite_b200_attn_varlen_fwd_alibi": 1, "dolomite_b200_attn_varlen_bwd_alibi": 3, "dolomite_b200_attn_decode_alibi": 1,
     "dolomite_b200_dropout_fwd": 1, "dolomite_b200_dropout_bwd": 1, "dolomite_b200_gemm_bf16_tile_n": 0,
 }
 launch_counts: dict[str, int] = {}

@@ -21,6 +21,7 @@ struct BwdParams {
     int head_chunk_q;  // the same for the query heads of the dQ kernel
     int n_tile_slots;  // upper bound of the number of 128-row key (dK/dV) or query (dQ) tiles of a head
     AttnDropout drop;  // attention-probability dropout of the forward being differentiated (threshold 0: none)
+    const float* alibi_slopes;  // [n_heads] fp32, read by the ALIBI instances only
 };
 
 // Delta[h, t] = sum_d dO[t, h, d] * O[t, h, d].  Block = DELTA_TOK tokens: every thread takes 16-byte vectors of dO and O
@@ -67,6 +68,8 @@ __global__ void __launch_bounds__(256)
 //     dV_j += P^T dO_i            (RS, B = dO MN-major)
 //     dK_j += dS^T Q_i            (RS, B = Q  MN-major)
 // Thread 0 also issues the TMA loads (K_j, V_j once; Q_i, dO_i through a 2-stage ring).
+// ALIBI: P^T = exp2(log2(e) * (S^T*scale + bias_k) - LSE_i), the bias of the forward (one per key row of the thread); the
+// bias has no gradient, so dS^T is unchanged.
 // dQ has its own kernel (attn_dq_kernel below: one CTA per query tile walks the key tiles in order), so that every
 // gradient is summed in a fixed order and the backward is bit-identical from run to run -- adding the dQ contributions
 // of the key-tile CTAs with atomics would not be.
@@ -74,7 +77,7 @@ constexpr int BWD_THREADS = 256;
 constexpr int BWD_QT = 64;  // query rows per step
 constexpr int QDO_STAGES = 2;
 
-template <int HD>
+template <int HD, bool ALIBI>
 __global__ void __launch_bounds__(BWD_THREADS, 1)
     attn_bwd_kernel(const __grid_constant__ CUtensorMap tq64, const __grid_constant__ CUtensorMap tqR,
                     const __grid_constant__ CUtensorMap to64, const __grid_constant__ CUtensorMap toR, const BwdParams p) {
@@ -187,8 +190,11 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
         reg_fence<BWD_QT / 2>(dpt);
 
         // ---------------- P^T, dS^T ----------------
+        // ALIBI: log2(e) * bias of the key row, computed here rather than before the MMAs so that it is not live across them
+        const float slope = ALIBI ? __ldg(p.alibi_slopes + head) : 0.f;
 #pragma unroll
-        for (int h = 0; h < 2; ++h)
+        for (int h = 0; h < 2; ++h) {
+            const float bias_r = ALIBI ? attn_alibi_bias(slope, kr[h]) * ATT_LOG2E : 0.f;
 #pragma unroll
             for (int b = 0; b < BWD_QT / 8; ++b)
 #pragma unroll
@@ -196,7 +202,11 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
                     const int q = q0 + 8 * b + wc + e;
                     const int i = 4 * b + 2 * h + e;
                     const bool ok = q >= kr[h] && q < loc.doc_len;  // causal, and a real query of the document
-                    float pr = ok ? fast_exp2(fmaf(st[i], p.scale_log2, -lse_c[b][e])) : 0.f;
+                    float pr;
+                    if constexpr (ALIBI)
+                        pr = ok ? fast_exp2(fmaf(st[i], p.scale_log2, bias_r) - lse_c[b][e]) : 0.f;
+                    else
+                        pr = ok ? fast_exp2(fmaf(st[i], p.scale_log2, -lse_c[b][e])) : 0.f;
                     float dp = dpt[i];
                     if (drop) {
                         const float z = attn_drop_scale(p.drop, head_key, loc.doc_start + q, loc.doc_start + kr[h]);
@@ -207,6 +217,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
                     }
                     dpt[i] = p.scale * pr * (dp - del_c[b][e]);
                 }
+        }
         uint32_t pa[BWD_QT / 16][4], da[BWD_QT / 16][4];
 #pragma unroll
         for (int kk = 0; kk < BWD_QT / 16; ++kk) {
@@ -256,7 +267,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
     }
 }
 
-template <int HD>
+template <int HD, bool ALIBI>
 int launch_bwd(const void* dout, const void* qkv, int64_t row_stride, const BwdParams& p, cudaStream_t st) {
     using CH = HeadChunks<HD>;
     CUtensorMap tq64, tqR, to64, toR;
@@ -266,7 +277,7 @@ int launch_bwd(const void* dout, const void* qkv, int64_t row_stride, const BwdP
     if (rc) return rc;
     constexpr int smem_bytes = 1024 + 2 * CH::tile_bytes(ATT_TILE) + 2 * QDO_STAGES * CH::tile_bytes(BWD_QT) + 128;
     static_assert(smem_bytes <= 232448, "attention backward shared memory budget exceeded");
-    auto kern = attn_bwd_kernel<HD>;
+    auto kern = attn_bwd_kernel<HD, ALIBI>;
     static bool attr_set = false;
     if (!attr_set) {
         DOLO_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
@@ -286,11 +297,11 @@ int launch_bwd(const void* dout, const void* qkv, int64_t row_stride, const BwdP
 //     dS = scale * P o (dP - Delta_i)             (registers, P = exp2(S*scale - LSE_i))
 //     dQ_i += dS K_j                              (RS, B = K MN-major)
 // and finally writes dQ_i (bf16) into the q slots of dqkv.  Thread 0 issues the TMA loads: Q_i and dO_i once, (K_j, V_j)
-// through a 2-stage ring.
+// through a 2-stage ring.  ALIBI: P = exp2(log2(e) * (S*scale + bias_k) - LSE_i), one bias per key column of the thread.
 constexpr int DQ_THREADS = 256;
 constexpr int DQ_KT = 64;  // keys per step
 
-template <int HD>
+template <int HD, bool ALIBI>
 __global__ void __launch_bounds__(DQ_THREADS, 1)
     attn_dq_kernel(const __grid_constant__ CUtensorMap tq64, const __grid_constant__ CUtensorMap tqR,
                    const __grid_constant__ CUtensorMap to64, const __grid_constant__ CUtensorMap toR, const BwdParams p) {
@@ -354,6 +365,7 @@ __global__ void __launch_bounds__(DQ_THREADS, 1)
     const bool drop = p.drop.threshold != 0;
     const uint32_t head_key = dropout_head_key(uint32_t(head), p.drop.key0, p.drop.key1);
     const float log2e = 1.4426950408889634f;
+    const float slope = ALIBI ? __ldg(p.alibi_slopes + head) : 0.f;
     float lse_r[2], del_r[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -391,6 +403,24 @@ __global__ void __launch_bounds__(DQ_THREADS, 1)
         reg_fence<DQ_KT / 2>(sc);
         reg_fence<DQ_KT / 2>(dp);
 
+        if constexpr (ALIBI) {
+#pragma unroll
+            for (int b = 0; b < DQ_KT / 8; ++b)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int k = j * DQ_KT + 8 * b + wc + e;
+                    const float bl = attn_alibi_bias(slope, k) * ATT_LOG2E;
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int i = 4 * b + 2 * h + e;
+                        const bool ok = k <= qr[h] && qr[h] < loc.doc_len;
+                        const float pr = ok ? fast_exp2(fmaf(sc[i], p.scale_log2, bl) - lse_r[h]) : 0.f;
+                        float d = dp[i];
+                        if (drop) d *= attn_drop_scale(p.drop, head_key, loc.doc_start + qr[h], loc.doc_start + k);
+                        sc[i] = p.scale * pr * (d - del_r[h]);
+                    }
+                }
+        } else
 #pragma unroll
         for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -443,7 +473,7 @@ __global__ void __launch_bounds__(DQ_THREADS, 1)
     }
 }
 
-template <int HD>
+template <int HD, bool ALIBI>
 int launch_dq(const void* dout, const void* qkv, int64_t row_stride, const BwdParams& p, cudaStream_t st) {
     using CH = HeadChunks<HD>;
     CUtensorMap tq64, tqR, to64, toR;
@@ -453,7 +483,7 @@ int launch_dq(const void* dout, const void* qkv, int64_t row_stride, const BwdPa
     if (rc) return rc;
     constexpr int smem_bytes = 1024 + 2 * CH::tile_bytes(ATT_TILE) + 4 * CH::tile_bytes(DQ_KT) + 128;
     static_assert(smem_bytes <= 232448, "attention dQ shared memory budget exceeded");
-    auto kern = attn_dq_kernel<HD>;
+    auto kern = attn_dq_kernel<HD, ALIBI>;
     static bool attr_set = false;
     if (!attr_set) {
         DOLO_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
@@ -488,12 +518,24 @@ extern "C" int dolomite_b200_attn_varlen_bwd(const void* dout, const void* qkv, 
                                                  n_groups, q_per_group, head_dim, softmax_scale, 0.f, 0, 0, workspace, stream);
 }
 
-extern "C" int dolomite_b200_attn_varlen_bwd_dropout(const void* dout, const void* qkv, int64_t row_stride, const void* out,
-                                                     const float* lse, void* dqkv, const int32_t* cu_seqlens, int n_docs,
-                                                     int64_t T, int max_seqlen, int n_groups, int q_per_group,
-                                                     int head_dim, float softmax_scale, float dropout_p, uint32_t key0,
-                                                     uint32_t key1, void* workspace, void* stream) {
-    (void)max_seqlen;
+namespace {
+
+template <int HD>
+int launch_bwd_dq(const void* dout, const void* qkv, int64_t row_stride, const BwdParams& p, cudaStream_t st) {
+    int rc;
+    if (p.alibi_slopes != nullptr) {
+        rc = launch_bwd<HD, true>(dout, qkv, row_stride, p, st);
+        return rc ? rc : launch_dq<HD, true>(dout, qkv, row_stride, p, st);
+    }
+    rc = launch_bwd<HD, false>(dout, qkv, row_stride, p, st);
+    return rc ? rc : launch_dq<HD, false>(dout, qkv, row_stride, p, st);
+}
+
+// alibi_slopes == nullptr: the plain kernels
+int attn_bwd(const void* dout, const void* qkv, int64_t row_stride, const void* out, const float* lse, void* dqkv,
+             const int32_t* cu_seqlens, int n_docs, int64_t T, int n_groups, int q_per_group, int head_dim,
+             float softmax_scale, float dropout_p, uint32_t key0, uint32_t key1, const float* alibi_slopes, void* workspace,
+             void* stream) {
     DOLO_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, "attn_bwd: dropout_p=%f must be in [0, 1)", double(dropout_p));
     if (T == 0 || n_docs == 0) return DOLO_OK;
     DOLO_REQUIRE(n_groups > 0 && q_per_group > 0, "attn_bwd: bad head grouping");
@@ -504,6 +546,10 @@ extern "C" int dolomite_b200_attn_varlen_bwd_dropout(const void* dout, const voi
     DOLO_REQUIRE(T < (1ll << 31), "attn_bwd: T too large");
     const int nh = n_groups * q_per_group;
     DOLO_REQUIRE(int64_t(nh) * T < (1ll << 31), "attn_bwd: heads * T too large for the dQ tile reduce");
+    switch (head_dim) {
+        case 16: case 32: case 64: case 80: case 96: case 128: break;
+        default: return dolo_set_error("attn_bwd: unsupported head_dim %d (supported: 16,32,64,80,96,128)", head_dim);
+    }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     float* delta = static_cast<float*>(workspace);
     {
@@ -532,16 +578,36 @@ extern "C" int dolomite_b200_attn_varlen_bwd_dropout(const void* dout, const voi
     p.drop.keep_scale = 1.f / (1.f - dropout_p);
     p.drop.key0 = key0;
     p.drop.key1 = key1;
-    int rc;
+    p.alibi_slopes = alibi_slopes;
     switch (head_dim) {
-        case 16: rc = launch_bwd<16>(dout, qkv, row_stride, p, st); if (!rc) rc = launch_dq<16>(dout, qkv, row_stride, p, st); break;
-        case 32: rc = launch_bwd<32>(dout, qkv, row_stride, p, st); if (!rc) rc = launch_dq<32>(dout, qkv, row_stride, p, st); break;
-        case 64: rc = launch_bwd<64>(dout, qkv, row_stride, p, st); if (!rc) rc = launch_dq<64>(dout, qkv, row_stride, p, st); break;
-        case 80: rc = launch_bwd<80>(dout, qkv, row_stride, p, st); if (!rc) rc = launch_dq<80>(dout, qkv, row_stride, p, st); break;
-        case 96: rc = launch_bwd<96>(dout, qkv, row_stride, p, st); if (!rc) rc = launch_dq<96>(dout, qkv, row_stride, p, st); break;
-        case 128: rc = launch_bwd<128>(dout, qkv, row_stride, p, st); if (!rc) rc = launch_dq<128>(dout, qkv, row_stride, p, st); break;
-        default: return dolo_set_error("attn_bwd: unsupported head_dim %d (supported: 16,32,64,80,96,128)", head_dim);
+        case 16: return launch_bwd_dq<16>(dout, qkv, row_stride, p, st);
+        case 32: return launch_bwd_dq<32>(dout, qkv, row_stride, p, st);
+        case 64: return launch_bwd_dq<64>(dout, qkv, row_stride, p, st);
+        case 80: return launch_bwd_dq<80>(dout, qkv, row_stride, p, st);
+        case 96: return launch_bwd_dq<96>(dout, qkv, row_stride, p, st);
+        default: return launch_bwd_dq<128>(dout, qkv, row_stride, p, st);
     }
-    if (rc) return rc;
-    return DOLO_OK;
+}
+
+}  // namespace
+
+extern "C" int dolomite_b200_attn_varlen_bwd_dropout(const void* dout, const void* qkv, int64_t row_stride, const void* out,
+                                                     const float* lse, void* dqkv, const int32_t* cu_seqlens, int n_docs,
+                                                     int64_t T, int max_seqlen, int n_groups, int q_per_group,
+                                                     int head_dim, float softmax_scale, float dropout_p, uint32_t key0,
+                                                     uint32_t key1, void* workspace, void* stream) {
+    (void)max_seqlen;
+    return attn_bwd(dout, qkv, row_stride, out, lse, dqkv, cu_seqlens, n_docs, T, n_groups, q_per_group, head_dim,
+                    softmax_scale, dropout_p, key0, key1, nullptr, workspace, stream);
+}
+
+extern "C" int dolomite_b200_attn_varlen_bwd_alibi(const void* dout, const void* qkv, int64_t row_stride, const void* out,
+                                                   const float* lse, void* dqkv, const int32_t* cu_seqlens, int n_docs,
+                                                   int64_t T, int max_seqlen, int n_groups, int q_per_group, int head_dim,
+                                                   float softmax_scale, float dropout_p, uint32_t key0, uint32_t key1,
+                                                   const float* alibi_slopes, void* workspace, void* stream) {
+    (void)max_seqlen;
+    DOLO_REQUIRE(alibi_slopes != nullptr, "attn_bwd_alibi: alibi_slopes is null");
+    return attn_bwd(dout, qkv, row_stride, out, lse, dqkv, cu_seqlens, n_docs, T, n_groups, q_per_group, head_dim,
+                    softmax_scale, dropout_p, key0, key1, alibi_slopes, workspace, stream);
 }

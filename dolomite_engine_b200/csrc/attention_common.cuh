@@ -93,6 +93,16 @@ __device__ __forceinline__ float attn_drop_scale(const AttnDropout& d, uint32_t 
     return dropout_hash_qk(uint32_t(q_tok), uint32_t(k_tok), head_key) >= d.threshold ? d.keep_scale : 0.f;
 }
 
+// ALiBi (modeling_utils/position_embedding/alibi.py:14-30, gpt_dolomite/base.py:261-287): the logit of (query, key) of
+// head h gets bias = slope_h * kpos, where kpos is the key's index inside its document (the packed form of
+// `cumsum(attention_mask) - 1`) or inside the KV cache.  The reference casts the bias to the hidden-state dtype, so it is
+// bf16(fp32(slope) * kpos); the slopes are the reference's fp32 values, computed on the host.
+__device__ __forceinline__ float attn_alibi_bias(float slope, int kpos) {
+    return __bfloat162float(__float2bfloat16_rn(slope * float(kpos)));
+}
+constexpr float ATT_LOG2E = 1.4426950408889634f;
+constexpr float ATT_LN2 = 0.6931471805599453f;
+
 // CTA order of the attention grids (1-D grid of n_tile_slots x n_heads CTAs, dispatched in index order).  Heads are taken
 // in CHUNKS of `chunk`; inside a chunk the heads are the fastest index and the tile the slower one, and the callers walk the
 // tiles of a document longest first.  The last wave of a chunk then holds short tiles only and the next chunk's long tiles

@@ -10,7 +10,10 @@
 // Cache layout: k_cache / v_cache [B, L_max, n_groups * head_dim] bf16 (position-major per sequence); `lens[b]` = number of
 // valid positions INCLUDING the token being decoded.  The query comes straight out of the packed c_attn output (slot layout of
 // attention/padding_free.py:79-116), one row per sequence.
-#include "common.cuh"
+// ALIBI: the score of a key gets the bias of its cache position (attn_alibi_bias, attention_common.cuh): the cache holds the
+// real tokens of a sequence from position 0 (hf_models/generation.py:56-79), so the position is the reference's
+// `cumsum(attention_mask) - 1`.
+#include "attention_common.cuh"
 #include "../../include/dolomite_b200.h"
 
 using namespace dolo;
@@ -19,11 +22,12 @@ namespace {
 
 constexpr int DEC_THREADS = 128;
 
-template <int HD>
+template <int HD, bool ALIBI>
 __global__ void __launch_bounds__(DEC_THREADS)
     attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int64_t row_stride, const __nv_bfloat16* __restrict__ k_cache,
                        const __nv_bfloat16* __restrict__ v_cache, const int32_t* __restrict__ lens,
-                       __nv_bfloat16* __restrict__ out, int64_t L_max, int n_groups, int q_per_group, float scale_log2) {
+                       __nv_bfloat16* __restrict__ out, int64_t L_max, int n_groups, int q_per_group, float scale_log2,
+                       const float* __restrict__ alibi_slopes) {
     static_assert(HD % 8 == 0 && HD <= DEC_THREADS, "one thread per output column");
     __shared__ __align__(16) float sq[HD];
     __shared__ float sp[DEC_THREADS];
@@ -41,6 +45,7 @@ __global__ void __launch_bounds__(DEC_THREADS)
     const __nv_bfloat16* kb = k_cache + (int64_t(b) * L_max) * kv_stride + int64_t(group) * HD;
     const __nv_bfloat16* vb = v_cache + (int64_t(b) * L_max) * kv_stride + int64_t(group) * HD;
     float m_run = -INFINITY, l_run = 0.f, acc = 0.f;
+    const float slope = ALIBI ? __ldg(alibi_slopes + head) : 0.f;
     for (int base = 0; base < len; base += DEC_THREADS) {
         // ---- phase A: one key per thread ----
         const int key = base + t;
@@ -56,7 +61,10 @@ __global__ void __launch_bounds__(DEC_THREADS)
                 dot += bf16_lo(kk.x) * qa.x + bf16_hi(kk.x) * qa.y + bf16_lo(kk.y) * qa.z + bf16_hi(kk.y) * qa.w;
                 dot += bf16_lo(kk.z) * qb.x + bf16_hi(kk.z) * qb.y + bf16_lo(kk.w) * qb.z + bf16_hi(kk.w) * qb.w;
             }
-            s = dot * scale_log2;  // log2 units
+            if constexpr (ALIBI)
+                s = fmaf(dot, scale_log2, attn_alibi_bias(slope, key) * ATT_LOG2E);
+            else
+                s = dot * scale_log2;  // log2 units
         }
         float cm = warp_max(s);
         if (lane == 0) red[wid] = cm;
@@ -95,23 +103,37 @@ __global__ void __launch_bounds__(DEC_THREADS)
     if (t < HD) out[int64_t(b) * (int64_t(n_heads) * HD) + int64_t(head) * HD + t] = __float2bfloat16_rn(l_run > 0.f ? acc / l_run : 0.f);
 }
 
-template <int HD>
+template <int HD, bool ALIBI>
 int launch_decode(const void* qkv, int64_t row_stride, const void* k_cache, const void* v_cache, const int32_t* lens, void* out,
-                  int B, int64_t L_max, int n_groups, int q_per_group, float scale, cudaStream_t st) {
+                  int B, int64_t L_max, int n_groups, int q_per_group, float scale, const float* alibi_slopes, cudaStream_t st) {
     dim3 grid((unsigned)B, (unsigned)(n_groups * q_per_group));
-    attn_decode_kernel<HD><<<grid, DEC_THREADS, 0, st>>>(
+    attn_decode_kernel<HD, ALIBI><<<grid, DEC_THREADS, 0, st>>>(
         static_cast<const __nv_bfloat16*>(qkv), row_stride, static_cast<const __nv_bfloat16*>(k_cache),
         static_cast<const __nv_bfloat16*>(v_cache), lens, static_cast<__nv_bfloat16*>(out), L_max, n_groups, q_per_group,
-        scale * 1.4426950408889634f);
+        scale * 1.4426950408889634f, alibi_slopes);
     DOLO_LAUNCH_OK("attn_decode");
     return DOLO_OK;
 }
 
 }  // namespace
 
-extern "C" int dolomite_b200_attn_decode(const void* qkv, int64_t row_stride, const void* k_cache, const void* v_cache,
-                                         const int32_t* lens, void* out, int batch, int64_t L_max, int n_groups,
-                                         int q_per_group, int head_dim, float softmax_scale, void* stream) {
+namespace {
+
+template <int HD>
+int launch_decode_any(const void* qkv, int64_t row_stride, const void* k_cache, const void* v_cache, const int32_t* lens,
+                      void* out, int B, int64_t L_max, int n_groups, int q_per_group, float scale, const float* alibi_slopes,
+                      cudaStream_t st) {
+    if (alibi_slopes != nullptr)
+        return launch_decode<HD, true>(qkv, row_stride, k_cache, v_cache, lens, out, B, L_max, n_groups, q_per_group, scale,
+                                       alibi_slopes, st);
+    return launch_decode<HD, false>(qkv, row_stride, k_cache, v_cache, lens, out, B, L_max, n_groups, q_per_group, scale,
+                                    nullptr, st);
+}
+
+// alibi_slopes == nullptr: the plain kernel
+int attn_decode(const void* qkv, int64_t row_stride, const void* k_cache, const void* v_cache, const int32_t* lens, void* out,
+                int batch, int64_t L_max, int n_groups, int q_per_group, int head_dim, float softmax_scale,
+                const float* alibi_slopes, void* stream) {
     DOLO_REQUIRE(batch >= 0 && L_max > 0, "attn_decode: bad sizes");
     if (batch == 0) return DOLO_OK;
     DOLO_REQUIRE(n_groups > 0 && q_per_group > 0, "attn_decode: bad head grouping");
@@ -120,12 +142,30 @@ extern "C" int dolomite_b200_attn_decode(const void* qkv, int64_t row_stride, co
                  "attn_decode: alignment");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     switch (head_dim) {
-        case 16: return launch_decode<16>(qkv, row_stride, k_cache, v_cache, lens, out, batch, L_max, n_groups, q_per_group, softmax_scale, st);
-        case 32: return launch_decode<32>(qkv, row_stride, k_cache, v_cache, lens, out, batch, L_max, n_groups, q_per_group, softmax_scale, st);
-        case 64: return launch_decode<64>(qkv, row_stride, k_cache, v_cache, lens, out, batch, L_max, n_groups, q_per_group, softmax_scale, st);
-        case 80: return launch_decode<80>(qkv, row_stride, k_cache, v_cache, lens, out, batch, L_max, n_groups, q_per_group, softmax_scale, st);
-        case 96: return launch_decode<96>(qkv, row_stride, k_cache, v_cache, lens, out, batch, L_max, n_groups, q_per_group, softmax_scale, st);
-        case 128: return launch_decode<128>(qkv, row_stride, k_cache, v_cache, lens, out, batch, L_max, n_groups, q_per_group, softmax_scale, st);
+        case 16: return launch_decode_any<16>(qkv, row_stride, k_cache, v_cache, lens, out, batch, L_max, n_groups, q_per_group, softmax_scale, alibi_slopes, st);
+        case 32: return launch_decode_any<32>(qkv, row_stride, k_cache, v_cache, lens, out, batch, L_max, n_groups, q_per_group, softmax_scale, alibi_slopes, st);
+        case 64: return launch_decode_any<64>(qkv, row_stride, k_cache, v_cache, lens, out, batch, L_max, n_groups, q_per_group, softmax_scale, alibi_slopes, st);
+        case 80: return launch_decode_any<80>(qkv, row_stride, k_cache, v_cache, lens, out, batch, L_max, n_groups, q_per_group, softmax_scale, alibi_slopes, st);
+        case 96: return launch_decode_any<96>(qkv, row_stride, k_cache, v_cache, lens, out, batch, L_max, n_groups, q_per_group, softmax_scale, alibi_slopes, st);
+        case 128: return launch_decode_any<128>(qkv, row_stride, k_cache, v_cache, lens, out, batch, L_max, n_groups, q_per_group, softmax_scale, alibi_slopes, st);
         default: return dolo_set_error("attn_decode: unsupported head_dim %d (supported: 16,32,64,80,96,128)", head_dim);
     }
+}
+
+}  // namespace
+
+extern "C" int dolomite_b200_attn_decode(const void* qkv, int64_t row_stride, const void* k_cache, const void* v_cache,
+                                         const int32_t* lens, void* out, int batch, int64_t L_max, int n_groups,
+                                         int q_per_group, int head_dim, float softmax_scale, void* stream) {
+    return attn_decode(qkv, row_stride, k_cache, v_cache, lens, out, batch, L_max, n_groups, q_per_group, head_dim,
+                       softmax_scale, nullptr, stream);
+}
+
+extern "C" int dolomite_b200_attn_decode_alibi(const void* qkv, int64_t row_stride, const void* k_cache, const void* v_cache,
+                                               const int32_t* lens, void* out, int batch, int64_t L_max, int n_groups,
+                                               int q_per_group, int head_dim, float softmax_scale,
+                                               const float* alibi_slopes, void* stream) {
+    DOLO_REQUIRE(alibi_slopes != nullptr, "attn_decode_alibi: alibi_slopes is null");
+    return attn_decode(qkv, row_stride, k_cache, v_cache, lens, out, batch, L_max, n_groups, q_per_group, head_dim,
+                       softmax_scale, alibi_slopes, stream);
 }

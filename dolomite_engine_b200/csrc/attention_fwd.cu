@@ -7,6 +7,8 @@
 //     online softmax     (each thread holds two query rows x 32 keys; row max / sum over the quad of a row)
 //     O += P V_j         (wgmma RS: P as the bf16 register A operand, V MN-major from shared memory)
 // and finally writes O / l and the natural-log LSE.
+// ALIBI: the logits are scale * s + bias_k with a per-(head, key) bias (see attn_alibi_bias); the running row max is then
+// kept in log2 units of the biased logit instead of in raw-score units.
 #include "attention_common.cuh"
 #include "../../include/dolomite_b200.h"
 
@@ -30,9 +32,10 @@ struct FwdParams {
     AttnDropout drop;  // threshold 0: none
     int head_chunk;    // CTA order (attention_common.cuh: attn_cta_order): heads per chunk, 0 = tiles fastest
     int n_tile_slots;  // upper bound of the number of query tiles (the grid has n_tile_slots x n_heads CTAs)
+    const float* alibi_slopes;  // [n_heads] fp32, read by the ALIBI instances only
 };
 
-template <int HD>
+template <int HD, bool ALIBI>
 __global__ void __launch_bounds__(FWD_THREADS, 1)
     attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap64, const __grid_constant__ CUtensorMap tmapR,
                     const FwdParams p) {
@@ -93,7 +96,9 @@ __global__ void __launch_bounds__(FWD_THREADS, 1)
     float o[HD / 2];
 #pragma unroll
     for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
-    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};  // raw-score row max, thread-partial row sum
+    // row max (raw score; ALIBI: log2 units of the biased logit), thread-partial row sum
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+    const float slope = ALIBI ? __ldg(p.alibi_slopes + head) : 0.f;
 
     mbar_wait(q_full, 0, 10);
     for (int j = 0; j < n_kv; ++j) {
@@ -117,6 +122,16 @@ __global__ void __launch_bounds__(FWD_THREADS, 1)
         // ---------------- online softmax over this key tile ----------------
         const bool diag = j == loc.tile;  // only the diagonal tile has keys past a query of the tile
         const int kbase = j * ATT_TILE + wc;
+        if constexpr (ALIBI) {  // sc <- log2(e) * (scale * s + bias_k): one bias per key column, shared by both rows
+#pragma unroll
+            for (int b = 0; b < ATT_TILE / 8; ++b)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const float bl = attn_alibi_bias(slope, kbase + 8 * b + e) * ATT_LOG2E;
+                    sc[4 * b + e] = fmaf(sc[4 * b + e], p.scale_log2, bl);
+                    sc[4 * b + 2 + e] = fmaf(sc[4 * b + 2 + e], p.scale_log2, bl);
+                }
+        }
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             float mx = m_run[h];
@@ -131,15 +146,16 @@ __global__ void __launch_bounds__(FWD_THREADS, 1)
             mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
             mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
             // key 0 of every tile j <= tile precedes every query of the tile: the row max is finite from tile 0 on
-            const float corr = fast_exp2((m_run[h] - mx) * p.scale_log2);
-            const float neg_m = -mx * p.scale_log2;
+            const float corr = ALIBI ? fast_exp2(m_run[h] - mx) : fast_exp2((m_run[h] - mx) * p.scale_log2);
+            const float neg_m = ALIBI ? -mx : -mx * p.scale_log2;
             float lsum = 0.f;
 #pragma unroll
             for (int b = 0; b < ATT_TILE / 8; ++b)
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                     float& x = sc[4 * b + 2 * h + e];
-                    float pr = fast_exp2(fmaf(x, p.scale_log2, neg_m));  // exp2(-inf) = 0 for masked keys
+                    // exp2(-inf) = 0 for masked keys
+                    float pr = ALIBI ? fast_exp2(x + neg_m) : fast_exp2(fmaf(x, p.scale_log2, neg_m));
                     lsum += pr;
                     if (drop)  // the row sum above is that of the undropped probabilities
                         pr *= attn_drop_scale(p.drop, head_key, loc.doc_start + qr[h], loc.doc_start + kbase + 8 * b + e);
@@ -194,11 +210,12 @@ __global__ void __launch_bounds__(FWD_THREADS, 1)
 #pragma unroll
         for (int b = 0; b < HD / 8; ++b)
             *reinterpret_cast<uint32_t*>(orow + 8 * b) = pack_bf16(o[4 * b + 2 * h] * inv_l, o[4 * b + 2 * h + 1] * inv_l);
-        if ((lane & 3) == 0) p.lse[int64_t(head) * p.T + row] = m_run[h] * p.scale + logf(l);
+        if ((lane & 3) == 0)
+            p.lse[int64_t(head) * p.T + row] = (ALIBI ? m_run[h] * ATT_LN2 : m_run[h] * p.scale) + logf(l);
     }
 }
 
-template <int HD>
+template <int HD, bool ALIBI>
 int launch_fwd(const void* qkv, int64_t row_stride, const FwdParams& p, cudaStream_t st) {
     using CH = HeadChunks<HD>;
     CUtensorMap t64, tR;
@@ -206,7 +223,7 @@ int launch_fwd(const void* qkv, int64_t row_stride, const FwdParams& p, cudaStre
     if (rc) return rc;
     constexpr int smem_bytes = 1024 + (1 + 2 * KV_STAGES) * CH::tile_bytes(ATT_TILE) + 128;
     static_assert(smem_bytes <= 232448, "attention forward shared memory budget exceeded");
-    auto kern = attn_fwd_kernel<HD>;
+    auto kern = attn_fwd_kernel<HD, ALIBI>;
     static bool attr_set = false;
     if (!attr_set) {
         DOLO_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
@@ -233,10 +250,12 @@ extern "C" int dolomite_b200_attn_varlen_fwd(const void* qkv, int64_t row_stride
                                                  q_per_group, head_dim, softmax_scale, 0.f, 0, 0, stream);
 }
 
-extern "C" int dolomite_b200_attn_varlen_fwd_dropout(const void* qkv, int64_t row_stride, void* out, float* lse,
-                                                     const int32_t* cu_seqlens, int n_docs, int64_t T, int max_seqlen,
-                                                     int n_groups, int q_per_group, int head_dim, float softmax_scale,
-                                                     float dropout_p, uint32_t key0, uint32_t key1, void* stream) {
+namespace {
+
+// alibi_slopes == nullptr: the plain kernels
+int attn_fwd(const void* qkv, int64_t row_stride, void* out, float* lse, const int32_t* cu_seqlens, int n_docs, int64_t T,
+             int n_groups, int q_per_group, int head_dim, float softmax_scale, float dropout_p, uint32_t key0, uint32_t key1,
+             const float* alibi_slopes, void* stream) {
     DOLO_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, "attn_fwd: dropout_p=%f must be in [0, 1)", double(dropout_p));
     DOLO_REQUIRE(n_docs >= 0 && T >= 0, "attn_fwd: negative sizes");
     if (T == 0 || n_docs == 0) return DOLO_OK;
@@ -264,15 +283,38 @@ extern "C" int dolomite_b200_attn_varlen_fwd_dropout(const void* qkv, int64_t ro
     // all heads in one chunk when the K / V of the whole batch stay in L2 anyway (GQA / short batches): nothing to lose to
     // re-reads, and the longest-first order then spans every head
     if (p.head_chunk > 0 && T * int64_t(n_groups) * head_dim * 4 <= (24ll << 20)) p.head_chunk = p.n_heads;
+    p.alibi_slopes = alibi_slopes;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    (void)max_seqlen;
+    const bool ab = alibi_slopes != nullptr;
     switch (head_dim) {
-        case 16: return launch_fwd<16>(qkv, row_stride, p, st);
-        case 32: return launch_fwd<32>(qkv, row_stride, p, st);
-        case 64: return launch_fwd<64>(qkv, row_stride, p, st);
-        case 80: return launch_fwd<80>(qkv, row_stride, p, st);
-        case 96: return launch_fwd<96>(qkv, row_stride, p, st);
-        case 128: return launch_fwd<128>(qkv, row_stride, p, st);
+        case 16: return ab ? launch_fwd<16, true>(qkv, row_stride, p, st) : launch_fwd<16, false>(qkv, row_stride, p, st);
+        case 32: return ab ? launch_fwd<32, true>(qkv, row_stride, p, st) : launch_fwd<32, false>(qkv, row_stride, p, st);
+        case 64: return ab ? launch_fwd<64, true>(qkv, row_stride, p, st) : launch_fwd<64, false>(qkv, row_stride, p, st);
+        case 80: return ab ? launch_fwd<80, true>(qkv, row_stride, p, st) : launch_fwd<80, false>(qkv, row_stride, p, st);
+        case 96: return ab ? launch_fwd<96, true>(qkv, row_stride, p, st) : launch_fwd<96, false>(qkv, row_stride, p, st);
+        case 128: return ab ? launch_fwd<128, true>(qkv, row_stride, p, st) : launch_fwd<128, false>(qkv, row_stride, p, st);
         default: return dolo_set_error("attn_fwd: unsupported head_dim %d (supported: 16,32,64,80,96,128)", head_dim);
     }
+}
+
+}  // namespace
+
+extern "C" int dolomite_b200_attn_varlen_fwd_dropout(const void* qkv, int64_t row_stride, void* out, float* lse,
+                                                     const int32_t* cu_seqlens, int n_docs, int64_t T, int max_seqlen,
+                                                     int n_groups, int q_per_group, int head_dim, float softmax_scale,
+                                                     float dropout_p, uint32_t key0, uint32_t key1, void* stream) {
+    (void)max_seqlen;
+    return attn_fwd(qkv, row_stride, out, lse, cu_seqlens, n_docs, T, n_groups, q_per_group, head_dim, softmax_scale,
+                    dropout_p, key0, key1, nullptr, stream);
+}
+
+extern "C" int dolomite_b200_attn_varlen_fwd_alibi(const void* qkv, int64_t row_stride, void* out, float* lse,
+                                                   const int32_t* cu_seqlens, int n_docs, int64_t T, int max_seqlen,
+                                                   int n_groups, int q_per_group, int head_dim, float softmax_scale,
+                                                   float dropout_p, uint32_t key0, uint32_t key1,
+                                                   const float* alibi_slopes, void* stream) {
+    (void)max_seqlen;
+    DOLO_REQUIRE(alibi_slopes != nullptr, "attn_fwd_alibi: alibi_slopes is null");
+    return attn_fwd(qkv, row_stride, out, lse, cu_seqlens, n_docs, T, n_groups, q_per_group, head_dim, softmax_scale,
+                    dropout_p, key0, key1, alibi_slopes, stream);
 }

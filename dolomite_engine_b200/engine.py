@@ -190,13 +190,24 @@ def _root_specs(cfg: CommonConfig) -> list[tuple[str, tuple, str]]:
     return specs
 
 
-def check_supported(cfg: CommonConfig) -> None:
+def check_supported(cfg: CommonConfig, *, attention_implementation: str = "flash_attention_2",
+                    use_padding_free_transformer: bool = True) -> None:
     """The B200 hot path implements the configurations SURVEY.md section 8 puts in scope; everything else raises
-    (mirrors the reference's NotImplementedError / ValueError conventions, SURVEY section 8b)."""
-    if cfg.position_embedding_type not in ("rope", "nope", "learned_absolute"):
+    (mirrors the reference's NotImplementedError / ValueError conventions, SURVEY section 8b).  The keyword arguments are
+    the model's `attn_implementation` / `use_padding_free_transformer`; only alibi depends on them."""
+    if cfg.position_embedding_type not in ("rope", "nope", "learned_absolute", "alibi"):
         raise NotImplementedError(
-            f"position_embedding_type={cfg.position_embedding_type!r}: the B200 path implements rope, nope and "
-            "learned_absolute (alibi is unsupported with flash attention in the reference too, gpt_dolomite/base.py:530)"
+            f"position_embedding_type={cfg.position_embedding_type!r}: the B200 path implements rope, nope, "
+            "learned_absolute and alibi"
+        )
+    if cfg.position_embedding_type == "alibi" and (
+        attention_implementation == "flash_attention_2" or use_padding_free_transformer
+    ):
+        # gpt_dolomite/base.py:529-530 asserts the same for flash attention; the padding-free transformer needs flash
+        raise NotImplementedError(
+            "position_embedding_type='alibi' runs with attn_implementation 'eager' or 'sdpa' and "
+            "use_padding_free_transformer=False (the reference: alibi is not implemented with flash attention, "
+            "gpt_dolomite/base.py:530)"
         )
     if cfg.rope_scaling is not None:
         rs = cfg.rope_scaling
@@ -230,8 +241,10 @@ class DolomiteEngine:
     """Owns the flat units of one model replica/shard and runs the explicit forward / backward."""
 
     def __init__(self, cfg: CommonConfig, device, world_size: int = 1, rank: int = 0, seed: int | None = 42,
-                 init_on_device: bool = False):
-        check_supported(cfg)
+                 init_on_device: bool = False, attention_implementation: str = "flash_attention_2",
+                 use_padding_free_transformer: bool = True):
+        check_supported(cfg, attention_implementation=attention_implementation,
+                        use_padding_free_transformer=use_padding_free_transformer)
         self.cfg = cfg
         self.device = torch.device(device)
         self.world_size, self.rank = world_size, rank
@@ -261,6 +274,15 @@ class DolomiteEngine:
             for u in self.units:
                 u.full_master_from(u.init_full(g))
         self._setup_rope()
+        # ALiBi: the slopes stay on the device (a non-persistent buffer in the reference: not part of the state dict).
+        # Whether a pass applies the bias is decided per forward (`alibi=`), as the reference decides per call
+        # (gpt_dolomite/base.py:559-598); backward and recomputed blocks reuse the decision of their forward.
+        self.alibi_slopes = None
+        if cfg.position_embedding_type == "alibi":
+            from .alibi import alibi_slopes
+
+            self.alibi_slopes = alibi_slopes(cfg.n_head).to(self.device)
+        self._alibi_now = None  # slopes of the pass being run / backpropagated; None = no bias
         self.comm = None  # set by distributed.ShardedDataParallel
         self._saved = None
         self.requires_gradient_sync = True
@@ -522,7 +544,8 @@ class DolomiteEngine:
             self._kv_sink(i, qkv)
         p_att = self._drop_p("attn_pdrop")
         attn, lse = K.attn_varlen_fwd(qkv, cu_seqlens, max_seqlen, self.n_groups, self.q_per_group, self.hd, self.softmax_scale,
-                                      dropout_p=p_att, dropout_keys=self._drop_keys(4 * i + 3) if p_att > 0 else (0, 0))
+                                      dropout_p=p_att, dropout_keys=self._drop_keys(4 * i + 3) if p_att > 0 else (0, 0),
+                                      alibi_slopes=self._alibi_now)
         p_res = self._drop_p("resid_pdrop")
         if p_res > 0:  # resid_dropout sits between c_proj and `* m_residual` / `+ residual` (padding_free.py:75, layer.py:73-77)
             y = self._linear(u, p + "attn.c_proj.weight", attn, p + "attn.c_proj.bias")
@@ -545,12 +568,15 @@ class DolomiteEngine:
         return h, (x_in, rstd1, ln1, qkv, attn, lse, h_mid, rstd2, ln2, fc, act)
 
     def forward(self, input_ids, position_ids, cu_seqlens, max_seqlen: int, labels=None, ignore_index: int = -100,
-                save_for_backward: bool = True, fuse_head_loss: bool = False):
+                save_for_backward: bool = True, fuse_head_loss: bool = False, alibi: bool = False):
         """Returns (logits_or_None, loss_or_None).  input_ids int64 [T]; cu_seqlens int32 [B+1].
         `fuse_head_loss`: the caller will backpropagate d(loss) = 1 (what train_step does), so the LM head's backward can run
-        chunk-wise inside the loss computation and the [T, V] logits are never materialised."""
+        chunk-wise inside the loss computation and the [T, V] logits are never materialised.
+        `alibi`: add the ALiBi bias of an alibi model to the attention logits (the key's index inside its document);
+        False runs an alibi model as NoPE, which is what the reference's SDPA attention does without an attention mask."""
         cfg = self.cfg
         self._begin_dropout_pass()
+        self._alibi_now = self._alibi_slopes_for(alibi)
         self._fp8_now = self.fp8 is not None and self.fp8_autocast and self.training and save_for_backward
         self._fp8_wcache.clear()
         T = input_ids.numel()
@@ -621,10 +647,17 @@ class DolomiteEngine:
         if save_for_backward:
             self._saved = dict(input_ids=input_ids, position_ids=position_ids, cu_seqlens=cu_seqlens, max_seqlen=max_seqlen,
                                layers=saved_layers, h_last=h, rstd_f=rstd_f, hf=hf, dlogits=dlogits, d_hf=d_hf, T=T,
-                               dropout_seed=self._dropout_now, fp8=self._fp8_now)
+                               dropout_seed=self._dropout_now, fp8=self._fp8_now, alibi=self._alibi_now)
         self._fp8_now = False
         self._fp8_wcache.clear()
         return logits_out, loss
+
+    def _alibi_slopes_for(self, alibi: bool):
+        if not alibi:
+            return None
+        if self.alibi_slopes is None:
+            raise ValueError("alibi=True needs a model with position_embedding_type='alibi'")
+        return self.alibi_slopes
 
     @staticmethod
     def _head_chunk_rows(T: int, V: int, budget_bytes: int = 1 << 30, multiple: int = 8) -> int:
@@ -645,7 +678,8 @@ class DolomiteEngine:
         return slots[:, :, self.q_per_group], slots[:, :, self.q_per_group + 1]
 
     @torch.no_grad()
-    def prefill(self, input_ids, position_ids, cu_seqlens, max_seqlen: int, cache: "KVCache", n_sequences: int | None = None):
+    def prefill(self, input_ids, position_ids, cu_seqlens, max_seqlen: int, cache: "KVCache", n_sequences: int | None = None,
+                alibi: bool = False):
         """packed forward over the prompts (document b = sequence b for b < n_sequences; later documents, e.g. the alignment
         dummy of `_pad_packed_stream`, are run but not cached) that also fills `cache`; -> logits [T, V]"""
         cu = cu_seqlens.tolist()
@@ -661,18 +695,20 @@ class DolomiteEngine:
 
         self._kv_sink = sink
         try:
-            logits, _ = self.forward(input_ids, position_ids, cu_seqlens, max_seqlen, save_for_backward=False)
+            logits, _ = self.forward(input_ids, position_ids, cu_seqlens, max_seqlen, save_for_backward=False, alibi=alibi)
         finally:
             self._kv_sink = None
         cache.lens.copy_(torch.tensor([cu[b + 1] - cu[b] for b in range(len(cu) - 1)], dtype=torch.int32))
         return logits
 
     @torch.no_grad()
-    def decode_step(self, input_ids, cache: "KVCache", active=None):
+    def decode_step(self, input_ids, cache: "KVCache", active=None, alibi: bool = False):
         """one new token per sequence: input_ids int64 [B]; appends its keys / values at position cache.lens[b] (sequences
         with active[b] == False are computed but their cache does not advance) -> logits [B, V].  Every op is the training
-        kernel at T = B rows, except attention, which is the single-query cache kernel (csrc/attention_decode.cu)."""
+        kernel at T = B rows, except attention, which is the single-query cache kernel (csrc/attention_decode.cu).
+        `alibi`: ALiBi bias of each cache position (the cache holds the real tokens of a sequence from position 0)."""
         cfg = self.cfg
+        slopes = self._alibi_slopes_for(alibi)
         if self.comm is not None:
             raise NotImplementedError("decoding runs on an unsharded engine (world_size 1)")
         B = input_ids.numel()
@@ -695,7 +731,8 @@ class DolomiteEngine:
             k_new, v_new = self.kv_slices(qkv)
             cache.k[i][rows, pos] = k_new.reshape(B, -1)
             cache.v[i][rows, pos] = v_new.reshape(B, -1)
-            attn = K.attn_decode(qkv, cache.k[i], cache.v[i], lens_incl, self.n_groups, self.q_per_group, self.hd, self.softmax_scale)
+            attn = K.attn_decode(qkv, cache.k[i], cache.v[i], lens_incl, self.n_groups, self.q_per_group, self.hd, self.softmax_scale,
+                                 alibi_slopes=slopes)
             h_mid = K.gemm(attn, u.views[p + "attn.c_proj.weight"], bias=u.views.get(p + "attn.c_proj.bias"), c=h, alpha=m_res,
                            beta=1.0)
             ln2, _ = self._norm_fwd(h_mid, u, p + "ln_2.")
@@ -825,6 +862,7 @@ class DolomiteEngine:
         m_res = 1.0 if cfg.m_residual is None else float(cfg.m_residual)
         head_name = "transformer.wte.weight" if cfg.tie_word_embeddings else "lm_head.weight"
         self._dropout_now = s.get("dropout_seed")  # the masks of the forward being backpropagated
+        self._alibi_now = s.get("alibi")  # and its ALiBi decision (recomputed blocks too)
         self._fp8_now = s.get("fp8", False)  # and its FP8 mode (recomputed blocks too)
         self._fp8_wcache.clear()
         p_res = self._drop_p("resid_pdrop")
@@ -883,7 +921,8 @@ class DolomiteEngine:
             p_att = self._drop_p("attn_pdrop")
             dqkv = K.attn_varlen_bwd(d_attn, qkv, attn, lse, s["cu_seqlens"], s["max_seqlen"], self.n_groups,
                                      self.q_per_group, self.hd, self.softmax_scale, dropout_p=p_att,
-                                     dropout_keys=self._drop_keys(4 * i + 3) if p_att > 0 else (0, 0))
+                                     dropout_keys=self._drop_keys(4 * i + 3) if p_att > 0 else (0, 0),
+                                     alibi_slopes=self._alibi_now)
             del d_attn
             if self.rope_cos is not None:
                 K.rope_qk_inplace(dqkv, self.n_groups, self.q_per_group, self.hd, self.rope_cos, self.rope_sin,

@@ -48,7 +48,9 @@ def last_token_logits(model, input_ids: torch.Tensor, attention_mask: torch.Tens
     cu[1:] = lens.cumsum(0)
     last = (cu[1:] - 1).long()
     ids, pos, cu_p, _, _ = _pad_packed_stream(ids, pos, cu, None)
-    logits = _EngineFunction.apply(model._anchor, model, ids, pos, cu_p, int(max(lens_host)), None, -100, False)
+    # the reference's `generate` always passes an attention mask, so eager and SDPA both add the ALiBi bias
+    logits = _EngineFunction.apply(model._anchor, model, ids, pos, cu_p, int(max(lens_host)), None, -100, False,
+                                   model._alibi_pass(True))
     return logits[last].float()
 
 
@@ -75,7 +77,7 @@ def _prefill(model, input_ids: torch.Tensor, attention_mask: torch.Tensor, max_n
     cache = KVCache(eng, B, max(lens_host) + max_new_tokens + 8)
     # (the packed stream may carry a trailing dummy document that rounds the token count up to 8: it is not cached)
     ids_p, pos_p, cu_p, _, _ = _pad_packed_stream(ids, pos, cu, None)
-    logits = eng.prefill(ids_p, pos_p, cu_p, int(max(lens_host)), cache, n_sequences=B)
+    logits = eng.prefill(ids_p, pos_p, cu_p, int(max(lens_host)), cache, n_sequences=B, alibi=model._alibi_pass(True))
     return logits[last].float(), cache
 
 
@@ -108,7 +110,8 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
         elif cache is None:
             logits, cache = _prefill(model, ids, mask, int(max_new_tokens))
         else:
-            logits = model.engine.decode_step(ids[:, -1].contiguous(), cache, active=~was_finished).float()
+            logits = model.engine.decode_step(ids[:, -1].contiguous(), cache, active=~was_finished,
+                                              alibi=model._alibi_pass(True)).float()
         was_finished = finished.clone()
         if do_sample:
             probs = _filter_logits(logits, temperature, top_k, top_p).softmax(-1)

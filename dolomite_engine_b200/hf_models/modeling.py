@@ -38,14 +38,17 @@ class _EngineFunction(torch.autograd.Function):
     are accumulated by the engine into its flat fp32 gradient buffers (exactly where FSDP would leave them)."""
 
     @staticmethod
-    def forward(ctx, anchor, model, input_ids, position_ids, cu_seqlens, max_seqlen, labels, ignore_index, save=True):
+    def forward(ctx, anchor, model, input_ids, position_ids, cu_seqlens, max_seqlen, labels, ignore_index, save=True,
+                alibi=False):
         # `save`: the caller's torch.is_grad_enabled() (always False in here); under no_grad (evaluation) no activation is kept
+        # `alibi`: the pass adds the ALiBi bias (DolomitePreTrainedModel._alibi_pass)
         engine = model.engine
         # `assume_unit_loss_grad` (set by the training wrappers: train_step calls loss.backward() on the raw loss) lets the
         # engine run the LM head's backward chunk-wise inside the loss computation without ever materialising [T, V]
         logits, loss = engine.forward(input_ids, position_ids, cu_seqlens, max_seqlen, labels=labels,
                                       ignore_index=ignore_index, save_for_backward=bool(save),
-                                      fuse_head_loss=bool(save) and labels is not None and model.assume_unit_loss_grad)
+                                      fuse_head_loss=bool(save) and labels is not None and model.assume_unit_loss_grad,
+                                      alibi=bool(alibi))
         ctx.model = model
         ctx.loss_mode = labels is not None
         return loss.reshape(()) if ctx.loss_mode else logits
@@ -61,7 +64,7 @@ class _EngineFunction(torch.autograd.Function):
             engine.backward(grad_scale_dev=scale)
         else:
             engine.backward(dlogits=grad_out.contiguous())
-        return (None,) * 9
+        return (None,) * 10
 
 
 def _pad_packed_stream(input_ids, position_ids, cu_seqlens, shift_labels, multiple: int = 8):
@@ -121,7 +124,9 @@ class DolomitePreTrainedModel(nn.Module):
                     "Use oracle/ for CPU reference computations in tests."
                 )
             device = torch.device("cuda", torch.cuda.current_device())
-        self.engine = DolomiteEngine(config, device, world_size=world_size, rank=rank, seed=seed, init_on_device=init_on_device)
+        self.engine = DolomiteEngine(config, device, world_size=world_size, rank=rank, seed=seed, init_on_device=init_on_device,
+                                     attention_implementation=self.attention_implementation,
+                                     use_padding_free_transformer=self._use_padding_free_transformer)
         self.flat_params = nn.ParameterList([u.master for u in self.engine.units])
         self._anchor = torch.zeros(1, device=device, requires_grad=True)
         self.assume_unit_loss_grad = False
@@ -196,6 +201,14 @@ class DolomitePreTrainedModel(nn.Module):
             return tuple(v for v in (result.loss, result.logits) if v is not None)
         return result
 
+    def _alibi_pass(self, has_attention_mask: bool) -> bool:
+        """Whether a padded-batch pass adds the ALiBi bias (gpt_dolomite/base.py:559-598 `_get_maybe_causal_mask`): eager
+        attention always adds it through its mask; SDPA only when an attention_mask is passed -- without one it runs
+        `is_causal=True` and the bias is dropped (attention/sdpa.py:56-64), so an sdpa + alibi model runs as NoPE."""
+        if self.engine.alibi_slopes is None:
+            return False
+        return self.attention_implementation == "eager" or has_attention_mask
+
     def _token_multiple(self) -> int:
         """FP8 training forward: the token count is also the row length of the transposed fp8 operands of the weight
         gradients, which the FP8 GEMM wants in multiples of 16.  Evaluation and generation run bf16 and pack as bf16 does."""
@@ -244,7 +257,8 @@ class DolomitePreTrainedModel(nn.Module):
             nxt = torch.where(nxt_valid & mask, nxt, torch.full_like(nxt, -100))
             shift_labels = nxt.reshape(-1)[keep].contiguous()
         ids_p, pos_p, cu, shift_labels, T_real = _pad_packed_stream(ids_p, pos_p, cu, shift_labels, self._token_multiple())
-        out = _EngineFunction.apply(self._anchor, self, ids_p, pos_p, cu, int(max(max_seqlen, 1)), shift_labels, -100, torch.is_grad_enabled())
+        out = _EngineFunction.apply(self._anchor, self, ids_p, pos_p, cu, int(max(max_seqlen, 1)), shift_labels, -100,
+                                    torch.is_grad_enabled(), self._alibi_pass(attention_mask is not None))
         if shift_labels is not None:
             result = CausalLMOutputWithPast(loss=out, logits=None)
         else:
@@ -266,8 +280,9 @@ class DolomitePreTrainedModel(nn.Module):
 
         return generate(self, input_ids, attention_mask, **generate_kwargs)
 
-    def forward_pretraining_loss(self, input_ids, position_ids, cu_seqlens, max_seqlen: int, labels):
-        return _EngineFunction.apply(self._anchor, self, input_ids, position_ids, cu_seqlens, int(max_seqlen), labels, -100, torch.is_grad_enabled())
+    def forward_pretraining_loss(self, input_ids, position_ids, cu_seqlens, max_seqlen: int, labels, alibi: bool = False):
+        return _EngineFunction.apply(self._anchor, self, input_ids, position_ids, cu_seqlens, int(max_seqlen), labels, -100,
+                                     torch.is_grad_enabled(), alibi)
 
     # ------------------------------------------------------------------------------------------
     # state dict / (de)serialisation with the reference's names

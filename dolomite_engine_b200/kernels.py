@@ -523,15 +523,31 @@ def gemm_fp8_wgrad_multi(problems: list[tuple], dy_fmt: int = E5M2, x_fmt: int =
 # ------------------------------------------------------------------------------------------------
 # packed var-len causal attention (attention/padding_free.py:51-62)
 # ------------------------------------------------------------------------------------------------
+def _req_slopes(alibi_slopes, n_heads: int) -> None:
+    _req(alibi_slopes, torch.float32, "alibi_slopes")
+    if alibi_slopes.numel() != n_heads or not alibi_slopes.is_contiguous():
+        raise ValueError(f"alibi_slopes must be a contiguous fp32 [{n_heads}] tensor, got {tuple(alibi_slopes.shape)}")
+
+
 def attn_varlen_fwd(qkv, cu_seqlens, max_seqlen: int, n_groups: int, q_per_group: int, head_dim: int, scale: float, out=None,
-                    dropout_p: float = 0.0, dropout_keys: tuple[int, int] = (0, 0)):
+                    dropout_p: float = 0.0, dropout_keys: tuple[int, int] = (0, 0), alibi_slopes=None):
     """`dropout_p` > 0: attention-probability dropout (training mode; attention/padding_free.py:49-59), masks from
-    `dropout_keys` (kernels.dropout_keys); the backward call must be given the same p and keys"""
+    `dropout_keys` (kernels.dropout_keys); the backward call must be given the same p and keys.
+    `alibi_slopes` (fp32 [n_heads], alibi.alibi_slopes): ALiBi key bias bf16(slope * index of the key in its document);
+    the backward call must be given the same slopes"""
     _req(qkv, _BF16, "qkv"), _req(cu_seqlens, torch.int32, "cu_seqlens")
     T = qkv.shape[0]
     nh = n_groups * q_per_group
     o = torch.empty(T, nh * head_dim, dtype=_BF16, device=qkv.device) if out is None else out
     lse = torch.empty(nh, T, dtype=torch.float32, device=qkv.device)
+    if alibi_slopes is not None:
+        _req_slopes(alibi_slopes, nh)
+        _lib.call(
+            "dolomite_b200_attn_varlen_fwd_alibi", qkv.data_ptr(), qkv.stride(0), o.data_ptr(), lse.data_ptr(),
+            cu_seqlens.data_ptr(), cu_seqlens.numel() - 1, T, int(max_seqlen), n_groups, q_per_group, head_dim, scale,
+            float(dropout_p), dropout_keys[0], dropout_keys[1], alibi_slopes.data_ptr(), _stream(),
+        )
+        return o, lse
     if dropout_p:
         _lib.call(
             "dolomite_b200_attn_varlen_fwd_dropout", qkv.data_ptr(), qkv.stride(0), o.data_ptr(), lse.data_ptr(),
@@ -547,13 +563,22 @@ def attn_varlen_fwd(qkv, cu_seqlens, max_seqlen: int, n_groups: int, q_per_group
 
 
 def attn_varlen_bwd(dout, qkv, out, lse, cu_seqlens, max_seqlen, n_groups, q_per_group, head_dim, scale, dqkv=None,
-                    dropout_p: float = 0.0, dropout_keys: tuple[int, int] = (0, 0)):
+                    dropout_p: float = 0.0, dropout_keys: tuple[int, int] = (0, 0), alibi_slopes=None):
     _req(dout, _BF16, "dout"), _req(qkv, _BF16, "qkv")
     T = qkv.shape[0]
     if dqkv is None:
         dqkv = torch.empty_like(qkv)
     ws_bytes = _lib.load().dolomite_b200_attn_varlen_bwd_workspace_bytes(T, n_groups, q_per_group, head_dim)
     ws = _workspace(ws_bytes, qkv.device)
+    if alibi_slopes is not None:
+        _req_slopes(alibi_slopes, n_groups * q_per_group)
+        _lib.call(
+            "dolomite_b200_attn_varlen_bwd_alibi", dout.data_ptr(), qkv.data_ptr(), qkv.stride(0), out.data_ptr(),
+            lse.data_ptr(), dqkv.data_ptr(), cu_seqlens.data_ptr(), cu_seqlens.numel() - 1, T, int(max_seqlen), n_groups,
+            q_per_group, head_dim, scale, float(dropout_p), dropout_keys[0], dropout_keys[1], alibi_slopes.data_ptr(),
+            ws.data_ptr(), _stream(),
+        )
+        return dqkv
     if dropout_p:
         _lib.call(
             "dolomite_b200_attn_varlen_bwd_dropout", dout.data_ptr(), qkv.data_ptr(), qkv.stride(0), out.data_ptr(),
@@ -569,14 +594,22 @@ def attn_varlen_bwd(dout, qkv, out, lse, cu_seqlens, max_seqlen, n_groups, q_per
     return dqkv
 
 
-def attn_decode(qkv, k_cache, v_cache, lens, n_groups: int, q_per_group: int, head_dim: int, scale: float):
+def attn_decode(qkv, k_cache, v_cache, lens, n_groups: int, q_per_group: int, head_dim: int, scale: float,
+                alibi_slopes=None):
     """one new token per sequence against its KV cache: qkv [B, qkv_dim] (roped), caches [B, L_max, n_groups * head_dim], lens
-    int32 [B] (valid positions including the new token) -> [B, n_heads * head_dim]"""
+    int32 [B] (valid positions including the new token) -> [B, n_heads * head_dim].  `alibi_slopes`: ALiBi bias of each
+    cache position (see attn_varlen_fwd)"""
     _req(qkv, _BF16, "qkv"), _req(k_cache, _BF16, "k_cache"), _req(v_cache, _BF16, "v_cache"), _req(lens, torch.int32, "lens")
     B = qkv.shape[0]
     assert k_cache.shape == v_cache.shape and k_cache.shape[0] == B and k_cache.shape[2] == n_groups * head_dim
     assert k_cache.is_contiguous() and v_cache.is_contiguous() and qkv.stride(1) == 1
     out = torch.empty(B, n_groups * q_per_group * head_dim, dtype=_BF16, device=qkv.device)
+    if alibi_slopes is not None:
+        _req_slopes(alibi_slopes, n_groups * q_per_group)
+        _lib.call("dolomite_b200_attn_decode_alibi", qkv.data_ptr(), qkv.stride(0), k_cache.data_ptr(), v_cache.data_ptr(),
+                  lens.data_ptr(), out.data_ptr(), B, k_cache.shape[1], n_groups, q_per_group, head_dim, scale,
+                  alibi_slopes.data_ptr(), _stream())
+        return out
     _lib.call("dolomite_b200_attn_decode", qkv.data_ptr(), qkv.stride(0), k_cache.data_ptr(), v_cache.data_ptr(), lens.data_ptr(),
               out.data_ptr(), B, k_cache.shape[1], n_groups, q_per_group, head_dim, scale, _stream())
     return out

@@ -143,7 +143,13 @@ class ModelWrapperForPretraining(ModelWrapper):
         self.reset_attention_mask = reset_attention_mask
         self.reset_position_ids = reset_position_ids
         super().__init__(*args, **kwargs)
-        assert self.use_padding_free_transformer, "the B200 pretraining path is the padding-free transformer"
+        if not self.use_padding_free_transformer:
+            # padded pretraining (model_wrapper/pretraining.py:129-194 without cu_seqlens): every row of the batch is one
+            # document of `sequence_length` tokens and no attention mask is passed -- which is the same packed stream as
+            # the padding-free path without reset_attention_mask, so both stage and run it the same way
+            assert not self.reset_attention_mask, (
+                "currently reset_attention_mask is only implemented for padding free transformer")
+            assert not self.reset_position_ids, "currently reset_position_ids is only implemented for padding free transformer"
         if self.reset_position_ids:
             assert self.reset_attention_mask, "reset_attention_mask should be specified with reset_position_ids"
         self.model.assume_unit_loss_grad = True  # train_step calls loss.backward() on the raw loss
@@ -187,7 +193,9 @@ class ModelWrapperForPretraining(ModelWrapper):
         assert tokens.dtype == torch.int64 and tokens.dim() == 2
         assert tokens.shape[0] * (tokens.shape[1] - 1) <= self.micro_batch_size * self.sequence_length
         ids, labels, pos, cu, max_seqlen = self._stage(tokens)
-        return self.model.forward_pretraining_loss(ids, pos, cu, max_seqlen, labels)
+        # padded batches pass no attention mask: eager alibi models add the bias, sdpa ones run as NoPE
+        alibi = not self.use_padding_free_transformer and self.model._alibi_pass(has_attention_mask=False)
+        return self.model.forward_pretraining_loss(ids, pos, cu, max_seqlen, labels, alibi=alibi)
 
 
 class ModelWrapperForFinetuning(ModelWrapper):

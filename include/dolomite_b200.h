@@ -243,6 +243,14 @@ int dolomite_b200_accum_bf16_into_f32(const void* src, float* dst, float scale, 
 int dolomite_b200_attn_decode(const void* qkv, int64_t row_stride, const void* k_cache, const void* v_cache, const int32_t* lens,
                               void* out, int batch, int64_t L_max, int n_groups, int q_per_group, int head_dim,
                               float softmax_scale, void* stream);
+/* The same with ALiBi (eager / SDPA attention of a `position_embedding_type: alibi` model decoding with a mask:
+ * model_wrapper/base.py:110-136 `generate` -> gpt_dolomite/base.py:261-287 `_get_alibi_bias`, :559-598
+ * `_get_maybe_causal_mask`): the score of cache position k of head h gets bias bf16(alibi_slopes[h] * k).
+ *   alibi_slopes  fp32 [n_heads], the reference's slopes (modeling_utils/position_embedding/alibi.py:32-44); null is an
+ *                 error. */
+int dolomite_b200_attn_decode_alibi(const void* qkv, int64_t row_stride, const void* k_cache, const void* v_cache,
+                                    const int32_t* lens, void* out, int batch, int64_t L_max, int n_groups, int q_per_group,
+                                    int head_dim, float softmax_scale, const float* alibi_slopes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * bf16 GEMM on Hopper tensor cores (TMA -> smem -> wgmma -> register accumulators -> epilogue), replacing the cuBLAS
@@ -407,6 +415,24 @@ int dolomite_b200_attn_varlen_bwd_dropout(const void* dout, const void* qkv, int
                                           int max_seqlen, int n_groups, int q_per_group, int head_dim,
                                           float softmax_scale, float dropout_p, uint32_t key0, uint32_t key1,
                                           void* workspace, void* stream);
+/* The same with ALiBi (position_embedding_type: alibi with eager or SDPA attention on padded batches; the reference's
+ * call sites: gpt_dolomite/base.py:261-287 `_get_alibi_bias` -> modeling_utils/position_embedding/alibi.py:14-30, added to
+ * the logits through the mask of `_get_maybe_causal_mask`, base.py:559-598, in attention/base.py:233-245 (eager
+ * baddbmm) and attention/sdpa.py:56-64 (attn_mask of scaled_dot_product_attention)).  The logit of (query, key k) of
+ * head h is softmax_scale * <q, k> + bf16(alibi_slopes[h] * kpos(k)), kpos = the key's index inside its document; the
+ * softmax scale does not multiply the bias.  The logits stay fp32 (as in SDPA's fused kernels; eager rounds them to
+ * bf16).  lse is the natural log-sum-exp of the biased logits; the backward must be given the slopes of its forward.
+ *   alibi_slopes  fp32 [n_heads], the reference's slopes (alibi.py:32-44); null is an error.
+ * dropout_p / key0 / key1 as in the *_dropout functions (dropout_p == 0: none). */
+int dolomite_b200_attn_varlen_fwd_alibi(const void* qkv, int64_t row_stride, void* out, float* lse,
+                                        const int32_t* cu_seqlens, int n_docs, int64_t T, int max_seqlen, int n_groups,
+                                        int q_per_group, int head_dim, float softmax_scale, float dropout_p, uint32_t key0,
+                                        uint32_t key1, const float* alibi_slopes, void* stream);
+int dolomite_b200_attn_varlen_bwd_alibi(const void* dout, const void* qkv, int64_t row_stride, const void* out,
+                                        const float* lse, void* dqkv, const int32_t* cu_seqlens, int n_docs, int64_t T,
+                                        int max_seqlen, int n_groups, int q_per_group, int head_dim, float softmax_scale,
+                                        float dropout_p, uint32_t key0, uint32_t key1, const float* alibi_slopes,
+                                        void* workspace, void* stream);
 
 #ifdef __cplusplus
 }
