@@ -836,7 +836,9 @@ __device__ __forceinline__ void st_cluster_f32(float* local_smem, uint32_t rank,
     asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(remote), "f"(v) : "memory");
 }
 
-template <int NV, int SPLIT>
+// TAIL: V % 8 != 0.  The row's last vector (index V8 - 1) then holds only V - 8 (V8 - 1) logits; its other lanes are
+// left out of the max and the sum and get a zero gradient.  Without TAIL the kernel is the plain full-vector one.
+template <int NV, int SPLIT, bool TAIL>
 __global__ void __launch_bounds__(kCeThreads, 2)
     ce_rows_kernel(const uint4* logits, int64_t ld8, const int64_t* __restrict__ labels, uint4* dlogits,
                    float* __restrict__ loss_tok, const float* __restrict__ scratch, int64_t T, int64_t V,
@@ -844,7 +846,9 @@ __global__ void __launch_bounds__(kCeThreads, 2)
     __shared__ float red[kCeThreads / 32];
     __shared__ float xch[2][4];  // [max | sum][cluster rank]: written by every CTA of the cluster (DSMEM)
     const int crank = SPLIT > 1 ? int(cluster_ctarank()) : 0;
-    const int64_t V8 = V >> 3;
+    const int64_t V8 = (V + 7) >> 3;
+    const int64_t vlast = V8 - 1;
+    const int tail = int(V - 8 * vlast);  // valid lanes of the last vector, 1 .. 8
     const int64_t per = (V8 + SPLIT - 1) / SPLIT;
     const int64_t v_lo = crank * per, v_hi = min(V8, v_lo + per);
     const float n_valid = scratch[0];
@@ -876,11 +880,13 @@ __global__ void __launch_bounds__(kCeThreads, 2)
         float m = -INFINITY;
 #pragma unroll
         for (int k = 0; k < NV; ++k) {
-            if (v_lo + k * kCeThreads + threadIdx.x < v_hi) {
+            const int64_t i = v_lo + k * kCeThreads + threadIdx.x;
+            if (i < v_hi) {
                 float f[8];
                 unpack8(v[k], f);
+                const int nl = TAIL && i == vlast ? tail : 8;
 #pragma unroll
-                for (int j = 0; j < 8; ++j) m = fmaxf(m, f[j] * scale2);
+                for (int j = 0; j < 8; ++j) m = fmaxf(m, !TAIL || j < nl ? f[j] * scale2 : -INFINITY);
             }
         }
         m = ce_block_reduce(m, red, true);
@@ -893,11 +899,14 @@ __global__ void __launch_bounds__(kCeThreads, 2)
         float s = 0.f;
 #pragma unroll
         for (int k = 0; k < NV; ++k) {
-            if (v_lo + k * kCeThreads + threadIdx.x < v_hi) {
+            const int64_t i = v_lo + k * kCeThreads + threadIdx.x;
+            if (i < v_hi) {
                 float f[8];
                 unpack8(v[k], f);
+                const int nl = TAIL && i == vlast ? tail : 8;
 #pragma unroll
-                for (int j = 0; j < 8; ++j) s += fast_exp2(fmaf(f[j], scale2, -m));
+                for (int j = 0; j < 8; ++j)
+                    if (!TAIL || j < nl) s += fast_exp2(fmaf(f[j], scale2, -m));
             }
         }
         s = ce_block_reduce(s, red, false);
@@ -927,10 +936,12 @@ __global__ void __launch_bounds__(kCeThreads, 2)
                     for (int j = 0; j < 8; ++j) xl = (j == lsub) ? f[j] : xl;
                     loss_tok[row] = (lse2 - xl * scale2) * 0.6931471805599453f;
                 }
+                const int nl = TAIL && i == vlast ? tail : 8;
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
                     const float pj = fast_exp2(fmaf(f[j], scale2, -lse2));
                     f[j] = ((has_label && j == lsub) ? pj - 1.f : pj) * gmul;
+                    if (TAIL && j >= nl) f[j] = 0.f;
                 }
                 dr[i] = pack8(f);
             }
@@ -940,11 +951,11 @@ __global__ void __launch_bounds__(kCeThreads, 2)
     }
 }
 
-template <int NV, int SPLIT>
+template <int NV, int SPLIT, bool TAIL>
 int launch_ce_rows(const void* logits, int64_t ldl, const int64_t* labels, void* dlogits, float* loss_tok,
                    const float* scratch, int64_t T, int64_t V, int64_t ignore_index, float logit_scale, float grad_scale,
                    cudaStream_t st) {
-    auto kern = ce_rows_kernel<NV, SPLIT>;
+    auto kern = ce_rows_kernel<NV, SPLIT, TAIL>;
     int64_t clusters = 2 * int64_t(dolo_num_sms()) / SPLIT;  // two 256-thread CTAs per SM (a row lives in a CTA's registers)
     if (clusters > T) clusters = T;
     cudaLaunchConfig_t cfg = {};
@@ -1503,21 +1514,27 @@ extern "C" int dolomite_b200_cross_entropy_count(const int64_t* labels, int64_t 
 extern "C" int dolomite_b200_cross_entropy_rows(const void* logits, int64_t ldl, const int64_t* labels, void* dlogits,
                                                 float* loss_per_token, const float* scratch, int64_t T, int64_t V,
                                                 int64_t ignore_index, float logit_scale, float grad_scale, void* stream) {
-    DOLO_REQUIRE(V > 0 && V % 8 == 0 && ldl % 8 == 0 && ldl >= V,
-                 "cross_entropy: V=%lld / ld=%lld must be multiples of 8", (long long)V, (long long)ldl);
+    DOLO_REQUIRE(V > 0 && ldl % 8 == 0 && ldl >= V,
+                 "cross_entropy: V=%lld must be >= 1 and ld=%lld a multiple of 8 and >= V", (long long)V, (long long)ldl);
     DOLO_REQUIRE(aligned16(logits) && aligned16(dlogits), "cross_entropy: pointers must be 16-byte aligned");
     if (T == 0) return DOLO_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     // vectors per thread with 256 threads and the whole row in ONE CTA; wider rows are split over a 2- or 4-CTA cluster
-    const int64_t V8 = V / 8;
+    const int64_t V8 = (V + 7) / 8;
     const int64_t nv1 = (V8 + kCeThreads - 1) / kCeThreads;
-#define DOLO_CE(NV, SPLIT)                                                                                          \
-    return launch_ce_rows<NV, SPLIT>(logits, ldl, labels, dlogits, loss_per_token, scratch, T, V, ignore_index, \
-                                     logit_scale, grad_scale, st)
+#define DOLO_CE(NV, SPLIT)                                                                                             \
+    return V % 8 ? launch_ce_rows<NV, SPLIT, true>(logits, ldl, labels, dlogits, loss_per_token, scratch, T, V,      \
+                                                   ignore_index, logit_scale, grad_scale, st)                         \
+                 : launch_ce_rows<NV, SPLIT, false>(logits, ldl, labels, dlogits, loss_per_token, scratch, T, V,     \
+                                                    ignore_index, logit_scale, grad_scale, st)
     if (nv1 <= 4) DOLO_CE(4, 1);
     if (nv1 <= 8) DOLO_CE(8, 1);
     if (nv1 <= 16) DOLO_CE(16, 1);
-    if (nv1 <= 24) DOLO_CE(24, 1);  // one CTA per row whenever it fits: the cluster barrier costs a GPU-scope fence per use
+    // one CTA per row whenever it fits: the cluster barrier costs a GPU-scope fence per use.  The masked last vector of an
+    // odd width pushes the 24-vector instance to 632 bytes of spill loads per thread, so such rows take the 2-CTA cluster.
+    if (nv1 <= 24 && V % 8 == 0)
+        return launch_ce_rows<24, 1, false>(logits, ldl, labels, dlogits, loss_per_token, scratch, T, V, ignore_index,
+                                            logit_scale, grad_scale, st);
     if (nv1 <= 32) DOLO_CE(16, 2);
     if (nv1 <= 48) DOLO_CE(12, 4);
     if (nv1 <= 64) DOLO_CE(16, 4);

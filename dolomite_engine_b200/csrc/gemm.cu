@@ -476,10 +476,15 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         }
         const bool has_bias = pr.bias != nullptr;
         const bool has_c = pr.C != nullptr;
-        // the tile's bias slice: loaded now, kept in shared memory for the epilogue
+        // the tile's bias slice: loaded now, kept in shared memory for the epilogue.  An odd N ends in a half pair, whose
+        // upper element (column N) is not read; its value only ever reaches the clipped column N of the slab.
         uint32_t bias_v = 0;
-        if (has_bias && wt < TN / 2 && col0 + 2 * wt < pr.N)
-            bias_v = __ldg(reinterpret_cast<const uint32_t*>(pr.bias + col0 + 2 * wt));
+        if (has_bias && wt < TN / 2 && col0 + 2 * wt < pr.N) {
+            if (col0 + 2 * wt + 1 < pr.N)
+                bias_v = __ldg(reinterpret_cast<const uint32_t*>(pr.bias + col0 + 2 * wt));
+            else
+                bias_v = __bfloat16_as_ushort(pr.bias[col0 + 2 * wt]);
+        }
         int prev_stage = -1;
         for (int kb = ti.kb0; kb < ti.kb1; ++kb) {
             mbar_wait(&full_bar[stage], phase, 3);
@@ -785,12 +790,22 @@ struct GemmProblemArgs {
 static int setup_problem(GemmMaps& maps, GemmParams& p, int q, const GemmProblemArgs& g, int a_mn_major, int b_mn_major,
                          int d_is_f32, const GroupArgs& ga, int tile_n) {
     const int64_t M = g.M, N = g.N, K = g.K;
+    // M, N and K may take any value: the tensor maps carry the exact extents, so TMA zero-fills the operand tails of the
+    // last k-block and tile and clips the D rows and columns.  Only the row strides and the base addresses (checked when
+    // the tensor maps are made) need 16-byte alignment.  A TMA store writes whole 16-byte segments: when a row of D ends
+    // inside one (N not a multiple of 16 bytes), the rest of that segment, columns [N, round_up(N, 16 bytes)), receives
+    // zeros, so ldd must cover it.
     DOLO_REQUIRE(K > 0, "gemm: K must be > 0");
-    DOLO_REQUIRE(K % 8 == 0 && N % 8 == 0, "gemm: K=%lld and N=%lld must be multiples of 8", (long long)K, (long long)N);
     DOLO_REQUIRE(g.lda % 8 == 0 && g.ldb % 8 == 0 && g.ldd % (d_is_f32 ? 4 : 8) == 0,
                  "gemm: leading dimensions must keep 16-byte alignment");
-    DOLO_REQUIRE(!a_mn_major || M % 8 == 0, "gemm: MN-major A requires M %% 8 == 0");
+    {
+        const int64_t per = d_is_f32 ? 4 : 8;
+        DOLO_REQUIRE(g.ldd >= (N + per - 1) / per * per,
+                     "gemm: ldd=%lld must cover N=%lld rounded up to 16 bytes (the TMA store writes that segment)",
+                     (long long)g.ldd, (long long)N);
+    }
     DOLO_REQUIRE(g.C == nullptr || g.ldc % (d_is_f32 ? 4 : 8) == 0, "gemm: ldc alignment");
+    DOLO_REQUIRE((reinterpret_cast<uintptr_t>(g.bias) & 3) == 0, "gemm: bias must be 4-byte aligned");
     DOLO_REQUIRE(M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31), "gemm: dimension too large");
     // K-major: dims {K, rows}, box {64, tile rows} (128 for A, tile_n for B).  MN-major: dims {rows, K}, box {64, 64}.
     uint64_t dims[2], strides[2];
@@ -800,6 +815,8 @@ static int setup_problem(GemmMaps& maps, GemmParams& p, int q, const GemmProblem
         // gather-on-load: the producer warp reads A's rows itself (no tensor map)
         DOLO_REQUIRE(!a_mn_major, "gemm: gather-on-load needs a K-major A");
         DOLO_REQUIRE((reinterpret_cast<uintptr_t>(g.A) & 15) == 0, "gemm: gather-on-load needs a 16-byte aligned A");
+        // the producer warp copies whole 16-byte vectors of a row: a K tail inside a vector would be read as data
+        DOLO_REQUIRE(K % 8 == 0, "gemm: gather-on-load needs K %% 8 == 0 (K=%lld)", (long long)K);
         p.gather_a = g.A;
         p.gather_lda = g.lda;
         p.gather_k = int(K);

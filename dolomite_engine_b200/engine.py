@@ -233,8 +233,9 @@ def check_supported(cfg: CommonConfig, *, attention_implementation: str = "flash
             raise NotImplementedError("MoE experts with bias are not supported (ScatterMoE asserts the same, moe/scatter.py:22)")
         if cfg.n_inner % 64 or cfg.n_embd % 64:
             raise NotImplementedError("MoE: n_embd and n_inner must be multiples of 64 (grouped GEMM K tiles)")
-    if cfg.n_embd % 8 or cfg.n_inner % 8 or cfg.vocab_size % 8:
-        raise NotImplementedError("n_embd, n_inner and vocab_size must be multiples of 8 (16-byte vector kernels / TMA)")
+    # vocab_size may be any value: [T, V] logits live in buffers with 16-byte row strides (kernels.rows_empty)
+    if cfg.n_embd % 8 or cfg.n_inner % 8:
+        raise NotImplementedError("n_embd and n_inner must be multiples of 8 (16-byte vector kernels / TMA)")
 
 
 class DolomiteEngine:
@@ -626,7 +627,7 @@ class DolomiteEngine:
             d_hf = torch.empty_like(hf)
             # FP8 head: the chunk rows are the contraction of its weight-gradient GEMM, a multiple of 16
             rows = self._head_chunk_rows(T, head.shape[0], self.head_chunk_bytes, 16 if self._is_fp8(head_name) else 8)
-            buf = torch.empty(min(rows, T), head.shape[0], dtype=torch.bfloat16, device=hf.device)
+            buf = K.rows_empty(min(rows, T), head.shape[0], device=hf.device)
             self._fp8_keep = {head_name}
             for r0 in range(0, T, rows):
                 r1 = min(T, r0 + rows)
@@ -643,7 +644,7 @@ class DolomiteEngine:
                 # fused CE fwd+bwd: dlogits overwrites the logits
                 loss, _, dlogits = K.cross_entropy_fwd_bwd(logits, labels, ignore_index=ignore_index, dlogits=None)
             else:
-                logits_out = logits
+                logits_out = logits.contiguous()  # [T, V] as the reference returns it: a copy when V % 8 != 0
         if save_for_backward:
             self._saved = dict(input_ids=input_ids, position_ids=position_ids, cu_seqlens=cu_seqlens, max_seqlen=max_seqlen,
                                layers=saved_layers, h_last=h, rstd_f=rstd_f, hf=hf, dlogits=dlogits, d_hf=d_hf, T=T,
@@ -749,7 +750,7 @@ class DolomiteEngine:
         head = root.views["transformer.wte.weight"] if cfg.tie_word_embeddings else root.views["lm_head.weight"]
         logits = K.gemm(hf, head, alpha=1.0 if cfg.m_width is None else 1.0 / float(cfg.m_width))
         cache.lens.add_(1 if active is None else active.to(torch.int32))
-        return logits
+        return logits.contiguous()
 
     # ------------------------------------------------------------------------------------------
     # backward
@@ -874,7 +875,8 @@ class DolomiteEngine:
                 raise RuntimeError("forward(fuse_head_loss=True) assumed d(loss) = 1; an upstream gradient cannot be applied")
             d_hf = s["d_hf"]
         else:
-            dl = dlogits if dlogits is not None else s["dlogits"]
+            # a caller's [T, V] gradient is staged into 16-byte rows when V % 8 != 0 (the dgrad / wgrad operand)
+            dl = K.rows_aligned(dlogits) if dlogits is not None else s["dlogits"]
             if dl is None:
                 raise RuntimeError("no loss gradient available: forward was run without labels and no dlogits was given")
             if grad_scale_dev is not None:

@@ -42,6 +42,31 @@ def _req(t: torch.Tensor, dtype, name: str) -> None:
 
 
 # ------------------------------------------------------------------------------------------------
+# Row layout of [rows, cols] outputs.  TMA and the 16-byte vector kernels need 16-byte row strides, so a width that is
+# not a multiple of 16 bytes (the logits of an odd vocabulary) is allocated [rows, round_up(cols, 16 B)] and used as a
+# [rows, cols] view of that buffer.  The extra columns are never part of a result (the GEMM's TMA stores and the
+# cross-entropy kernel may write zeros there).  Widths that are already multiples give a plain contiguous tensor.
+# ------------------------------------------------------------------------------------------------
+def rows_empty(rows: int, cols: int, dtype=_BF16, device=None) -> torch.Tensor:
+    """uninitialised [rows, cols] tensor whose row stride is a multiple of 16 bytes"""
+    per = 16 // torch.empty((), dtype=dtype).element_size()
+    ld = -(-cols // per) * per
+    if ld == cols:
+        return torch.empty(rows, cols, dtype=dtype, device=device)
+    return torch.empty(rows, ld, dtype=dtype, device=device)[:, :cols]
+
+
+def rows_aligned(t: torch.Tensor) -> torch.Tensor:
+    """`t` ([rows, cols], unit column stride) if its row stride keeps 16 bytes, else a copy into rows_empty"""
+    per = 16 // t.element_size()
+    if t.stride(1) == 1 and t.stride(0) % per == 0 and t.data_ptr() % 16 == 0:
+        return t
+    out = rows_empty(t.shape[0], t.shape[1], t.dtype, t.device)
+    out.copy_(t)
+    return out
+
+
+# ------------------------------------------------------------------------------------------------
 # RMSNorm (normalization/rmsnorm/base.py:18-25)
 # ------------------------------------------------------------------------------------------------
 def rmsnorm_fwd(x: torch.Tensor, w: torch.Tensor, eps: float, out: torch.Tensor | None = None):
@@ -250,8 +275,15 @@ def colsum_accum(x, out, scale: float = 1.0):
 
 
 def scale_by_device_scalar(x, scale):
+    """x *= scale in place; x contiguous, or [rows, cols] rows of a rows_empty buffer (whole rows of the buffer are
+    scaled, its spare columns included)"""
     _req(x, _BF16, "x"), _req(scale, torch.float32, "scale")
-    _lib.call("dolomite_b200_scale_bf16_by_device_scalar", x.data_ptr(), x.numel(), scale.data_ptr(), _stream())
+    n = x.numel()
+    if not x.is_contiguous():
+        assert x.dim() == 2 and x.stride(1) == 1 and x.stride(0) >= x.shape[1]
+        n = x.shape[0] * x.stride(0)
+        assert x.storage_offset() + n <= x.untyped_storage().nbytes() // x.element_size()
+    _lib.call("dolomite_b200_scale_bf16_by_device_scalar", x.data_ptr(), n, scale.data_ptr(), _stream())
 
 
 def add_scaled(a, b, alpha: float, out=None):
@@ -360,7 +392,7 @@ def gemm(a, b, *, a_mn=False, b_mn=False, out=None, out_dtype=_BF16, c=None, alp
     if K != Kb:
         raise _lib.DolomiteB200Error(f"gemm: contraction mismatch {K} vs {Kb}")
     if out is None:
-        out = torch.empty(M, N, dtype=out_dtype, device=a.device)
+        out = rows_empty(M, N, out_dtype, a.device)
     d_is_f32 = int(out.dtype == torch.float32)
     assert out.stride(1) == 1 and out.shape == (M, N)
     if c is not None:

@@ -166,7 +166,9 @@ int dolomite_b200_embedding_bwd(const int64_t* ids, const void* dout, float* dwt
 /* ------------------------------------------------------------------------------------------------
  * Cross entropy (mean over non-ignored tokens), fused forward + backward --
  *   model_wrapper/pretraining.py:124-125 (F.cross_entropy on [T,V]) and gpt_dolomite/main.py:185-200.
- *   logits bf16 [T, ldl]; labels int64 [T]; label == ignore_index contributes nothing.
+ *   logits bf16 [T, ldl]; labels int64 [T]; label == ignore_index contributes nothing.  Any V in [1, 131072] with
+ *   ldl % 8 == 0 and ldl >= V: columns [V, ldl) are never read as data (they may hold anything, NaN included) and
+ *   receive 0 in dlogits where the last 16-byte vector of a row straddles V.
  *   Writes per-token loss (fp32, 0 for ignored), the scalar mean loss, and overwrites dlogits (may alias
  *   logits) with (softmax - onehot) * grad_scale / n_valid in bf16.
  *   scratch: 2 floats.  logit_scale multiplies logits before the softmax (1/m_width, gpt_dolomite/main.py:155-156).
@@ -262,7 +264,12 @@ int dolomite_b200_attn_decode_alibi(const void* qkv, int64_t row_stride, const v
  *   A is logical [M,K]: a_mn_major == 0 -> stored row-major [M,K] (ld = lda);  1 -> stored [K,M] (ld = lda).
  *   B is logical [N,K]: b_mn_major == 0 -> stored row-major [N,K] (ld = ldb);  1 -> stored [K,N] (ld = ldb).
  *   D/C: row-major [M,N]; d_is_f32 selects fp32 (else bf16) for BOTH D and C.  C may be NULL (beta ignored)
- *   or alias D.  bias: bf16 [N] or NULL.   K % 8 == 0, lds % 8 == 0, 16-byte aligned bases.
+ *   or alias D.  bias: bf16 [N] (4-byte aligned) or NULL.   M, N, K >= 1 of any value (an LM head of any vocabulary:
+ *   N = V forward, K = V dgrad, M = V wgrad); the row strides keep 16 bytes (lda, ldb, ldd, ldc % 8 == 0 for bf16,
+ *   ldd, ldc % 4 == 0 for fp32) and the bases are 16-byte aligned.  TMA zero-fills operand tails and clips D / C
+ *   tails: columns of a row beyond N (or K) are never read as data.  TMA stores write whole 16-byte segments, so when
+ *   N is not a multiple of 16 bytes the columns [N, round_up(N, 16 bytes)) of D receive zeros (ldd must cover them);
+ *   nothing beyond that segment is written.
  *   flags: bit0 = the caller promises bf16 D and no C (checked).  With or without it, every launch stages its output
  *   tiles in shared memory and writes them with TMA stores (reduce-adds for split-K), so D and C need 16-byte aligned
  *   bases and row strides.
