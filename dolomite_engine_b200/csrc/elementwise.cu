@@ -303,8 +303,10 @@ __global__ void __launch_bounds__(MAX_THREADS)
             __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(&ob);
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
-                const __nv_bfloat162 s1s = sin_sign < 0.f ? __hneg2(s1[j]) : s1[j];  // backward: the inverse rotation
-                const __nv_bfloat162 s2s = sin_sign < 0.f ? __hneg2(s2[j]) : s2[j];
+                // backward: the transpose rotation dx1 = dy1*c1 + dy2*s2, dx2 = dy2*c2 - dy1*s1 (the halves of the sin
+                // row trade places; the same thing for the reference's tables, whose halves are equal)
+                const __nv_bfloat162 s1s = sin_sign < 0.f ? __hneg2(s2[j]) : s1[j];
+                const __nv_bfloat162 s2s = sin_sign < 0.f ? __hneg2(s1[j]) : s2[j];
                 o1[j] = __hadd2_rn(__hmul2_rn(x1[j], c1[j]), __hmul2_rn(__hneg2(x2[j]), s1s));  // _rn: never contracted into an fma
                 o2[j] = __hadd2_rn(__hmul2_rn(x2[j], c2[j]), __hmul2_rn(x1[j], s2s));
             }
@@ -1074,7 +1076,12 @@ __global__ void clip_coef_kernel(const float* sumsq, float max_norm, float* coef
     const float norm = sqrtf(sumsq[0]);
     if (norm_out) norm_out[0] = norm;
     float c = 1.f;
-    if (max_norm > 0.f) c = fminf(1.f, max_norm / (norm + 1e-6f));
+    if (max_norm > 0.f) {
+        // torch.clamp(max_norm / (norm + 1e-6), max=1): a NaN norm gives a NaN coefficient (fminf would give 1), so a NaN
+        // gradient poisons every parameter as it does in the reference instead of updating the finite ones unclipped
+        const float r = max_norm / (norm + 1e-6f);
+        c = r >= 1.f ? 1.f : r;
+    }
     coef[0] = c;
 }
 
@@ -1494,7 +1501,7 @@ extern "C" int dolomite_b200_embedding_fwd(const int64_t* ids, const void* wte, 
 extern "C" int dolomite_b200_embedding_bwd(const int64_t* ids, const void* dout, float* dwte, int64_t T, int H,
                                            int64_t V, float scale, void* stream) {
     DOLO_REQUIRE(H > 0 && H % 8 == 0, "embedding_bwd: H=%d must be a multiple of 8", H);
-    DOLO_REQUIRE(aligned16(dout), "embedding_bwd: pointers must be 16-byte aligned");
+    DOLO_REQUIRE(aligned16(dout) && aligned16(dwte), "embedding_bwd: pointers must be 16-byte aligned");  // dwte: float4
     if (T == 0) return DOLO_OK;
     DOLO_REQUIRE(T < (int64_t(1) << 36), "embedding_bwd: T too large");
     const unsigned grid = unsigned((T + kThreads / 32 - 1) / (kThreads / 32));  // one warp per token

@@ -34,7 +34,20 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
     return v;
 }
 
-// one warp per token.  logits bf16 [T, E]; selects k experts by repeated arg-max (ties -> lowest index)
+// Rank of a logit in torch.topk's order as an unsigned key: NaN above everything, then the float order (-inf included,
+// -0 equal to +0).  Every logit has a key >= 0x007fffff (that of -inf), so key 0 marks experts that are not candidates
+// (chosen already, or lanes past E).
+__device__ __forceinline__ uint32_t topk_key(float x) {
+    if (x != x) return 0xffffffffu;
+    const uint32_t u = __float_as_uint(x + 0.f);  // -0 -> +0
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float topk_value(uint32_t key) {
+    return __uint_as_float((key & 0x80000000u) ? (key & 0x7fffffffu) : ~key);
+}
+
+// one warp per token.  logits bf16 [T, E]; selects k experts by repeated arg-max of topk_key (ties -> lowest index):
+// every logit, -inf and NaN included, can be chosen, so the k chosen experts are distinct and in [0, E) (k <= E).
 __global__ void moe_route_kernel(const __nv_bfloat16* __restrict__ logits, int64_t T, int E, int k,
                                  int32_t* __restrict__ sel_idx, float* __restrict__ sel_w,
                                  int32_t* __restrict__ counts) {
@@ -42,16 +55,16 @@ __global__ void moe_route_kernel(const __nv_bfloat16* __restrict__ logits, int64
     const int lane = threadIdx.x & 31;
     if (t >= T) return;
     constexpr int MAXE = 8;  // experts per lane -> E <= 256
-    float v[MAXE];
+    uint32_t v[MAXE];
 #pragma unroll
     for (int i = 0; i < MAXE; ++i) {
         const int e = lane + i * 32;
-        v[i] = e < E ? __bfloat162float(logits[t * E + e]) : -INFINITY;
+        v[i] = e < E ? topk_key(__bfloat162float(logits[t * E + e])) : 0u;
     }
     float chosen_v[8];
     int chosen_e[8];
     for (int j = 0; j < k; ++j) {
-        float best = -INFINITY;
+        uint32_t best = 0u;
         int be = 0x7fffffff;
 #pragma unroll
         for (int i = 0; i < MAXE; ++i) {
@@ -60,15 +73,15 @@ __global__ void moe_route_kernel(const __nv_bfloat16* __restrict__ logits, int64
         }
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) {
-            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+            const uint32_t ob = __shfl_xor_sync(0xffffffffu, best, o);
             const int oe = __shfl_xor_sync(0xffffffffu, be, o);
             if (ob > best || (ob == best && oe < be)) { best = ob; be = oe; }
         }
-        chosen_v[j] = best;
+        chosen_v[j] = topk_value(best);
         chosen_e[j] = be;
 #pragma unroll
         for (int i = 0; i < MAXE; ++i)
-            if (lane + i * 32 == be) v[i] = -INFINITY;
+            if (lane + i * 32 == be) v[i] = 0u;
     }
     if (lane == 0) {
         float m = chosen_v[0];

@@ -219,7 +219,8 @@ int dolomite_b200_dropout_bwd(const void* dy, void* dx, int64_t n, float p, floa
 /* ------------------------------------------------------------------------------------------------
  * Optimizer-side flat-shard kernels (train_utils.py:99-106: clip_grad_norm_ + AdamW step).
  *   sumsq: out[0] += sum(g^2)  (fp32 grads), summed in a fixed order (bit-identical from run to run); workspace:
- *   dolomite_b200_sumsq_workspace_bytes() bytes, 4-byte aligned.   clip coef: coef = min(1, max_norm / (sqrt(sumsq) + 1e-6)).
+ *   dolomite_b200_sumsq_workspace_bytes() bytes, 4-byte aligned.   clip coef: coef = min(1, max_norm / (sqrt(sumsq) + 1e-6)),
+ *   NaN for a NaN norm (torch.clamp); 1 when max_norm <= 0.
  *   adamw: torch.optim.AdamW semantics on fp32 master shard; also emits the bf16 copy that the next
  *   all-gather ships.  `clip_coef` is a device pointer (nullable -> 1).  step >= 1.
  * ------------------------------------------------------------------------------------------------ */
