@@ -59,26 +59,95 @@ __global__ void __launch_bounds__(256)
     }
 }
 
-// One CTA = one 128-row key/value tile of one kv-head group of one document, two warpgroups of 64 key rows each; it loops
-// over the query heads of the group and the 64-row query tiles that see the key tile (causal) and keeps dK_j, dV_j
-// accumulating in registers.  Everything is computed in the "transposed" frame (accumulator row == key row) so that P^T and
-// dS^T feed the tensor core straight from registers as the A operand.  Per step, every warpgroup runs
+// Both kernels below are warp-specialised (384 threads): warpgroup 0 is the producer and keeps only ATT_PRODUCER_REGS
+// registers per thread; warpgroups 1 and 2 are the consumers, each owning 64 rows of the CTA's 128-row tile.  One elected
+// producer thread is the only one that waits on `empty` barriers and issues the TMA loads of the ring, so no consumer ever
+// waits for the other: the two consumer warpgroups drift apart and one's elementwise phase overlaps the other's MMAs.
+constexpr int ATT_BWD_THREADS = 384;
+constexpr int ATT_PRODUCER_REGS = 24;
+constexpr int ATT_CONSUMER_REGS = 240;
+static_assert(ATT_PRODUCER_REGS * 128 + 2 * ATT_CONSUMER_REGS * 128 <= 65536, "register file exceeded");
+
+// One CTA = one 128-row key/value tile of one kv-head group of one document; it loops over the query heads of the group and
+// the 64-row query tiles that see the key tile (causal) and keeps dK_j, dV_j accumulating in registers.  Everything is
+// computed in the "transposed" frame (accumulator row == key row) so that P^T and dS^T feed the tensor core straight from
+// registers as the A operand.  Per step, every consumer warpgroup (64 key rows) runs
 //     S^T  = K_j Q_i^T            (SS)           dP^T = V_j dO_i^T             (SS)
 //     P^T  = exp2(S^T*scale - LSE_i) ,  dS^T = scale * P^T o (dP^T - Delta_i)     (registers)
 //     dV_j += P^T dO_i            (RS, B = dO MN-major)
 //     dK_j += dS^T Q_i            (RS, B = Q  MN-major)
-// Thread 0 also issues the TMA loads (K_j, V_j once; Q_i, dO_i through a 2-stage ring).
+// Producer: thread 0 loads K_j, V_j once; an elected lane of warp 0 streams Q_i, dO_i through a QDO_STAGES-deep ring and
+// warp 1 stages the 64 LSE_i (times log2 e) and Delta_i values of each step into the same ring stage with plain loads (the
+// rows of a document start anywhere, so they are not bulk-copy aligned); both arrive on the stage's `full` barrier.
+// Only the steps whose query tile reaches a key row of the warpgroup (qi <= i0 + cw) or crosses the document end test the
+// causal / bounds predicate; the interior steps run the bare formula.  The MMAs of a step run in the serial order SS ->
+// elementwise -> RS: issuing the next step's SS group behind the RS group makes ptxas serialise every wgmma of the kernel.
 // ALIBI: P^T = exp2(log2(e) * (S^T*scale + bias_k) - LSE_i), the bias of the forward (one per key row of the thread); the
 // bias has no gradient, so dS^T is unchanged.
 // dQ has its own kernel (attn_dq_kernel below: one CTA per query tile walks the key tiles in order), so that every
 // gradient is summed in a fixed order and the backward is bit-identical from run to run -- adding the dQ contributions
 // of the key-tile CTAs with atomics would not be.
-constexpr int BWD_THREADS = 256;
 constexpr int BWD_QT = 64;  // query rows per step
-constexpr int QDO_STAGES = 2;
+
+// Hides a shared-memory base address from the compiler's loop-invariant code motion, so that the wgmma descriptors built
+// from it are recomputed next to each MMA instead of being hoisted out of the step loop and held in registers.
+__device__ __forceinline__ void opaque(uint32_t& x) { asm volatile("" : "+r"(x)); }
+// Wait without the watchdog of mbar_wait, for waits with an MMA group in flight: ptxas serialises every wgmma of a kernel
+// that has a trap path (or any other divergent branch) while a group is in flight.
+__device__ __forceinline__ void mbar_spin(uint64_t* bar, uint32_t parity) {
+    asm volatile("{\n\t.reg .pred P1;\n\tWAIT_%=:\n\tmbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t@!P1 bra WAIT_%=;\n\t}"
+                 ::"r"(smem_u32(bar)), "r"(parity)
+                 : "memory");
+}
+// Arrive of lane 0 only, as a predicated instruction rather than a branch, for the same reason.
+__device__ __forceinline__ void mbar_arrive_lane0(uint64_t* bar, int lane) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.eq.s32 p, %1, 0;\n\t@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}" ::"r"(smem_u32(bar)),
+                 "r"(lane)
+                 : "memory");
+}
+constexpr int QDO_STAGES = 4;
+
+// P^T (into st) and dS^T (into dpt) of one step from S^T, dP^T; MASK = test causality and the document end per element
+template <bool ALIBI, bool MASK>
+__device__ __forceinline__ void bwd_p_ds(float (&st)[BWD_QT / 2], float (&dpt)[BWD_QT / 2], const float* ls, const float* ds,
+                                         const BwdParams& p, const TileLoc& loc, int q0, int wc, const int (&kr)[2], int head,
+                                         uint32_t head_key, bool drop) {
+    // ALIBI: log2(e) * bias of the key row
+    const float slope = ALIBI ? __ldg(p.alibi_slopes + head) : 0.f;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const float bias_r = ALIBI ? attn_alibi_bias(slope, kr[h]) * ATT_LOG2E : 0.f;
+#pragma unroll
+        for (int b = 0; b < BWD_QT / 8; ++b) {
+            const float2 l = *reinterpret_cast<const float2*>(ls + 8 * b + wc);
+            const float2 d = *reinterpret_cast<const float2*>(ds + 8 * b + wc);
+            const float lse_c[2] = {l.x, l.y}, del_c[2] = {d.x, d.y};
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int q = q0 + 8 * b + wc + e;
+                const int i = 4 * b + 2 * h + e;
+                const bool ok = !MASK || (q >= kr[h] && q < loc.doc_len);  // causal, and a real query of the document
+                float pr;
+                if constexpr (ALIBI)
+                    pr = ok ? fast_exp2(fmaf(st[i], p.scale_log2, bias_r) - lse_c[e]) : 0.f;
+                else
+                    pr = ok ? fast_exp2(fmaf(st[i], p.scale_log2, -lse_c[e])) : 0.f;
+                float dp = dpt[i];
+                if (drop) {
+                    const float z = attn_drop_scale(p.drop, head_key, loc.doc_start + q, loc.doc_start + kr[h]);
+                    dp *= z;
+                    st[i] = pr * z;  // dropped-and-rescaled probabilities: what dV sees
+                } else {
+                    st[i] = pr;
+                }
+                dpt[i] = p.scale * pr * (dp - del_c[e]);
+            }
+        }
+    }
+}
 
 template <int HD, bool ALIBI>
-__global__ void __launch_bounds__(BWD_THREADS, 1)
+__global__ void __launch_bounds__(ATT_BWD_THREADS, 1)
     attn_bwd_kernel(const __grid_constant__ CUtensorMap tq64, const __grid_constant__ CUtensorMap tqR,
                     const __grid_constant__ CUtensorMap to64, const __grid_constant__ CUtensorMap toR, const BwdParams p) {
     using CH = HeadChunks<HD>;
@@ -103,21 +172,15 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
     uint8_t* sV = sK + KV_BYTES;
     uint8_t* sQ = sV + KV_BYTES;                // [QDO_STAGES]
     uint8_t* sO = sQ + QDO_STAGES * QT_BYTES;   // [QDO_STAGES] dO
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sO + QDO_STAGES * QT_BYTES);
-    uint64_t* kv_full = bars;       // 1
-    uint64_t* qd_full = bars + 1;   // [QDO_STAGES]
-    uint64_t* qd_empty = bars + 3;  // [QDO_STAGES], one arrive per warp
+    float* sL = reinterpret_cast<float*>(sO + QDO_STAGES * QT_BYTES);  // [QDO_STAGES][LSE * log2 e, Delta][BWD_QT]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sL + QDO_STAGES * 2 * BWD_QT);
+    uint64_t* kv_full = bars;                    // 1
+    uint64_t* qd_full = bars + 1;                // [QDO_STAGES]: TMA bytes + one arrive per lane of producer warp 1
+    uint64_t* qd_empty = bars + 1 + QDO_STAGES;  // [QDO_STAGES], one arrive per consumer warp
 
     const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const float log2e = 1.4426950408889634f;
 
-    auto load_step = [&](int n, int s) {
-        const int hl = n / n_i, qi = i0 + n % n_i;
-        const int head = group * p.q_per_group + hl;
-        const int q_col = (group * (p.q_per_group + 2) + hl) * HD;
-        mbar_expect_tx(&qd_full[s], 2 * QT_BYTES);
-        tma_load_chunked<HD, BWD_QT>(sQ + s * QT_BYTES, &tq64, &tqR, &qd_full[s], q_col, loc.doc_start + qi * BWD_QT);
-        tma_load_chunked<HD, BWD_QT>(sO + s * QT_BYTES, &to64, &toR, &qd_full[s], head * HD, loc.doc_start + qi * BWD_QT);
-    };
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tq64);
         tma_prefetch_desc(&to64);
@@ -127,55 +190,81 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
         }
         mbar_init(kv_full, 1);
         for (int i = 0; i < QDO_STAGES; ++i) {
-            mbar_init(&qd_full[i], 1);
-            mbar_init(&qd_empty[i], BWD_THREADS / 32);
+            mbar_init(&qd_full[i], 1 + 32);
+            mbar_init(&qd_empty[i], 8);
         }
         mbar_fence_init();
         mbar_expect_tx(kv_full, 2 * KV_BYTES);
         tma_load_chunked<HD, ATT_TILE>(sK, &tq64, &tqR, kv_full, k_col, loc.doc_start + k0);
         tma_load_chunked<HD, ATT_TILE>(sV, &tq64, &tqR, kv_full, v_col, loc.doc_start + k0);
-        for (int n = 0; n < QDO_STAGES && n < n_steps; ++n) load_step(n, n);
     }
     __syncthreads();
 
+    if (wg == 0) {
+        // ================= producer =================
+        setmaxnreg_dec<ATT_PRODUCER_REGS>();  // all four warps, before warps 2, 3 leave
+        if (warp == 0) {
+            if (elect_one()) {
+                int s = 0;
+                uint32_t ph = 0;
+                for (int n = 0; n < n_steps; ++n) {
+                    const int hl = n / n_i, qi = i0 + n % n_i;
+                    const int q_col = (group * (p.q_per_group + 2) + hl) * HD;
+                    mbar_wait(&qd_empty[s], ph ^ 1, 32);
+                    mbar_expect_tx(&qd_full[s], 2 * QT_BYTES);
+                    tma_load_chunked<HD, BWD_QT>(sQ + s * QT_BYTES, &tq64, &tqR, &qd_full[s], q_col,
+                                                 loc.doc_start + qi * BWD_QT);
+                    tma_load_chunked<HD, BWD_QT>(sO + s * QT_BYTES, &to64, &toR, &qd_full[s],
+                                                 (group * p.q_per_group + hl) * HD, loc.doc_start + qi * BWD_QT);
+                    if (++s == QDO_STAGES) s = 0, ph ^= 1;
+                }
+            }
+        } else if (warp == 1) {
+            int s = 0;
+            uint32_t ph = 0;
+            for (int n = 0; n < n_steps; ++n) {
+                const int hl = n / n_i, qi = i0 + n % n_i;
+                const int64_t row0 = int64_t(group * p.q_per_group + hl) * p.T + loc.doc_start;
+                mbar_wait(&qd_empty[s], ph ^ 1, 33);
+                float* ls = sL + s * 2 * BWD_QT;
+#pragma unroll
+                for (int r = lane; r < BWD_QT; r += 32) {
+                    const int q = qi * BWD_QT + r;
+                    ls[r] = q < loc.doc_len ? __ldg(p.lse + row0 + q) * log2e : 0.f;
+                    ls[BWD_QT + r] = q < loc.doc_len ? __ldg(p.delta + row0 + q) : 0.f;
+                }
+                mbar_arrive(&qd_full[s]);
+                if (++s == QDO_STAGES) s = 0, ph ^= 1;
+            }
+        }
+        return;
+    }
+
+    // ================= consumers: warpgroup cw owns key rows [k0 + 64 cw, k0 + 64 cw + 64) =================
+    setmaxnreg_inc<ATT_CONSUMER_REGS>();
+    const int cw = wg - 1;
+    const int n_steps_u = __shfl_sync(0xffffffffu, n_steps, 0);  // warp-uniform to ptxas, see attn_dq_kernel
     const int wr = (warp & 3) * 16 + (lane >> 2);  // first of the two accumulator rows of this thread (and wr + 8)
     const int wc = 2 * (lane & 3);                 // first accumulator column inside each n8 block
-    const int kr[2] = {k0 + wg * 64 + wr, k0 + wg * 64 + wr + 8};  // doc-relative keys of the two rows
+    const int kr[2] = {k0 + cw * 64 + wr, k0 + cw * 64 + wr + 8};  // doc-relative keys of the two rows
     const bool drop = p.drop.threshold != 0;
-    const float log2e = 1.4426950408889634f;
-    const uint32_t sk = smem_u32(sK) , sv = smem_u32(sV);
+    const uint32_t sk0 = smem_u32(sK), sv0 = smem_u32(sV);
 
     float dv[HD / 2], dk[HD / 2];
 #pragma unroll
     for (int i = 0; i < HD / 2; ++i) dv[i] = dk[i] = 0.f;
+    float st[BWD_QT / 2], dpt[BWD_QT / 2];
 
-    mbar_wait(kv_full, 0, 30);
-    for (int n = 0; n < n_steps; ++n) {
-        const int s = n & (QDO_STAGES - 1);
-        const int hl = n / n_i, qi = i0 + n % n_i;
-        const int head = group * p.q_per_group + hl;
-        const int q0 = qi * BWD_QT;
-        const uint32_t head_key = dropout_head_key(uint32_t(head), p.drop.key0, p.drop.key1);
-        // LSE / Delta of this thread's 16 query columns
-        float lse_c[BWD_QT / 8][2], del_c[BWD_QT / 8][2];
-#pragma unroll
-        for (int b = 0; b < BWD_QT / 8; ++b)
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-                const int q = q0 + 8 * b + wc + e;
-                const int64_t idx = int64_t(head) * p.T + loc.doc_start + q;
-                lse_c[b][e] = q < loc.doc_len ? __ldg(p.lse + idx) * log2e : 0.f;
-                del_c[b][e] = q < loc.doc_len ? __ldg(p.delta + idx) : 0.f;
-            }
-        mbar_wait(&qd_full[s], (n / QDO_STAGES) & 1, 31);
+    // S^T, dP^T of the step in ring stage s (one commit group)
+    auto issue_ss = [&](int s) {
         const uint32_t sq = smem_u32(sQ + s * QT_BYTES), so = smem_u32(sO + s * QT_BYTES);
-
-        float st[BWD_QT / 2], dpt[BWD_QT / 2];
+        uint32_t sk = sk0, sv = sv0;
+        opaque(sk), opaque(sv);
         wgmma_fence();
 #pragma unroll
         for (int c = 0; c < CH::NCHUNK; ++c) {
             const int w = CH::width(c);
-            const uint32_t krow = CH::offset(c, ATT_TILE) + wg * 64 * 2 * w;  // this warpgroup's 64 key rows of the chunk
+            const uint32_t krow = CH::offset(c, ATT_TILE) + cw * 64 * 2 * w;  // this warpgroup's 64 key rows of the chunk
 #pragma unroll
             for (int k = 0; k < w / 16; ++k) {
                 wgmma_ss<BWD_QT, 0, 0>(st, chunk_desc_kmajor(sk + krow, w, k), chunk_desc_kmajor(sq + CH::offset(c, BWD_QT), w, k),
@@ -185,39 +274,28 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
             }
         }
         wgmma_commit();
+    };
+
+    mbar_spin(kv_full, 0);
+    int s = 0;
+    uint32_t ph = 0;
+    for (int n = 0; n < n_steps_u; ++n) {
+        const int hl = n / n_i, qi = i0 + n % n_i;
+        const int head = group * p.q_per_group + hl;
+        const int q0 = qi * BWD_QT;
+        const uint32_t head_key = dropout_head_key(uint32_t(head), p.drop.key0, p.drop.key1);
+        mbar_spin(&qd_full[s], ph);
+        issue_ss(s);
         wgmma_wait<0>();
         reg_fence<BWD_QT / 2>(st);
         reg_fence<BWD_QT / 2>(dpt);
 
         // ---------------- P^T, dS^T ----------------
-        // ALIBI: log2(e) * bias of the key row, computed here rather than before the MMAs so that it is not live across them
-        const float slope = ALIBI ? __ldg(p.alibi_slopes + head) : 0.f;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const float bias_r = ALIBI ? attn_alibi_bias(slope, kr[h]) * ATT_LOG2E : 0.f;
-#pragma unroll
-            for (int b = 0; b < BWD_QT / 8; ++b)
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const int q = q0 + 8 * b + wc + e;
-                    const int i = 4 * b + 2 * h + e;
-                    const bool ok = q >= kr[h] && q < loc.doc_len;  // causal, and a real query of the document
-                    float pr;
-                    if constexpr (ALIBI)
-                        pr = ok ? fast_exp2(fmaf(st[i], p.scale_log2, bias_r) - lse_c[b][e]) : 0.f;
-                    else
-                        pr = ok ? fast_exp2(fmaf(st[i], p.scale_log2, -lse_c[b][e])) : 0.f;
-                    float dp = dpt[i];
-                    if (drop) {
-                        const float z = attn_drop_scale(p.drop, head_key, loc.doc_start + q, loc.doc_start + kr[h]);
-                        dp *= z;
-                        st[i] = pr * z;  // dropped-and-rescaled probabilities: what dV sees
-                    } else {
-                        st[i] = pr;
-                    }
-                    dpt[i] = p.scale * pr * (dp - del_c[b][e]);
-                }
-        }
+        const float* ls = sL + s * 2 * BWD_QT;
+        if (qi <= i0 + cw || (qi + 1) * BWD_QT > loc.doc_len)
+            bwd_p_ds<ALIBI, true>(st, dpt, ls, ls + BWD_QT, p, loc, q0, wc, kr, head, head_key, drop);
+        else
+            bwd_p_ds<ALIBI, false>(st, dpt, ls, ls + BWD_QT, p, loc, q0, wc, kr, head, head_key, drop);
         uint32_t pa[BWD_QT / 16][4], da[BWD_QT / 16][4];
 #pragma unroll
         for (int kk = 0; kk < BWD_QT / 16; ++kk) {
@@ -226,6 +304,8 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
         }
 
         // ---------------- dV += P^T dO,  dK += dS^T Q ----------------
+        uint32_t sq = smem_u32(sQ + s * QT_BYTES), so = smem_u32(sO + s * QT_BYTES);
+        opaque(sq), opaque(so);
         wgmma_fence();
 #pragma unroll
         for (int c = 0; c < CH::NCHUNK; ++c) {
@@ -242,16 +322,12 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
             }
         }
         wgmma_commit();
-
         wgmma_wait<0>();
         reg_fence<HD / 2>(dv);
         reg_fence<HD / 2>(dk);
-        if (lane == 0) mbar_arrive(&qd_empty[s]);  // Q_i / dO_i of this warp's MMAs are read
-        if (threadIdx.x == 0 && n + QDO_STAGES < n_steps) {
-            mbar_wait(&qd_empty[s], (n / QDO_STAGES) & 1, 32);
-            load_step(n + QDO_STAGES, s);
-        }
         __syncwarp();
+        mbar_arrive_lane0(&qd_empty[s], lane);  // Q_i / dO_i / LSE_i / Delta_i of this warp's step are read
+        if (++s == QDO_STAGES) s = 0, ph ^= 1;
     }
 
     // ---------------- dK_j, dV_j -> the k / v slots of dqkv ----------------
@@ -275,7 +351,8 @@ int launch_bwd(const void* dout, const void* qkv, int64_t row_stride, const BwdP
     if (rc) return rc;
     rc = attn_make_maps<HD>(dout, int64_t(p.n_heads) * HD, p.T, &to64, &toR);
     if (rc) return rc;
-    constexpr int smem_bytes = 1024 + 2 * CH::tile_bytes(ATT_TILE) + 2 * QDO_STAGES * CH::tile_bytes(BWD_QT) + 128;
+    constexpr int smem_bytes = 1024 + 2 * CH::tile_bytes(ATT_TILE) + 2 * QDO_STAGES * CH::tile_bytes(BWD_QT) +
+                               QDO_STAGES * 2 * BWD_QT * 4 + 128;
     static_assert(smem_bytes <= 232448, "attention backward shared memory budget exceeded");
     auto kern = attn_bwd_kernel<HD, ALIBI>;
     static bool attr_set = false;
@@ -286,23 +363,66 @@ int launch_bwd(const void* dout, const void* qkv, int64_t row_stride, const BwdP
     const int64_t max_tiles = (p.T + ATT_TILE - 1) / ATT_TILE + p.n_docs;
     DOLO_REQUIRE(max_tiles == p.n_tile_slots && max_tiles * p.n_groups < (1ll << 31), "attn_bwd: grid too large");
     dim3 grid((unsigned)(max_tiles * p.n_groups));
-    kern<<<grid, BWD_THREADS, smem_bytes, st>>>(tq64, tqR, to64, toR, p);
+    kern<<<grid, ATT_BWD_THREADS, smem_bytes, st>>>(tq64, tqR, to64, toR, p);
     DOLO_LAUNCH_OK("attn_varlen_bwd");
     return DOLO_OK;
 }
 
-// dQ of the backward: one CTA = one 128-row query tile of one head of one document, two warpgroups of 64 queries each,
-// looping over the 64-row key tiles the queries see, in order.  Per key tile every warpgroup recomputes
+// dQ of the backward: one CTA = one 128-row query tile of one head of one document, two consumer warpgroups of 64 queries
+// each, looping over the 64-row key tiles the queries see, in order.  Per key tile every consumer warpgroup recomputes
 //     S  = Q_i K_j^T ,  dP = dO_i V_j^T           (SS)
 //     dS = scale * P o (dP - Delta_i)             (registers, P = exp2(S*scale - LSE_i))
 //     dQ_i += dS K_j                              (RS, B = K MN-major)
-// and finally writes dQ_i (bf16) into the q slots of dqkv.  Thread 0 issues the TMA loads: Q_i and dO_i once, (K_j, V_j)
-// through a 2-stage ring.  ALIBI: P = exp2(log2(e) * (S*scale + bias_k) - LSE_i), one bias per key column of the thread.
-constexpr int DQ_THREADS = 256;
+// and finally writes dQ_i (bf16) into the q slots of dqkv.  Thread 0 loads Q_i and dO_i once; an elected producer lane
+// streams (K_j, V_j) through a KV_STAGES-deep ring.  Only the key tiles that reach the warpgroup's diagonal, and every key
+// tile of a query tile that crosses the document end, test the causal / bounds predicate.  The SS MMAs of key tile j + 1
+// are issued right behind the RS MMAs of key tile j.  ALIBI: P = exp2(log2(e) * (S*scale + bias_k) - LSE_i), one bias per
+// key column of the thread.
 constexpr int DQ_KT = 64;  // keys per step
+constexpr int KV_STAGES = 4;
+
+// dS (into sc) of key tile j from S, dP; MASK = test causality and the document end per element
+template <bool ALIBI, bool MASK>
+__device__ __forceinline__ void dq_ds(float (&sc)[DQ_KT / 2], const float (&dp)[DQ_KT / 2], const BwdParams& p,
+                                      const TileLoc& loc, int j, int wc, const int (&qr)[2], const float (&lse_r)[2],
+                                      const float (&del_r)[2], float slope, uint32_t head_key, bool drop) {
+    if constexpr (ALIBI) {
+#pragma unroll
+        for (int b = 0; b < DQ_KT / 8; ++b)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int k = j * DQ_KT + 8 * b + wc + e;
+                const float bl = attn_alibi_bias(slope, k) * ATT_LOG2E;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int i = 4 * b + 2 * h + e;
+                    const bool ok = !MASK || (k <= qr[h] && qr[h] < loc.doc_len);
+                    const float pr = ok ? fast_exp2(fmaf(sc[i], p.scale_log2, bl) - lse_r[h]) : 0.f;
+                    float d = dp[i];
+                    if (drop) d *= attn_drop_scale(p.drop, head_key, loc.doc_start + qr[h], loc.doc_start + k);
+                    sc[i] = p.scale * pr * (d - del_r[h]);
+                }
+            }
+    } else {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int b = 0; b < DQ_KT / 8; ++b)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int k = j * DQ_KT + 8 * b + wc + e;
+                    const int i = 4 * b + 2 * h + e;
+                    const bool ok = !MASK || (k <= qr[h] && qr[h] < loc.doc_len);  // causal, and a real query of the document
+                    const float pr = ok ? fast_exp2(fmaf(sc[i], p.scale_log2, -lse_r[h])) : 0.f;
+                    float d = dp[i];
+                    if (drop) d *= attn_drop_scale(p.drop, head_key, loc.doc_start + qr[h], loc.doc_start + k);
+                    sc[i] = p.scale * pr * (d - del_r[h]);
+                }
+    }
+}
 
 template <int HD, bool ALIBI>
-__global__ void __launch_bounds__(DQ_THREADS, 1)
+__global__ void __launch_bounds__(ATT_BWD_THREADS, 1)
     attn_dq_kernel(const __grid_constant__ CUtensorMap tq64, const __grid_constant__ CUtensorMap tqR,
                    const __grid_constant__ CUtensorMap to64, const __grid_constant__ CUtensorMap toR, const BwdParams p) {
     using CH = HeadChunks<HD>;
@@ -325,20 +445,15 @@ __global__ void __launch_bounds__(DQ_THREADS, 1)
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_align_1024(smem_raw);
     uint8_t* sQ = smem;
-    uint8_t* sO = sQ + Q_BYTES;       // dO
-    uint8_t* sK = sO + Q_BYTES;       // [2]
-    uint8_t* sV = sK + 2 * KT_BYTES;  // [2]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sV + 2 * KT_BYTES);
-    uint64_t* q_full = bars;        // 1
-    uint64_t* kv_full = bars + 1;   // [2]
-    uint64_t* kv_empty = bars + 3;  // [2], one arrive per warp
+    uint8_t* sO = sQ + Q_BYTES;               // dO
+    uint8_t* sK = sO + Q_BYTES;               // [KV_STAGES]
+    uint8_t* sV = sK + KV_STAGES * KT_BYTES;  // [KV_STAGES]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sV + KV_STAGES * KT_BYTES);
+    uint64_t* q_full = bars;                    // 1
+    uint64_t* kv_full = bars + 1;               // [KV_STAGES]
+    uint64_t* kv_empty = bars + 1 + KV_STAGES;  // [KV_STAGES], one arrive per consumer warp
 
     const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    auto load_kv = [&](int j, int s) {
-        mbar_expect_tx(&kv_full[s], 2 * KT_BYTES);
-        tma_load_chunked<HD, DQ_KT>(sK + s * KT_BYTES, &tq64, &tqR, &kv_full[s], k_col, loc.doc_start + j * DQ_KT);
-        tma_load_chunked<HD, DQ_KT>(sV + s * KT_BYTES, &tq64, &tqR, &kv_full[s], v_col, loc.doc_start + j * DQ_KT);
-    };
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tq64);
         tma_prefetch_desc(&to64);
@@ -347,21 +462,42 @@ __global__ void __launch_bounds__(DQ_THREADS, 1)
             tma_prefetch_desc(&toR);
         }
         mbar_init(q_full, 1);
-        for (int i = 0; i < 2; ++i) {
+        for (int i = 0; i < KV_STAGES; ++i) {
             mbar_init(&kv_full[i], 1);
-            mbar_init(&kv_empty[i], DQ_THREADS / 32);
+            mbar_init(&kv_empty[i], 8);
         }
         mbar_fence_init();
         mbar_expect_tx(q_full, 2 * Q_BYTES);
         tma_load_chunked<HD, ATT_TILE>(sQ, &tq64, &tqR, q_full, q_col, loc.doc_start + q0);
         tma_load_chunked<HD, ATT_TILE>(sO, &to64, &toR, q_full, head * HD, loc.doc_start + q0);
-        for (int j = 0; j < 2 && j < n_kt; ++j) load_kv(j, j);
     }
     __syncthreads();
 
+    if (wg == 0) {
+        // ================= producer =================
+        setmaxnreg_dec<ATT_PRODUCER_REGS>();
+        if (warp == 0 && elect_one()) {
+            int s = 0;
+            uint32_t ph = 0;
+            for (int j = 0; j < n_kt; ++j) {
+                mbar_wait(&kv_empty[s], ph ^ 1, 42);
+                mbar_expect_tx(&kv_full[s], 2 * KT_BYTES);
+                tma_load_chunked<HD, DQ_KT>(sK + s * KT_BYTES, &tq64, &tqR, &kv_full[s], k_col, loc.doc_start + j * DQ_KT);
+                tma_load_chunked<HD, DQ_KT>(sV + s * KT_BYTES, &tq64, &tqR, &kv_full[s], v_col, loc.doc_start + j * DQ_KT);
+                if (++s == KV_STAGES) s = 0, ph ^= 1;
+            }
+        }
+        return;
+    }
+
+    // ================= consumers: warpgroup cw owns queries [q0 + 64 cw, q0 + 64 cw + 64) =================
+    setmaxnreg_inc<ATT_CONSUMER_REGS>();
+    const int cw = wg - 1;
+    // the key-tile count, read back through a shuffle, is warp-uniform to ptxas: the loop branches with an SS group in flight
+    const int n_kt_u = __shfl_sync(0xffffffffu, n_kt, 0);
     const int wr = (warp & 3) * 16 + (lane >> 2);
     const int wc = 2 * (lane & 3);
-    const int qr[2] = {q0 + wg * 64 + wr, q0 + wg * 64 + wr + 8};  // doc-relative queries of the two rows
+    const int qr[2] = {q0 + cw * 64 + wr, q0 + cw * 64 + wr + 8};  // doc-relative queries of the two rows
     const bool drop = p.drop.threshold != 0;
     const uint32_t head_key = dropout_head_key(uint32_t(head), p.drop.key0, p.drop.key1);
     const float log2e = 1.4426950408889634f;
@@ -374,22 +510,23 @@ __global__ void __launch_bounds__(DQ_THREADS, 1)
         lse_r[h] = ok ? __ldg(p.lse + idx) * log2e : 0.f;
         del_r[h] = ok ? __ldg(p.delta + idx) : 0.f;
     }
+    // key tiles j >= j_diag reach this warpgroup's diagonal; all of them test the predicate if its rows cross the document end
+    const int j_diag = (q0 + cw * 64 + 64 > loc.doc_len) ? 0 : q0 / DQ_KT + cw;
     const uint32_t sq = smem_u32(sQ), so = smem_u32(sO);
     float dq[HD / 2];
 #pragma unroll
     for (int i = 0; i < HD / 2; ++i) dq[i] = 0.f;
+    float sc[DQ_KT / 2], dp[DQ_KT / 2];
 
-    mbar_wait(q_full, 0, 40);
-    for (int j = 0; j < n_kt; ++j) {
-        const int s = j & 1;
-        mbar_wait(&kv_full[s], (j >> 1) & 1, 41);
-        const uint32_t sk = smem_u32(sK + s * KT_BYTES), sv = smem_u32(sV + s * KT_BYTES);
-        float sc[DQ_KT / 2], dp[DQ_KT / 2];
+    // S, dP of the key tile in ring stage s (one commit group)
+    auto issue_ss = [&](int s) {
+        uint32_t sk = smem_u32(sK + s * KT_BYTES), sv = smem_u32(sV + s * KT_BYTES);
+        opaque(sk), opaque(sv);
         wgmma_fence();
 #pragma unroll
         for (int c = 0; c < CH::NCHUNK; ++c) {
             const int w = CH::width(c);
-            const uint32_t qrow = CH::offset(c, ATT_TILE) + wg * 64 * 2 * w;  // this warpgroup's 64 query rows of the chunk
+            const uint32_t qrow = CH::offset(c, ATT_TILE) + cw * 64 * 2 * w;  // this warpgroup's 64 query rows of the chunk
 #pragma unroll
             for (int k = 0; k < w / 16; ++k) {
                 wgmma_ss<DQ_KT, 0, 0>(sc, chunk_desc_kmajor(sq + qrow, w, k), chunk_desc_kmajor(sk + CH::offset(c, DQ_KT), w, k),
@@ -399,46 +536,31 @@ __global__ void __launch_bounds__(DQ_THREADS, 1)
             }
         }
         wgmma_commit();
+    };
+
+    mbar_spin(q_full, 0);
+    int s = 0;
+    uint32_t ph = 0;
+    mbar_spin(&kv_full[0], 0);
+    issue_ss(0);
+    for (int j = 0; j < n_kt_u; ++j) {
         wgmma_wait<0>();
         reg_fence<DQ_KT / 2>(sc);
         reg_fence<DQ_KT / 2>(dp);
-
-        if constexpr (ALIBI) {
-#pragma unroll
-            for (int b = 0; b < DQ_KT / 8; ++b)
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const int k = j * DQ_KT + 8 * b + wc + e;
-                    const float bl = attn_alibi_bias(slope, k) * ATT_LOG2E;
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const int i = 4 * b + 2 * h + e;
-                        const bool ok = k <= qr[h] && qr[h] < loc.doc_len;
-                        const float pr = ok ? fast_exp2(fmaf(sc[i], p.scale_log2, bl) - lse_r[h]) : 0.f;
-                        float d = dp[i];
-                        if (drop) d *= attn_drop_scale(p.drop, head_key, loc.doc_start + qr[h], loc.doc_start + k);
-                        sc[i] = p.scale * pr * (d - del_r[h]);
-                    }
-                }
-        } else
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-#pragma unroll
-            for (int b = 0; b < DQ_KT / 8; ++b)
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const int k = j * DQ_KT + 8 * b + wc + e;
-                    const int i = 4 * b + 2 * h + e;
-                    const bool ok = k <= qr[h] && qr[h] < loc.doc_len;  // causal, and a real query of the document
-                    const float pr = ok ? fast_exp2(fmaf(sc[i], p.scale_log2, -lse_r[h])) : 0.f;
-                    float d = dp[i];
-                    if (drop) d *= attn_drop_scale(p.drop, head_key, loc.doc_start + qr[h], loc.doc_start + k);
-                    sc[i] = p.scale * pr * (d - del_r[h]);
-                }
+        if (j >= j_diag)
+            dq_ds<ALIBI, true>(sc, dp, p, loc, j, wc, qr, lse_r, del_r, slope, head_key, drop);
+        else
+            dq_ds<ALIBI, false>(sc, dp, p, loc, j, wc, qr, lse_r, del_r, slope, head_key, drop);
         uint32_t da[DQ_KT / 16][4];
 #pragma unroll
         for (int kk = 0; kk < DQ_KT / 16; ++kk) acc_to_a_frag(sc, kk, da[kk]);
 
+        const int s1 = s + 1 == KV_STAGES ? 0 : s + 1;
+        const uint32_t ph1 = s1 == 0 ? ph ^ 1 : ph;
+        const bool more = j + 1 < n_kt_u;
+        if (more) mbar_spin(&kv_full[s1], ph1);
+        uint32_t sk = smem_u32(sK + s * KT_BYTES);
+        opaque(sk);
         wgmma_fence();
 #pragma unroll
         for (int c = 0; c < CH::NCHUNK; ++c) {
@@ -453,14 +575,17 @@ __global__ void __launch_bounds__(DQ_THREADS, 1)
             }
         }
         wgmma_commit();
-        wgmma_wait<0>();
-        reg_fence<HD / 2>(dq);
-        if (lane == 0) mbar_arrive(&kv_empty[s]);
-        if (threadIdx.x == 0 && j + 2 < n_kt) {
-            mbar_wait(&kv_empty[s], (j >> 1) & 1, 42);  // both warpgroups are done with key tile j
-            load_kv(j + 2, s);
+
+        if (more) {
+            issue_ss(s1);
+            wgmma_wait<1>();  // the RS group of key tile j is done; the SS group of key tile j + 1 runs on
+        } else {
+            wgmma_wait<0>();
         }
+        reg_fence<HD / 2>(dq);
         __syncwarp();
+        mbar_arrive_lane0(&kv_empty[s], lane);  // K_j / V_j of this warp's MMAs are read
+        s = s1, ph = ph1;
     }
 
 #pragma unroll
@@ -481,7 +606,7 @@ int launch_dq(const void* dout, const void* qkv, int64_t row_stride, const BwdPa
     if (rc) return rc;
     rc = attn_make_maps<HD>(dout, int64_t(p.n_heads) * HD, p.T, &to64, &toR);
     if (rc) return rc;
-    constexpr int smem_bytes = 1024 + 2 * CH::tile_bytes(ATT_TILE) + 4 * CH::tile_bytes(DQ_KT) + 128;
+    constexpr int smem_bytes = 1024 + 2 * CH::tile_bytes(ATT_TILE) + 2 * KV_STAGES * CH::tile_bytes(DQ_KT) + 128;
     static_assert(smem_bytes <= 232448, "attention dQ shared memory budget exceeded");
     auto kern = attn_dq_kernel<HD, ALIBI>;
     static bool attr_set = false;
@@ -492,7 +617,7 @@ int launch_dq(const void* dout, const void* qkv, int64_t row_stride, const BwdPa
     const int64_t max_tiles = (p.T + ATT_TILE - 1) / ATT_TILE + p.n_docs;
     DOLO_REQUIRE(max_tiles == p.n_tile_slots && max_tiles * p.n_heads < (1ll << 31), "attn_bwd: grid too large");
     dim3 grid((unsigned)(max_tiles * p.n_heads));
-    kern<<<grid, DQ_THREADS, smem_bytes, st>>>(tq64, tqR, to64, toR, p);
+    kern<<<grid, ATT_BWD_THREADS, smem_bytes, st>>>(tq64, tqR, to64, toR, p);
     DOLO_LAUNCH_OK("attn_varlen_bwd_dq");
     return DOLO_OK;
 }
