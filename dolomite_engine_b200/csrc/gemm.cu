@@ -1,12 +1,13 @@
-// bf16 GEMM for sm_90a (H100):  TMA (cp.async.bulk.tensor) -> 128B-swizzled smem ring -> wgmma (m64n128k16 or
-// m64n256k16 per consumer warpgroup, fp32 accumulators in registers) -> epilogue (alpha / bias / beta*C, bf16 | fp32)
-// through double-buffered shared-memory slabs -> asynchronous TMA stores.
+// bf16 and fp8 GEMM for sm_90a (H100):  TMA (cp.async.bulk.tensor) -> 128B-swizzled smem ring -> wgmma (m64n128 or
+// m64n256 per consumer warpgroup, fp32 accumulators in registers) -> epilogue (scale / alpha / bias / beta*C, bf16 |
+// fp32) through double-buffered shared-memory slabs -> asynchronous TMA stores.
 //
-// Persistent, warp-specialised: warpgroup 0 = producer (one elected thread issues the TMA loads; the whole first warp for
+// One kernel body serves both operand types; an operand policy (Bf16Ops, Fp8Ops) names what differs.  Persistent,
+// warp-specialised: warpgroup 0 = producer (one elected thread issues the TMA loads; the whole first warp for
 // gather-on-load), warpgroups 1 and 2 = consumers, each owning 64 rows of the output tile.  The tile is 128 x 128 (six
-// 32 KB stages) or, for dense launches, 128 x 256 (four 48 KB stages; setmaxnreg moves registers from the producer to
-// the consumers, which hold 128 accumulators each).  choose_tile_n picks the width per launch from the tile counts.
-// Both operands may be K-major (row-major [rows, K]) or MN-major (stored [K, rows]); the latter is what dgrad / wgrad
+// 32 KB stages) or, for dense bf16 launches, 128 x 256 (four 48 KB stages; setmaxnreg moves registers from the producer
+// to the consumers, which hold 128 accumulators each).  choose_tile_n picks the width per launch from the tile counts.
+// bf16 operands may be K-major (row-major [rows, K]) or MN-major (stored [K, rows]); the latter is what dgrad / wgrad
 // need, so no transposes are ever materialised:
 //     fwd   Y[T,N]  = X[T,K]  . W[N,K]^T          A K-major,  B K-major
 //     dgrad dX[T,K] = dY[T,N] . W[N,K]            A K-major,  B MN-major (stored [N(contraction), K(out)])
@@ -22,23 +23,18 @@ using namespace dolo;
 namespace {
 
 constexpr int BM = 128;
-constexpr int BN = 128;  // tile width of the grouped, gather-on-load and split-K modes and of the fp8 kernel
-constexpr int BK = 64;   // 64 bf16 = 128 bytes = one swizzle span
-constexpr int STAGES = 6;
+constexpr int BN = 128;  // tile width of the grouped, gather-on-load and split-K modes and of fp8 launches
+constexpr int BK = 64;   // bf16 k-block: 64 bf16 = 128 bytes = one swizzle span
 constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KB
-constexpr int B_STAGE_BYTES = BN * BK * 2;  // 16 KB
-constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
 constexpr int GEMM_THREADS = 384;  // warpgroup 0 producer, 1..2 consumers
-constexpr int SMEM_BYTES = 1024 /*align slack*/ + STAGES * STAGE_BYTES + 256 /*barriers*/;
-static_assert(SMEM_BYTES <= 232448, "shared memory budget exceeded (227 KB per block on sm_90)");
 
-// Epilogue staging of the bf16 kernel: each consumer warpgroup owns two slabs of 64 rows x 128 B (64 bf16 or 32 fp32
+// Epilogue staging: each consumer warpgroup owns two slabs of 64 rows x 128 B (64 bf16 or 32 fp32
 // columns, 128B-swizzled like the D / C tensor maps) and a copy of the tile's bias slice (up to 256 bf16).
 constexpr int EPI_SLAB_BYTES = 64 * 128;
 constexpr int EPI_BYTES = 2 /*warpgroups*/ * 2 /*slabs*/ * EPI_SLAB_BYTES;
 constexpr int EPI_BIAS_BYTES = 2 /*warpgroups*/ * 256 * 2;
 
-// Shared memory of the bf16 kernel per output tile width TN: the stage ring (128 x 128 keeps six 32 KB stages, 128 x 256
+// Shared memory of the kernel per output tile width TN: the stage ring (128 x 128 keeps six 32 KB stages, 128 x 256
 // four 48 KB stages), then the epilogue slabs, the bias slices and the barriers.
 template <int TN>
 struct Ring {
@@ -70,8 +66,8 @@ constexpr double TILE256_COST = 1.65;
 
 constexpr int MAXP = 4;  // problems per launch (the four weight gradients of a transformer block share one launch)
 
-// d / c: rank-3 maps {N, M, groups} of D and C with a box of one epilogue slab {128 B of columns, 64 rows, 1} (bf16 kernel
-// only; the group dimension is 1 except for the K-grouped expert weight gradients)
+// d / c: rank-3 maps {N, M, groups} of D and C with a box of one epilogue slab {128 B of columns, 64 rows, 1} (the group
+// dimension is 1 except for the K-grouped expert weight gradients)
 struct GemmMaps {
     CUtensorMap a[MAXP], b[MAXP], d[MAXP], c[MAXP];
 };
@@ -108,6 +104,8 @@ struct GemmParams {
     int b_group_rows;
     const int* group_k_offsets;
     int num_groups;
+    const float* a_scale_inv[MAXP];  // fp8: scale_inv of A and of B per problem (device scalars)
+    const float* b_scale_inv[MAXP];
 };
 
 struct TileInfo {
@@ -129,6 +127,8 @@ __device__ __forceinline__ void tile_coords(int t, int num_m, int num_n, int gm,
     n_blk = r / gsize;
 }
 
+// GROUPED: the operand type has the launch modes of p.grouped (otherwise every launch is dense)
+template <bool GROUPED>
 __device__ __forceinline__ TileInfo tile_info(int t, const GemmParams& p) {
     TileInfo ti;
     ti.q = 0;
@@ -141,7 +141,7 @@ __device__ __forceinline__ TileInfo tile_info(int t, const GemmParams& p) {
     ti.kb0 = 0;
     ti.kb1 = pr.num_kb;
     ti.valid = true;
-    if (p.grouped == 3) {
+    if (GROUPED && p.grouped == 3) {
         // split-K: tile index also enumerates the K split; partial products are reduce-added (TMA, fp32)
         const int per = pr.num_m * pr.num_n;
         const int split = t / per;
@@ -150,7 +150,7 @@ __device__ __forceinline__ TileInfo tile_info(int t, const GemmParams& p) {
         ti.kb0 = split * kb_per;
         ti.kb1 = min(pr.num_kb, ti.kb0 + kb_per);
         ti.valid = ti.kb1 > ti.kb0;
-    } else if (p.grouped == 2) {
+    } else if (GROUPED && p.grouped == 2) {
         const int per = pr.num_m * pr.num_n;
         ti.grp = t / per;
         tile_coords(t - ti.grp * per, pr.num_m, pr.num_n, pr.group_m, ti.m_blk, ti.n_blk);
@@ -159,7 +159,7 @@ __device__ __forceinline__ TileInfo tile_info(int t, const GemmParams& p) {
         ti.valid = ti.kb1 > ti.kb0;
     } else {
         tile_coords(t, pr.num_m, pr.num_n, pr.group_m, ti.m_blk, ti.n_blk);
-        if (p.grouped == 1) {
+        if (GROUPED && p.grouped == 1) {
             ti.grp = p.m_tile_group[ti.m_blk];
             ti.valid = ti.grp >= 0;
         }
@@ -214,16 +214,19 @@ struct Epilogue {
         named_bar_sync(1 + cw, 128);
     }
 
-    // D tile (row0, col0) of group grp = (acc + bias) * alpha (+ beta * C), written (or reduce-added) through the slabs.
-    // The fp32 expression and its order are those of a plain register epilogue, so results do not depend on the path.
-    template <int TN, bool F32>
+    // D tile (row0, col0) of group grp = (acc + bias) * alpha (+ beta * C), or with SCALED (s * acc + bias) * alpha
+    // (+ beta * C), written (or reduce-added) through the slabs.  The fp32 expression and its order are those of a plain
+    // register epilogue, so results do not depend on the path.  s stays inside the expression (s * acc + bias contracts
+    // to one FFMA), so it is not folded into the accumulators beforehand.
+    template <int TN, bool F32, bool SCALED>
     __device__ __forceinline__ void store(const float (&acc)[TN / 2], const CUtensorMap* dmap, const CUtensorMap* cmap,
-                                          int col0, int row0, int grp, float alpha, float beta, bool has_bias, bool has_c,
-                                          bool reduce) {
+                                          int col0, int row0, int grp, float s, float alpha, float beta, bool has_bias,
+                                          bool has_c, bool reduce) {
         constexpr int CHUNK = F32 ? 32 : 64;  // columns of one slab
         constexpr int NB = CHUNK / 8;         // n8 accumulator blocks per slab
         const int lane = threadIdx.x & 31;
         const int wrow = ((threadIdx.x >> 5) & 3) * 16;  // this warp's first row inside the warpgroup's 64
+        auto scaled = [s](float a) { return SCALED ? s * a : a; };
 #pragma unroll
         for (int ch = 0; ch < TN / CHUNK; ++ch) {
             uint8_t* sl = slabs + slab * EPI_SLAB_BYTES;
@@ -248,15 +251,15 @@ struct Epilogue {
                     for (int h = 0; h < 2; ++h) {
                         const int r = wrow + 8 * h + (lane >> 2);
                         const int byte = jj * 32 + (lane & 3) * 8;
-                        float2* s = reinterpret_cast<float2*>(sl + r * 128 + ((((byte >> 4) ^ (r & 7)) << 4) | (byte & 15)));
-                        float v0 = (acc[4 * j + 2 * h] + b0) * alpha;
-                        float v1 = (acc[4 * j + 2 * h + 1] + b1) * alpha;
+                        float2* d = reinterpret_cast<float2*>(sl + r * 128 + ((((byte >> 4) ^ (r & 7)) << 4) | (byte & 15)));
+                        float v0 = (scaled(acc[4 * j + 2 * h]) + b0) * alpha;
+                        float v1 = (scaled(acc[4 * j + 2 * h + 1]) + b1) * alpha;
                         if (has_c) {
-                            const float2 c2 = *s;
+                            const float2 c2 = *d;
                             v0 += beta * c2.x;
                             v1 += beta * c2.y;
                         }
-                        *s = make_float2(v0, v1);
+                        *d = make_float2(v0, v1);
                     }
                 }
             } else {
@@ -277,8 +280,8 @@ struct Epilogue {
                             b0 = bf16_lo(bv);
                             b1 = bf16_hi(bv);
                         }
-                        float v0 = (acc[4 * j + 2 * h] + b0) * alpha;
-                        float v1 = (acc[4 * j + 2 * h + 1] + b1) * alpha;
+                        float v0 = (scaled(acc[4 * j + 2 * h]) + b0) * alpha;
+                        float v1 = (scaled(acc[4 * j + 2 * h + 1]) + b1) * alpha;
                         if (has_c) {
                             v0 += beta * bf16_lo(cv[i]);
                             v1 += beta * bf16_hi(cv[i]);
@@ -323,11 +326,43 @@ struct Epilogue {
     }
 };
 
-// TN: output tile width.  The 128 x 256 tile runs dense launches only (grouped == 0, no gather), because the grouped
+// Operand policies: what differs between the bf16 and the fp8 instances of the kernel body.  A k-block is one 128-byte
+// swizzle span of a row in both (64 bf16 or 128 fp8 elements), so the stages, the TMA boxes in bytes and the shared-memory
+// descriptors (+32 B per MMA step, four steps per k-block) are the same.
+//   KB_ELEMS  elements per k-block (the K coordinate of the TMA loads)
+//   mma       one MMA step of a consumer warpgroup: wgmma k16 bf16, or k32 fp8 (K-major operands, 128-wide tile only)
+//   SPLIT     promote per k-block: the accumulator is added into a second register set after every k-block and the
+//             next k-block starts from zero (TransformerEngine's split accumulator, used for dgrad / wgrad)
+//   SCALED    the epilogue has a scale: s = scale_inv_a * scale_inv_b of the problem
+//   GROUPED   the launch modes of p.grouped (grouped experts, gather-on-load, split-K) and MN-major operands exist
+template <bool A_MN_, bool B_MN_>
+struct Bf16Ops {
+    static constexpr bool A_MN = A_MN_, B_MN = B_MN_;
+    static constexpr int KB_ELEMS = BK;
+    static constexpr bool SPLIT = false, SCALED = false, GROUPED = true;
+    template <int TN>
+    static __device__ __forceinline__ void mma(float (&acc)[TN / 2], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+        wgmma_ss<TN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc, bdesc, scale_d);
+    }
+};
+
+template <int FA, int FB, bool SPLIT_>
+struct Fp8Ops {
+    static constexpr bool A_MN = false, B_MN = false;
+    static constexpr int KB_ELEMS = 128;
+    static constexpr bool SPLIT = SPLIT_, SCALED = true, GROUPED = false;
+    template <int TN>
+    static __device__ __forceinline__ void mma(float (&acc)[TN / 2], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+        static_assert(TN == 128, "fp8 tiles are 128 wide");
+        wgmma_fp8_n128<FA, FB>(acc, adesc, bdesc, scale_d);
+    }
+};
+
+// TN: output tile width.  The 128 x 256 tile runs dense bf16 launches only (grouped == 0, no gather), because the grouped
 // modes' tile tables are per 128 x 128 tile.
-template <bool A_MN, bool B_MN, int TN>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-    gemm_bf16_kernel(const __grid_constant__ GemmMaps maps, const __grid_constant__ GemmParams p) {
+template <class Op, int TN>
+__device__ __forceinline__ void gemm_body(const GemmMaps& maps, const GemmParams& p) {
+    constexpr bool A_MN = Op::A_MN, B_MN = Op::B_MN;
     constexpr int STAGES = Ring<TN>::STAGES;
     constexpr int B_STAGE_BYTES = Ring<TN>::B_BYTES;
     constexpr int STAGE_BYTES = Ring<TN>::STAGE_BYTES;
@@ -344,7 +379,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     const int num_tiles = p.num_tiles;
-    const bool gather = TN == 128 && !A_MN && p.a_row_index != nullptr;
+    const bool gather = Op::GROUPED && TN == 128 && !A_MN && p.a_row_index != nullptr;
 
     if (threadIdx.x == 0) {
         for (int q = 0; q < p.n_prob; ++q) {
@@ -373,7 +408,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
             int stage = 0;
             uint32_t phase = 0;
             for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-                const TileInfo ti = tile_info(t, p);
+                const TileInfo ti = tile_info<Op::GROUPED>(t, p);
                 if (!ti.valid) continue;
                 const CUtensorMap* tmap_b = &maps.b[ti.q];
                 const int b_outer = ti.grp * p.b_group_rows;
@@ -414,27 +449,27 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
             int stage = 0;
             uint32_t phase = 0;
             for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-                const TileInfo ti = tile_info(t, p);
+                const TileInfo ti = tile_info<Op::GROUPED>(t, p);
                 if (!ti.valid) continue;
                 const CUtensorMap* tmap_a = &maps.a[ti.q];
                 const CUtensorMap* tmap_b = &maps.b[ti.q];
                 const uint64_t ha = p.pr[ti.q].hint_a, hb = p.pr[ti.q].hint_b;
                 const int m_blk = ti.m_blk, n_blk = ti.n_blk;
-                const int b_outer = (p.grouped == 1) ? ti.grp * p.b_group_rows : 0;
+                const int b_outer = (Op::GROUPED && p.grouped == 1) ? ti.grp * p.b_group_rows : 0;
                 for (int kb = ti.kb0; kb < ti.kb1; ++kb) {
                     mbar_wait(&empty_bar[stage], phase ^ 1, 1);
                     uint8_t* sa = smem_a + stage * A_STAGE_BYTES;
                     uint8_t* sb = smem_b + stage * B_STAGE_BYTES;
                     mbar_expect_tx(&full_bar[stage], STAGE_BYTES);
                     if (!A_MN) {
-                        tma_load_2d_hint(sa, tmap_a, &full_bar[stage], kb * BK, m_blk * BM, ha);
+                        tma_load_2d_hint(sa, tmap_a, &full_bar[stage], kb * Op::KB_ELEMS, m_blk * BM, ha);
                     } else {
 #pragma unroll
                         for (int i = 0; i < BM / 64; ++i)
                             tma_load_2d_hint(sa + i * (BK * 128), tmap_a, &full_bar[stage], m_blk * BM + i * 64, kb * BK, ha);
                     }
                     if (!B_MN) {
-                        tma_load_2d_hint(sb, tmap_b, &full_bar[stage], kb * BK, b_outer + n_blk * TN, hb);
+                        tma_load_2d_hint(sb, tmap_b, &full_bar[stage], kb * Op::KB_ELEMS, b_outer + n_blk * TN, hb);
                     } else {
 #pragma unroll
                         for (int i = 0; i < TN / 64; ++i)
@@ -462,16 +497,17 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     int stage = 0;
     uint32_t phase = 0;
     float acc[TN / 2];
+    float tot[TN / 2];  // SPLIT: the sum of the promoted k-blocks
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        const TileInfo ti = tile_info(t, p);
+        const TileInfo ti = tile_info<Op::GROUPED>(t, p);
         const Problem& pr = p.pr[ti.q];
         const int row0 = ti.m_blk * BM + cw * 64;  // first row of this warpgroup's 64
         const int col0 = ti.n_blk * TN;
-        const int dgrp = p.grouped == 2 ? ti.grp : 0;
+        const int dgrp = Op::GROUPED && p.grouped == 2 ? ti.grp : 0;
         // K-grouped launch (expert weight gradients) and this expert received NO rows: its product is zero.  A launch that
         // OVERWRITES (beta = 0, no C) must still write the tile -- the caller did not clear the buffer.
         if (!ti.valid) {
-            if (p.grouped == 2 && p.d_is_f32 && pr.C == nullptr) epi.store_zero_f32<TN>(&maps.d[ti.q], col0, row0, dgrp);
+            if (Op::GROUPED && p.grouped == 2 && p.d_is_f32 && pr.C == nullptr) epi.store_zero_f32<TN>(&maps.d[ti.q], col0, row0, dgrp);
             continue;
         }
         const bool has_bias = pr.bias != nullptr;
@@ -492,42 +528,77 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
             const uint32_t sa = smem_u32(smem_a + stage * A_STAGE_BYTES);
             const uint32_t sb = smem_u32(smem_b + stage * B_STAGE_BYTES);
 #pragma unroll
-            for (int k = 0; k < BK / 16; ++k) {
-                // K-major: +32 B per K=16 step inside the 128 B swizzle span; SBO = 8 rows x 128 B; this warpgroup's
-                // 64 rows start 64 x 128 B into the tile.
+            for (int k = 0; k < 4; ++k) {
+                // K-major: +32 B per MMA step (K=16 bf16, K=32 fp8) inside the 128 B swizzle span; SBO = 8 rows x 128 B;
+                // this warpgroup's 64 rows start 64 x 128 B into the tile.
                 // MN-major: +16 K-rows x 128 B per step; LBO = next 64-wide MN chunk (BK rows x 128 B), SBO = 8 K-rows;
                 // this warpgroup's 64 rows are the cw-th chunk.
                 const uint64_t adesc = A_MN ? gmma_desc(sa + cw * (BK * 128) + k * 2048, BK * 128, 1024, 1)
                                             : gmma_desc(sa + cw * (64 * 128) + k * 32, 16, 1024, 1);
                 const uint64_t bdesc = B_MN ? gmma_desc(sb + k * 2048, BK * 128, 1024, 1)
                                             : gmma_desc(sb + k * 32, 16, 1024, 1);
-                wgmma_ss<TN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc, bdesc, (kb != ti.kb0 || k != 0) ? 1u : 0u);
+                Op::template mma<TN>(acc, adesc, bdesc, ((!Op::SPLIT && kb != ti.kb0) || k != 0) ? 1u : 0u);
             }
             wgmma_commit();
             // C of the tile's first two chunks: the load overlaps the rest of the mainloop.  Two k-blocks in, the
             // previous tile's last stores have long read their slabs, so the leader does not hold up the MMAs.
             if (kb == min(ti.kb0 + 2, ti.kb1 - 1) && has_c && epi.leader) epi.load_c_prefetch(&maps.c[ti.q], chunk_cols, col0, row0, dgrp);
-            wgmma_wait<1>();  // the previous k-block's MMAs retired: its stage may be refilled
-            if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-            prev_stage = stage;
+            if constexpr (Op::SPLIT) {
+                wgmma_wait<0>();  // this k-block's MMAs retired: its stage may be refilled, its product promoted
+                reg_fence<TN / 2>(acc);
+                if (lane == 0) mbar_arrive(&empty_bar[stage]);
+                if (kb == ti.kb0) {
+#pragma unroll
+                    for (int i = 0; i < TN / 2; ++i) tot[i] = acc[i];
+                } else {
+#pragma unroll
+                    for (int i = 0; i < TN / 2; ++i) tot[i] += acc[i];
+                }
+            } else {
+                wgmma_wait<1>();  // the previous k-block's MMAs retired: its stage may be refilled
+                if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+                prev_stage = stage;
+            }
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
-        wgmma_wait<0>();
-        reg_fence<TN / 2>(acc);
-        if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+        if constexpr (!Op::SPLIT) {
+            wgmma_wait<0>();
+            reg_fence<TN / 2>(acc);
+            if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+        }
+        const float(&res)[TN / 2] = Op::SPLIT ? tot : acc;
+        float s = 1.f;
+        if constexpr (Op::SCALED) s = __ldg(p.a_scale_inv[ti.q]) * __ldg(p.b_scale_inv[ti.q]);
         // the previous tile's epilogue has finished reading the bias slice: its last chunk ended in a barrier
         if (has_bias && wt < TN / 2) epi.bias[wt] = bias_v;
         epi.begin_tile();
 
         // ---------------- epilogue: registers -> shared-memory slabs -> TMA ----------------
         if (p.d_is_f32)
-            epi.store<TN, true>(acc, &maps.d[ti.q], &maps.c[ti.q], col0, row0, dgrp, pr.alpha, pr.beta, has_bias, has_c,
-                                p.grouped == 3);
+            epi.store<TN, true, Op::SCALED>(res, &maps.d[ti.q], &maps.c[ti.q], col0, row0, dgrp, s, pr.alpha, pr.beta,
+                                            has_bias, has_c, Op::GROUPED && p.grouped == 3);
         else
-            epi.store<TN, false>(acc, &maps.d[ti.q], &maps.c[ti.q], col0, row0, dgrp, pr.alpha, pr.beta, has_bias, has_c,
-                                 false);
+            epi.store<TN, false, Op::SCALED>(res, &maps.d[ti.q], &maps.c[ti.q], col0, row0, dgrp, s, pr.alpha, pr.beta,
+                                             has_bias, has_c, false);
     }
     if (epi.leader) tma_store_wait_all<0>();  // the slabs must outlive the stores that read them
+}
+
+template <bool A_MN, bool B_MN, int TN>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+    gemm_bf16_kernel(const __grid_constant__ GemmMaps maps, const __grid_constant__ GemmParams p) {
+    gemm_body<Bf16Ops<A_MN, B_MN>, TN>(maps, p);
+}
+
+// FP8 GEMM (TransformerEngine te.Linear under fp8_autocast): A [M, K] and B [N, K] are both row-major (the transposes come
+// from the cast kernel), 128 x 128 tiles.
+//   D = alpha * (scale_inv_a * scale_inv_b * acc + bias) + beta * C
+// SPLIT: split accumulation (dgrad / wgrad); otherwise the MMA accumulates over the whole contraction (fprop, TE's fast
+// accumulation).
+template <int FA, int FB, bool SPLIT>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+    gemm_fp8_kernel(const __grid_constant__ GemmMaps maps, const __grid_constant__ GemmParams p) {
+    gemm_body<Fp8Ops<FA, FB, SPLIT>, 128>(maps, p);
 }
 
 // SMs of the static persistent schedule: worker w takes tiles w, w + W, ... on `SMs - gemm_sm_margin` SMs
@@ -536,19 +607,18 @@ int gemm_workers() {
     return sms < 1 ? 1 : sms;
 }
 
-template <bool A_MN, bool B_MN, int TN>
+template <int TN, void (*KERNEL)(GemmMaps, GemmParams)>
 int launch_gemm(const GemmMaps& maps, const GemmParams& p, cudaStream_t st) {
-    auto kern = gemm_bf16_kernel<A_MN, B_MN, TN>;
     constexpr int smem_bytes = Ring<TN>::SMEM_BYTES;
     static bool attr_set = false;  // per instantiation
     if (!attr_set) {
-        DOLO_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+        DOLO_CUDA_OK(cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
         attr_set = true;
     }
     const int sms = gemm_workers();
     const int grid = p.num_tiles < sms ? p.num_tiles : sms;
-    kern<<<grid, GEMM_THREADS, smem_bytes, st>>>(maps, p);
-    DOLO_LAUNCH_OK("gemm_bf16");
+    KERNEL<<<grid, GEMM_THREADS, smem_bytes, st>>>(maps, p);
+    DOLO_LAUNCH_OK("gemm");
     return DOLO_OK;
 }
 
@@ -570,194 +640,6 @@ int choose_tile_n(int n, const int64_t* M, const int64_t* N) {
     const double c128 = double((t128 + w - 1) / w);
     const double c256 = double((t256 + w - 1) / w) * TILE256_COST;
     return c256 < c128 ? 256 : 128;
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// FP8 GEMM (TransformerEngine te.Linear under fp8_autocast): the same persistent schedule, stage ring and epilogue as the
-// bf16 kernel, with a k-block of 128 fp8 elements (still one 128-byte swizzle span, so a stage is still 32 KB).  fp8 wgmma
-// takes K-major operands only: A [M, K] and B [N, K] are both row-major, the transposes come from the cast kernel.
-//   D = alpha * (scale_inv_a * scale_inv_b * acc + bias) + beta * C
-// SPLIT: the wgmma accumulator is promoted into a second fp32 register set once per k-block (TE's "split accumulator",
-// used for dgrad / wgrad); otherwise the MMA accumulates over the whole contraction (fprop, TE's fast accumulation).
-// ---------------------------------------------------------------------------------------------------------------------
-constexpr int BK8 = 128;  // 128 fp8 = 128 bytes = one swizzle span
-static_assert(BM * BK8 == A_STAGE_BYTES && BN * BK8 == B_STAGE_BYTES, "fp8 stage must match the bf16 stage size");
-
-struct Fp8Scales {
-    const float* a[MAXP];  // scale_inv of A (device scalar)
-    const float* b[MAXP];
-};
-
-template <int FA, int FB, bool SPLIT>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-    gemm_fp8_kernel(const __grid_constant__ GemmMaps maps, const __grid_constant__ GemmParams p,
-                    const __grid_constant__ Fp8Scales sc) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_align_1024(smem_raw);
-    uint8_t* smem_a = smem;
-    uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
-    uint64_t* full_bar = bars;
-    uint64_t* empty_bar = bars + STAGES;
-
-    const int wg = threadIdx.x >> 7;
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-    const int num_tiles = p.num_tiles;
-
-    if (threadIdx.x == 0) {
-        for (int q = 0; q < p.n_prob; ++q) {
-            tma_prefetch_desc(&maps.a[q]);
-            tma_prefetch_desc(&maps.b[q]);
-        }
-        for (int i = 0; i < STAGES; ++i) {
-            mbar_init(&full_bar[i], 1);
-            mbar_init(&empty_bar[i], 8);
-        }
-        mbar_fence_init();
-    }
-    __syncthreads();
-
-    if (wg == 0) {
-        if (warp == 0 && elect_one()) {
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-                const TileInfo ti = tile_info(t, p);
-                for (int kb = ti.kb0; kb < ti.kb1; ++kb) {
-                    mbar_wait(&empty_bar[stage], phase ^ 1, 1);
-                    mbar_expect_tx(&full_bar[stage], STAGE_BYTES);
-                    tma_load_2d(smem_a + stage * A_STAGE_BYTES, &maps.a[ti.q], &full_bar[stage], kb * BK8, ti.m_blk * BM);
-                    tma_load_2d(smem_b + stage * B_STAGE_BYTES, &maps.b[ti.q], &full_bar[stage], kb * BK8, ti.n_blk * BN);
-                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                }
-            }
-        }
-        return;
-    }
-
-    const int cw = wg - 1;
-    const int wr = (warp & 3) * 16 + (lane >> 2);
-    const int wc = 2 * (lane & 3);
-    int stage = 0;
-    uint32_t phase = 0;
-    float acc[BN / 2];
-    float tot[SPLIT ? BN / 2 : 1];
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        const TileInfo ti = tile_info(t, p);
-        const Problem& pr = p.pr[ti.q];
-        const int64_t row0 = int64_t(ti.m_blk) * BM + cw * 64 + wr;
-        const int col0 = ti.n_blk * BN + wc;
-        int prev_stage = -1;
-        for (int kb = ti.kb0; kb < ti.kb1; ++kb) {
-            mbar_wait(&full_bar[stage], phase, 3);
-            wgmma_fence();
-            const uint32_t sa = smem_u32(smem_a + stage * A_STAGE_BYTES);
-            const uint32_t sb = smem_u32(smem_b + stage * B_STAGE_BYTES);
-#pragma unroll
-            for (int k = 0; k < BK8 / 32; ++k) {
-                // K-major, +32 B per K=32 step inside the swizzle span (the byte layout of the bf16 K=16 step)
-                const uint64_t adesc = gmma_desc(sa + cw * (64 * 128) + k * 32, 16, 1024, 1);
-                const uint64_t bdesc = gmma_desc(sb + k * 32, 16, 1024, 1);
-                const bool acc_on = SPLIT ? k != 0 : (kb != ti.kb0 || k != 0);
-                wgmma_fp8_n128<FA, FB>(acc, adesc, bdesc, acc_on ? 1u : 0u);
-            }
-            wgmma_commit();
-            if constexpr (SPLIT) {
-                wgmma_wait<0>();
-                reg_fence<BN / 2>(acc);
-                if (lane == 0) mbar_arrive(&empty_bar[stage]);
-                if (kb == ti.kb0) {
-#pragma unroll
-                    for (int i = 0; i < BN / 2; ++i) tot[i] = acc[i];
-                } else {
-#pragma unroll
-                    for (int i = 0; i < BN / 2; ++i) tot[i] += acc[i];
-                }
-            } else {
-                wgmma_wait<1>();
-                if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-                prev_stage = stage;
-            }
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        if constexpr (!SPLIT) {
-            wgmma_wait<0>();
-            reg_fence<BN / 2>(acc);
-            if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-        }
-        const float* res = SPLIT ? tot : acc;
-
-        const float s = __ldg(sc.a[ti.q]) * __ldg(sc.b[ti.q]);
-        const float alpha = pr.alpha, beta = pr.beta;
-        const __nv_bfloat16* bias = pr.bias;
-        const int N = pr.N;
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-            const int col = col0 + 8 * j;
-            if (col >= N) continue;
-            float b0 = 0.f, b1 = 0.f;
-            if (bias != nullptr) {
-                const uint32_t bv = *reinterpret_cast<const uint32_t*>(bias + col);
-                b0 = bf16_lo(bv);
-                b1 = bf16_hi(bv);
-            }
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int64_t row = row0 + 8 * h;
-                if (row >= pr.M) continue;
-                float v0 = (s * res[4 * j + 2 * h] + b0) * alpha;
-                float v1 = (s * res[4 * j + 2 * h + 1] + b1) * alpha;
-                if (p.d_is_f32) {
-                    float* d = static_cast<float*>(pr.D) + row * pr.ldd + col;
-                    if (pr.C) {
-                        const float2 c2 = *reinterpret_cast<const float2*>(static_cast<const float*>(pr.C) + row * pr.ldc + col);
-                        v0 += beta * c2.x;
-                        v1 += beta * c2.y;
-                    }
-                    *reinterpret_cast<float2*>(d) = make_float2(v0, v1);
-                } else {
-                    __nv_bfloat16* d = static_cast<__nv_bfloat16*>(pr.D) + row * pr.ldd + col;
-                    if (pr.C) {
-                        const uint32_t cv =
-                            *reinterpret_cast<const uint32_t*>(static_cast<const __nv_bfloat16*>(pr.C) + row * pr.ldc + col);
-                        v0 += beta * bf16_lo(cv);
-                        v1 += beta * bf16_hi(cv);
-                    }
-                    *reinterpret_cast<uint32_t*>(d) = pack_bf16(v0, v1);
-                }
-            }
-        }
-    }
-}
-
-template <int FA, int FB, bool SPLIT>
-int launch_gemm_fp8(const GemmMaps& maps, const GemmParams& p, const Fp8Scales& sc, cudaStream_t st) {
-    auto kern = gemm_fp8_kernel<FA, FB, SPLIT>;
-    static bool attr_set = false;
-    if (!attr_set) {
-        DOLO_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-        attr_set = true;
-    }
-    int sms = dolo_num_sms() - dolo_option_gemm_sm_margin();
-    if (sms < 1) sms = 1;
-    const int grid = p.num_tiles < sms ? p.num_tiles : sms;
-    kern<<<grid, GEMM_THREADS, SMEM_BYTES, st>>>(maps, p, sc);
-    DOLO_LAUNCH_OK("gemm_fp8");
-    return DOLO_OK;
-}
-
-template <int FA, int FB>
-int dispatch_fp8_split(int split, const GemmMaps& maps, const GemmParams& p, const Fp8Scales& sc, cudaStream_t st) {
-    return split ? launch_gemm_fp8<FA, FB, true>(maps, p, sc, st) : launch_gemm_fp8<FA, FB, false>(maps, p, sc, st);
-}
-
-int dispatch_fp8(int a_fmt, int b_fmt, int split, const GemmMaps& maps, const GemmParams& p, const Fp8Scales& sc,
-                 cudaStream_t st) {
-    if (a_fmt == 0 && b_fmt == 0) return dispatch_fp8_split<0, 0>(split, maps, p, sc, st);
-    if (a_fmt == 0 && b_fmt == 1) return dispatch_fp8_split<0, 1>(split, maps, p, sc, st);
-    if (a_fmt == 1 && b_fmt == 0) return dispatch_fp8_split<1, 0>(split, maps, p, sc, st);
-    return dispatch_fp8_split<1, 1>(split, maps, p, sc, st);
 }
 
 }  // namespace
@@ -783,20 +665,34 @@ struct GemmProblemArgs {
     const void* bias;
     float alpha, beta;
     int64_t M, N, K;
+    const float* a_scale_inv = nullptr;  // fp8 operands: their scale_inv (device scalars)
+    const float* b_scale_inv = nullptr;
 };
 
-// Fills maps.{a,b}[q] and p.pr[q] for one problem.  All problems of a launch share the operand layouts, the output type
-// and the tile width tile_n (128 or 256).
-static int setup_problem(GemmMaps& maps, GemmParams& p, int q, const GemmProblemArgs& g, int a_mn_major, int b_mn_major,
-                         int d_is_f32, const GroupArgs& ga, int tile_n) {
+// Fills maps.{a,b}[q] and p.pr[q] for one problem.  All problems of a launch share the operand type (ab: bytes per
+// element of A and B, 2 = bf16, 1 = fp8), the operand layouts, the output type and the tile width tile_n (128 or 256).
+static int setup_problem(GemmMaps& maps, GemmParams& p, int q, const GemmProblemArgs& g, int ab, int a_mn_major,
+                         int b_mn_major, int d_is_f32, const GroupArgs& ga, int tile_n) {
     const int64_t M = g.M, N = g.N, K = g.K;
+    if (ab == 1) {
+        // fp8: K-major operands; N % 16 == 0 keeps every row of D a whole number of 16-byte segments
+        DOLO_REQUIRE(M > 0 && N > 0 && K > 0, "gemm_fp8: empty problem (M=%lld N=%lld K=%lld)", (long long)M,
+                     (long long)N, (long long)K);
+        DOLO_REQUIRE(K % 16 == 0 && N % 16 == 0, "gemm_fp8: K=%lld and N=%lld must be multiples of 16", (long long)K,
+                     (long long)N);
+        DOLO_REQUIRE(g.lda % 16 == 0 && g.ldb % 16 == 0 && g.lda >= K && g.ldb >= K,
+                     "gemm_fp8: lda / ldb must be >= K and multiples of 16 (16-byte aligned fp8 rows)");
+        DOLO_REQUIRE(g.a_scale_inv != nullptr && g.b_scale_inv != nullptr, "gemm_fp8: missing scale_inv pointer");
+        p.a_scale_inv[q] = g.a_scale_inv;
+        p.b_scale_inv[q] = g.b_scale_inv;
+    }
     // M, N and K may take any value: the tensor maps carry the exact extents, so TMA zero-fills the operand tails of the
     // last k-block and tile and clips the D rows and columns.  Only the row strides and the base addresses (checked when
     // the tensor maps are made) need 16-byte alignment.  A TMA store writes whole 16-byte segments: when a row of D ends
     // inside one (N not a multiple of 16 bytes), the rest of that segment, columns [N, round_up(N, 16 bytes)), receives
     // zeros, so ldd must cover it.
     DOLO_REQUIRE(K > 0, "gemm: K must be > 0");
-    DOLO_REQUIRE(g.lda % 8 == 0 && g.ldb % 8 == 0 && g.ldd % (d_is_f32 ? 4 : 8) == 0,
+    DOLO_REQUIRE(g.lda * ab % 16 == 0 && g.ldb * ab % 16 == 0 && g.ldd % (d_is_f32 ? 4 : 8) == 0,
                  "gemm: leading dimensions must keep 16-byte alignment");
     {
         const int64_t per = d_is_f32 ? 4 : 8;
@@ -807,7 +703,8 @@ static int setup_problem(GemmMaps& maps, GemmParams& p, int q, const GemmProblem
     DOLO_REQUIRE(g.C == nullptr || g.ldc % (d_is_f32 ? 4 : 8) == 0, "gemm: ldc alignment");
     DOLO_REQUIRE((reinterpret_cast<uintptr_t>(g.bias) & 3) == 0, "gemm: bias must be 4-byte aligned");
     DOLO_REQUIRE(M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31), "gemm: dimension too large");
-    // K-major: dims {K, rows}, box {64, tile rows} (128 for A, tile_n for B).  MN-major: dims {rows, K}, box {64, 64}.
+    // K-major: dims {K, rows}, box {one 128-byte k-block, tile rows} (128 for A, tile_n for B).  MN-major (bf16): dims
+    // {rows, K}, box {64, 64}.
     uint64_t dims[2], strides[2];
     uint32_t box[2];
     int rc;
@@ -822,24 +719,24 @@ static int setup_problem(GemmMaps& maps, GemmParams& p, int q, const GemmProblem
         p.gather_k = int(K);
     } else {
         if (!a_mn_major) {
-            dims[0] = uint64_t(K); dims[1] = uint64_t(M); strides[0] = 2; strides[1] = uint64_t(g.lda) * 2;
-            box[0] = BK; box[1] = BM;
+            dims[0] = uint64_t(K); dims[1] = uint64_t(M); strides[0] = ab; strides[1] = uint64_t(g.lda) * ab;
+            box[0] = 128 / ab; box[1] = BM;
         } else {
             dims[0] = uint64_t(M); dims[1] = uint64_t(K); strides[0] = 2; strides[1] = uint64_t(g.lda) * 2;
             box[0] = 64; box[1] = BK;
         }
-        rc = dolo_make_tmap(&maps.a[q], g.A, 2, 2, dims, strides, box, DOLO_SW_128);
+        rc = dolo_make_tmap(&maps.a[q], g.A, ab, 2, dims, strides, box, DOLO_SW_128);
         if (rc) return rc;
     }
-    strides[0] = 2;
+    strides[0] = ab;
     if (!b_mn_major) {
-        dims[0] = uint64_t(K); dims[1] = uint64_t(ga.mode == 1 ? ga.b_total_outer : N); strides[1] = uint64_t(g.ldb) * 2;
-        box[0] = BK; box[1] = uint32_t(tile_n);
+        dims[0] = uint64_t(K); dims[1] = uint64_t(ga.mode == 1 ? ga.b_total_outer : N); strides[1] = uint64_t(g.ldb) * ab;
+        box[0] = 128 / ab; box[1] = uint32_t(tile_n);
     } else {
         dims[0] = uint64_t(N); dims[1] = uint64_t(ga.mode == 1 ? ga.b_total_outer : K); strides[1] = uint64_t(g.ldb) * 2;
         box[0] = 64; box[1] = BK;
     }
-    rc = dolo_make_tmap(&maps.b[q], g.B, 2, 2, dims, strides, box, DOLO_SW_128);
+    rc = dolo_make_tmap(&maps.b[q], g.B, ab, 2, dims, strides, box, DOLO_SW_128);
     if (rc) return rc;
     {
         // D and C: dims {N, M, groups}, box = one epilogue slab {128 B of columns, 64 rows, 1}
@@ -870,7 +767,7 @@ static int setup_problem(GemmMaps& maps, GemmParams& p, int q, const GemmProblem
     pr.alpha = g.alpha;
     pr.beta = g.C ? g.beta : 0.f;
     pr.hint_a = pr.hint_b = TMA_HINT_NORMAL;
-    if (dolo_option_gemm_l2_hints() && ga.mode == 0 && K >= 4096 && (M + N) * K * 2 > (24ll << 20)) {
+    if (ab == 2 && dolo_option_gemm_l2_hints() && ga.mode == 0 && K >= 4096 && (M + N) * K * 2 > (24ll << 20)) {
         // long contraction, operands larger than what the L2 keeps anyway: stream the bigger one, keep the smaller one
         const bool a_smaller = M <= N;
         pr.hint_a = a_smaller ? TMA_HINT_EVICT_LAST : TMA_HINT_EVICT_FIRST;
@@ -878,10 +775,10 @@ static int setup_problem(GemmMaps& maps, GemmParams& p, int q, const GemmProblem
     }
     pr.num_m = int((M + BM - 1) / BM);
     pr.num_n = int((N + tile_n - 1) / tile_n);
-    pr.num_kb = int((K + BK - 1) / BK);
+    pr.num_kb = int((K * ab + 127) / 128);  // 128-byte k-blocks
     {
-        // A panel of group_m x 128 rows x K bf16 should fit comfortably in the 50 MB L2 next to the streaming B tiles
-        const int64_t panel_bytes = int64_t(BM) * K * 2;
+        // A panel of group_m x 128 rows x K should fit comfortably in the 50 MB L2 next to the streaming B tiles
+        const int64_t panel_bytes = int64_t(BM) * K * ab;
         int64_t gm = (12ll << 20) / (panel_bytes > 0 ? panel_bytes : 1);
         if (gm < 4) gm = 4;
         if (gm > 64) gm = 64;
@@ -892,15 +789,28 @@ static int setup_problem(GemmMaps& maps, GemmParams& p, int q, const GemmProblem
 
 template <int TN>
 static int dispatch_layout(int a_mn_major, int b_mn_major, const GemmMaps& maps, const GemmParams& p, cudaStream_t st) {
-    if (!a_mn_major && !b_mn_major) return launch_gemm<false, false, TN>(maps, p, st);
-    if (!a_mn_major && b_mn_major) return launch_gemm<false, true, TN>(maps, p, st);
-    if (a_mn_major && !b_mn_major) return launch_gemm<true, false, TN>(maps, p, st);
-    return launch_gemm<true, true, TN>(maps, p, st);
+    if (!a_mn_major && !b_mn_major) return launch_gemm<TN, gemm_bf16_kernel<false, false, TN>>(maps, p, st);
+    if (!a_mn_major && b_mn_major) return launch_gemm<TN, gemm_bf16_kernel<false, true, TN>>(maps, p, st);
+    if (a_mn_major && !b_mn_major) return launch_gemm<TN, gemm_bf16_kernel<true, false, TN>>(maps, p, st);
+    return launch_gemm<TN, gemm_bf16_kernel<true, true, TN>>(maps, p, st);
 }
 
 static int dispatch(int tile_n, int a_mn_major, int b_mn_major, const GemmMaps& maps, const GemmParams& p, cudaStream_t st) {
     return tile_n == 256 ? dispatch_layout<256>(a_mn_major, b_mn_major, maps, p, st)
                          : dispatch_layout<128>(a_mn_major, b_mn_major, maps, p, st);
+}
+
+template <int FA, int FB>
+static int dispatch_fp8_split(int split, const GemmMaps& maps, const GemmParams& p, cudaStream_t st) {
+    return split ? launch_gemm<BN, gemm_fp8_kernel<FA, FB, true>>(maps, p, st)
+                 : launch_gemm<BN, gemm_fp8_kernel<FA, FB, false>>(maps, p, st);
+}
+
+static int dispatch_fp8(int a_fmt, int b_fmt, int split, const GemmMaps& maps, const GemmParams& p, cudaStream_t st) {
+    if (a_fmt == 0 && b_fmt == 0) return dispatch_fp8_split<0, 0>(split, maps, p, st);
+    if (a_fmt == 0 && b_fmt == 1) return dispatch_fp8_split<0, 1>(split, maps, p, st);
+    if (a_fmt == 1 && b_fmt == 0) return dispatch_fp8_split<1, 0>(split, maps, p, st);
+    return dispatch_fp8_split<1, 1>(split, maps, p, st);
 }
 
 static int gemm_impl(const void* A, int64_t lda, int a_mn_major, const void* B, int64_t ldb, int b_mn_major, void* D,
@@ -915,7 +825,7 @@ static int gemm_impl(const void* A, int64_t lda, int a_mn_major, const void* B, 
     GemmParams p;
     memset(&p, 0, sizeof(p));
     GemmProblemArgs g{A, lda, B, ldb, D, ldd, C, ldc, bias, alpha, beta, M, N, K};
-    int rc = setup_problem(maps, p, 0, g, a_mn_major, b_mn_major, d_is_f32, ga, tile_n);
+    int rc = setup_problem(maps, p, 0, g, 2, a_mn_major, b_mn_major, d_is_f32, ga, tile_n);
     if (rc) return rc;
     p.n_prob = 1;
     p.pr[0].tile_start = 0;
@@ -948,7 +858,7 @@ extern "C" int dolomite_b200_gemm_bf16_wgrad_multi(int n_problems, const void* c
     for (int q = 0; q < n_problems; ++q) {
         GemmProblemArgs g{dY[q], ld_dy[q], X[q], ld_x[q], dW[q], ld_dw[q], accumulate[q] ? dW[q] : nullptr, ld_dw[q], nullptr,
                           alpha[q], 1.f, M[q], N[q], K};
-        int rc = setup_problem(maps, p, q, g, 1, 1, 1, GroupArgs(), tile_n);
+        int rc = setup_problem(maps, p, q, g, 2, 1, 1, 1, GroupArgs(), tile_n);
         if (rc) return rc;
         p.pr[q].tile_start = tiles;
         tiles += p.pr[q].num_m * p.pr[q].num_n;
@@ -1057,54 +967,6 @@ extern "C" int dolomite_b200_gemm_bf16_grouped_k(const void* A, int64_t lda, con
 // ---------------------------------------------------------------------------------------------------------------------
 // FP8 entry points (te.Linear fprop / dgrad / wgrad under fp8_autocast)
 // ---------------------------------------------------------------------------------------------------------------------
-static int setup_problem_fp8(GemmMaps& maps, GemmParams& p, Fp8Scales& sc, int q, const GemmProblemArgs& g,
-                             const float* a_scale_inv, const float* b_scale_inv, int d_is_f32) {
-    const int64_t M = g.M, N = g.N, K = g.K;
-    DOLO_REQUIRE(M > 0 && N > 0 && K > 0, "gemm_fp8: empty problem (M=%lld N=%lld K=%lld)", (long long)M, (long long)N,
-                 (long long)K);
-    DOLO_REQUIRE(K % 16 == 0 && N % 16 == 0, "gemm_fp8: K=%lld and N=%lld must be multiples of 16", (long long)K,
-                 (long long)N);
-    DOLO_REQUIRE(g.lda % 16 == 0 && g.ldb % 16 == 0 && g.lda >= K && g.ldb >= K,
-                 "gemm_fp8: lda / ldb must be >= K and multiples of 16 (16-byte aligned fp8 rows)");
-    DOLO_REQUIRE(g.ldd % (d_is_f32 ? 4 : 8) == 0 && g.ldd >= N && (g.C == nullptr || g.ldc % (d_is_f32 ? 4 : 8) == 0),
-                 "gemm_fp8: ldd / ldc must keep 16-byte alignment");
-    const uintptr_t ptr_bits = reinterpret_cast<uintptr_t>(g.A) | reinterpret_cast<uintptr_t>(g.B) |
-                               reinterpret_cast<uintptr_t>(g.D) | reinterpret_cast<uintptr_t>(g.C);
-    DOLO_REQUIRE((ptr_bits & 15) == 0 && (reinterpret_cast<uintptr_t>(g.bias) & 3) == 0,
-                 "gemm_fp8: A, B, D and C must be 16-byte aligned");
-    DOLO_REQUIRE(a_scale_inv != nullptr && b_scale_inv != nullptr, "gemm_fp8: missing scale_inv pointer");
-    DOLO_REQUIRE(M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31), "gemm_fp8: dimension too large");
-    uint64_t dims[2] = {uint64_t(K), uint64_t(M)};
-    uint64_t strides[2] = {1, uint64_t(g.lda)};
-    uint32_t box[2] = {BK8, BM};
-    int rc = dolo_make_tmap(&maps.a[q], g.A, 1, 2, dims, strides, box, DOLO_SW_128);
-    if (rc) return rc;
-    dims[1] = uint64_t(N);
-    strides[1] = uint64_t(g.ldb);
-    box[1] = BN;
-    rc = dolo_make_tmap(&maps.b[q], g.B, 1, 2, dims, strides, box, DOLO_SW_128);
-    if (rc) return rc;
-    sc.a[q] = a_scale_inv;
-    sc.b[q] = b_scale_inv;
-    Problem& pr = p.pr[q];
-    pr.D = g.D;
-    pr.C = g.C;
-    pr.bias = static_cast<const __nv_bfloat16*>(g.bias);
-    pr.ldd = g.ldd;
-    pr.ldc = g.ldc;
-    pr.M = int(M);
-    pr.N = int(N);
-    pr.alpha = g.alpha;
-    pr.beta = g.C ? g.beta : 0.f;
-    pr.hint_a = pr.hint_b = TMA_HINT_NORMAL;
-    pr.num_m = int((M + BM - 1) / BM);
-    pr.num_n = int((N + BN - 1) / BN);
-    pr.num_kb = int((K + BK8 - 1) / BK8);
-    int64_t gm = (12ll << 20) / (int64_t(BM) * K);  // A panel of ~12 MB of the 50 MB L2, as for bf16
-    pr.group_m = int(gm < 4 ? 4 : (gm > 64 ? 64 : gm));
-    return DOLO_OK;
-}
-
 extern "C" int dolomite_b200_gemm_fp8(const void* A, int64_t lda, int a_fmt, const void* B, int64_t ldb, int b_fmt,
                                       const float* a_scale_inv, const float* b_scale_inv, void* D, int64_t ldd,
                                       int d_is_f32, const void* C, int64_t ldc, float alpha, float beta, const void* bias,
@@ -1114,17 +976,15 @@ extern "C" int dolomite_b200_gemm_fp8(const void* A, int64_t lda, int a_fmt, con
     if (M == 0 || N == 0) return DOLO_OK;
     GemmMaps maps;
     GemmParams p;
-    Fp8Scales sc;
     memset(&p, 0, sizeof(p));
-    memset(&sc, 0, sizeof(sc));
-    GemmProblemArgs g{A, lda, B, ldb, D, ldd, C, ldc, bias, alpha, beta, M, N, K};
-    int rc = setup_problem_fp8(maps, p, sc, 0, g, a_scale_inv, b_scale_inv, d_is_f32);
+    GemmProblemArgs g{A, lda, B, ldb, D, ldd, C, ldc, bias, alpha, beta, M, N, K, a_scale_inv, b_scale_inv};
+    int rc = setup_problem(maps, p, 0, g, 1, 0, 0, d_is_f32, GroupArgs(), BN);
     if (rc) return rc;
     p.n_prob = 1;
     p.num_tiles = p.pr[0].num_m * p.pr[0].num_n;
     p.d_is_f32 = d_is_f32;
     p.num_groups = 1;
-    return dispatch_fp8(a_fmt, b_fmt, split_accumulate, maps, p, sc, static_cast<cudaStream_t>(stream));
+    return dispatch_fp8(a_fmt, b_fmt, split_accumulate, maps, p, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int dolomite_b200_gemm_fp8_wgrad_multi(int n_problems, const void* const* dYt, const int64_t* ld_dyt,
@@ -1138,14 +998,12 @@ extern "C" int dolomite_b200_gemm_fp8_wgrad_multi(int n_problems, const void* co
                  "gemm_fp8_wgrad_multi: format must be 0 (e4m3) or 1 (e5m2)");
     GemmMaps maps;
     GemmParams p;
-    Fp8Scales sc;
     memset(&p, 0, sizeof(p));
-    memset(&sc, 0, sizeof(sc));
     int tiles = 0;
     for (int q = 0; q < n_problems; ++q) {
         GemmProblemArgs g{dYt[q], ld_dyt[q], Xt[q], ld_xt[q], dW[q], ld_dw[q], accumulate[q] ? dW[q] : nullptr, ld_dw[q],
-                          nullptr, alpha[q], 1.f, M[q], N[q], K};
-        int rc = setup_problem_fp8(maps, p, sc, q, g, dy_scale_inv[q], x_scale_inv[q], 1);
+                          nullptr, alpha[q], 1.f, M[q], N[q], K, dy_scale_inv[q], x_scale_inv[q]};
+        int rc = setup_problem(maps, p, q, g, 1, 0, 0, 1, GroupArgs(), BN);
         if (rc) return rc;
         p.pr[q].tile_start = tiles;
         tiles += p.pr[q].num_m * p.pr[q].num_n;
@@ -1154,5 +1012,5 @@ extern "C" int dolomite_b200_gemm_fp8_wgrad_multi(int n_problems, const void* co
     p.num_tiles = tiles;
     p.d_is_f32 = 1;
     p.num_groups = 1;
-    return dispatch_fp8(dy_fmt, x_fmt, split_accumulate, maps, p, sc, static_cast<cudaStream_t>(stream));
+    return dispatch_fp8(dy_fmt, x_fmt, split_accumulate, maps, p, static_cast<cudaStream_t>(stream));
 }

@@ -1,4 +1,4 @@
-"""CPU: what the compiler made of the bf16 GEMM kernel (sm_90a SASS of the built library; no GPU needed)."""
+"""CPU: what the compiler made of the bf16 and fp8 GEMM kernels (sm_90a SASS of the built library; no GPU needed)."""
 
 import re
 import shutil
@@ -30,6 +30,18 @@ def test_gemm_kernels_do_not_spill(lib_path):
     no stack frame, no local memory"""
     res = subprocess.run(["cuobjdump", "-res-usage", lib_path], capture_output=True, text=True).stdout
     found = re.findall(r"Function (\S*gemm_bf16_kernel\S*):\s*\n\s*(REG:.*)", res)
+    assert len(found) == 8, [f[0] for f in found]
+    for name, usage in found:
+        stack = int(re.search(r"STACK:(\d+)", usage).group(1))
+        local = int(re.search(r"LOCAL:(\d+)", usage).group(1))
+        assert stack == 0 and local == 0, (name, usage)
+
+
+def test_fp8_gemm_kernels_do_not_spill(lib_path):
+    """every gemm_fp8_kernel instantiation (four format pairs x split accumulation on / off) keeps its accumulators (and
+    the split accumulator's second register set) in registers: no stack frame, no local memory"""
+    res = subprocess.run(["cuobjdump", "-res-usage", lib_path], capture_output=True, text=True).stdout
+    found = re.findall(r"Function (\S*gemm_fp8_kernel\S*):\s*\n\s*(REG:.*)", res)
     assert len(found) == 8, [f[0] for f in found]
     for name, usage in found:
         stack = int(re.search(r"STACK:(\d+)", usage).group(1))

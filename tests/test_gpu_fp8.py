@@ -166,6 +166,63 @@ def test_gemm_wgrad_multi_matches_single(K):
         assert rel_l2(dw, ref) <= FP8_MMA_BOUND
 
 
+def _int_operand(rows, cols, fmt, g, lim=3):
+    """integers in [-lim, lim] (exact in e4m3 and e5m2 for lim <= 8) as fp8 bits, and their values"""
+    v = torch.randint(-lim, lim + 1, (rows, cols), generator=g).double()
+    return quantize_ref(v, 1.0, fmt), v
+
+
+def _halves(shape, g, lim=8):
+    """small multiples of 1/2, exact in bf16"""
+    return torch.randint(-2 * lim, 2 * lim + 1, shape, generator=g).double() / 2
+
+
+@pytest.mark.parametrize("fa,fb", [(E4M3, E4M3), (E5M2, E4M3), (E4M3, E5M2), (E5M2, E5M2)])
+@pytest.mark.parametrize("split", [True, False])
+def test_gemm_exact_arithmetic(K, fa, fb, split):
+    """Operands whose every partial sum is an integer below 2^11 (|a|, |b| <= 3, K = 208), power-of-two scales, alpha and
+    beta, bias and C small multiples of 1/2: every fp32 step of the pipeline is exact, so D equals the fp64 reference
+    rounded once to D's type, bit for bit -- every row, column, bias element and C tile in place, the M and N tails
+    included (M = 200, N = 272 on 128 x 128 tiles)."""
+    M, N, Kd = 200, 272, 208
+    g = torch.Generator().manual_seed(7 + 2 * fa + fb)
+    qa, va = _int_operand(M, Kd, fa, g)
+    qb, vb = _int_operand(N, Kd, fb, g)
+    sa, sb = 4.0, 0.5
+    prod = (va @ vb.t()) * sa * sb
+    A, B, SA, SB = qa.cuda(), qb.cuda(), _dev_scalar(sa), _dev_scalar(sb)
+    bias = _halves((N,), g)
+    for dt in (torch.float32, torch.bfloat16):
+        for with_bias, with_c in ((True, False), (False, True), (True, True)):
+            c = _halves((M, N), g)
+            alpha, beta = (2.0, 0.5) if dt == torch.bfloat16 else (0.5, 2.0)
+            want = (prod + (bias if with_bias else 0.0)) * alpha + (beta * c if with_c else 0.0)
+            d = K.gemm_fp8(A, fa, SA, B, fb, SB, out_dtype=dt, c=c.to(dt).cuda() if with_c else None, alpha=alpha,
+                           beta=beta, bias=bias.to(torch.bfloat16).cuda() if with_bias else None, split_accumulate=split)
+            assert torch.equal(d.cpu(), want.to(dt)), (dt, with_bias, with_c)
+    # the bf16 cases round: some outputs lie above 256, where bf16 does not hold every integer
+    assert (want.abs() > 256).any()
+
+
+@pytest.mark.parametrize("split", [True, False])
+def test_gemm_wgrad_multi_exact_arithmetic(K, split):
+    """one launch of four problems of different sizes, two accumulating into dW and two overwriting it, with the
+    exact-arithmetic operands above (|a|, |b| <= 2 over T = 336 rows): every dW equals its fp64 reference bit for bit"""
+    T = 336
+    g = torch.Generator().manual_seed(11)
+    probs, refs = [], []
+    for q, (M, N) in enumerate([(200, 272), (128, 384), (384, 144), (64, 128)]):
+        qa, va = _int_operand(M, T, E5M2, g, lim=2)
+        qb, vb = _int_operand(N, T, E4M3, g, lim=2)
+        sa, sb, alpha, acc = 2.0 ** -q, 0.5, 2.0 ** (q - 2), q in (1, 2)
+        dw = _halves((M, N), g)
+        refs.append((va @ vb.t()) * sa * sb * alpha + (dw if acc else 0.0))
+        probs.append((qa.cuda(), _dev_scalar(sa), qb.cuda(), _dev_scalar(sb), dw.float().cuda(), alpha, acc))
+    K.gemm_fp8_wgrad_multi(probs, split_accumulate=split)
+    for q, ((_, _, _, _, dw, _, _), ref) in enumerate(zip(probs, refs)):
+        assert torch.equal(dw.cpu(), ref.float()), q
+
+
 def test_gemm_rejects_bad_shapes(K):
     from dolomite_engine_b200._lib import DolomiteB200Error
 
