@@ -561,15 +561,47 @@ def _req_slopes(alibi_slopes, n_heads: int) -> None:
         raise ValueError(f"alibi_slopes must be a contiguous fp32 [{n_heads}] tensor, got {tuple(alibi_slopes.shape)}")
 
 
+def _attn_layout(qkv, n_heads: int, head_dim: int, **rows) -> None:
+    """the layouts the attention kernels address without looking at strides: qkv rows of unit column stride (any row
+    stride), every `rows` tensor (out, dout) a contiguous [T, n_heads * head_dim] tensor; checked before any launch"""
+    if qkv.dim() != 2 or qkv.stride(1) != 1:
+        raise ValueError(f"qkv must be a 2-D tensor with unit column stride, got strides {tuple(qkv.stride())}")
+    T = qkv.shape[0]
+    for name, t in rows.items():
+        if tuple(t.shape) != (T, n_heads * head_dim) or not t.is_contiguous():
+            raise ValueError(f"{name} must be a contiguous [{T}, {n_heads * head_dim}] tensor, got shape "
+                             f"{tuple(t.shape)} strides {tuple(t.stride())}")
+
+
+def _attn_lse_layout(lse, n_heads: int, T: int) -> None:
+    if lse.dtype != torch.float32 or tuple(lse.shape) != (n_heads, T) or not lse.is_contiguous():
+        raise ValueError(f"lse must be a contiguous fp32 [{n_heads}, {T}] tensor, got {lse.dtype} shape "
+                         f"{tuple(lse.shape)} strides {tuple(lse.stride())}")
+
+
+def _attn_dqkv(qkv, dqkv=None):
+    """the dQKV buffer of the backward: the kernels write it with qkv's row stride, so a new one gets qkv's strides and a
+    given one must have them"""
+    if dqkv is None:
+        return torch.empty_strided(qkv.shape, qkv.stride(), dtype=qkv.dtype, device=qkv.device)
+    if dqkv.shape != qkv.shape or dqkv.stride() != qkv.stride():
+        raise ValueError(f"dqkv must have qkv's shape {tuple(qkv.shape)} and strides {tuple(qkv.stride())}, got "
+                         f"{tuple(dqkv.shape)} / {tuple(dqkv.stride())}")
+    return dqkv
+
+
 def attn_varlen_fwd(qkv, cu_seqlens, max_seqlen: int, n_groups: int, q_per_group: int, head_dim: int, scale: float, out=None,
                     dropout_p: float = 0.0, dropout_keys: tuple[int, int] = (0, 0), alibi_slopes=None):
     """`dropout_p` > 0: attention-probability dropout (training mode; attention/padding_free.py:49-59), masks from
     `dropout_keys` (kernels.dropout_keys); the backward call must be given the same p and keys.
     `alibi_slopes` (fp32 [n_heads], alibi.alibi_slopes): ALiBi key bias bf16(slope * index of the key in its document);
     the backward call must be given the same slopes"""
-    _req(qkv, _BF16, "qkv"), _req(cu_seqlens, torch.int32, "cu_seqlens")
-    T = qkv.shape[0]
     nh = n_groups * q_per_group
+    _attn_layout(qkv, nh, head_dim, **({} if out is None else {"out": out}))
+    _req(qkv, _BF16, "qkv"), _req(cu_seqlens, torch.int32, "cu_seqlens")
+    if out is not None:
+        _req(out, _BF16, "out")
+    T = qkv.shape[0]
     o = torch.empty(T, nh * head_dim, dtype=_BF16, device=qkv.device) if out is None else out
     lse = torch.empty(nh, T, dtype=torch.float32, device=qkv.device)
     if alibi_slopes is not None:
@@ -596,10 +628,11 @@ def attn_varlen_fwd(qkv, cu_seqlens, max_seqlen: int, n_groups: int, q_per_group
 
 def attn_varlen_bwd(dout, qkv, out, lse, cu_seqlens, max_seqlen, n_groups, q_per_group, head_dim, scale, dqkv=None,
                     dropout_p: float = 0.0, dropout_keys: tuple[int, int] = (0, 0), alibi_slopes=None):
-    _req(dout, _BF16, "dout"), _req(qkv, _BF16, "qkv")
     T = qkv.shape[0]
-    if dqkv is None:
-        dqkv = torch.empty_like(qkv)
+    _attn_layout(qkv, n_groups * q_per_group, head_dim, dout=dout, out=out)
+    _attn_lse_layout(lse, n_groups * q_per_group, T)
+    dqkv = _attn_dqkv(qkv, dqkv)
+    _req(dout, _BF16, "dout"), _req(qkv, _BF16, "qkv"), _req(out, _BF16, "out"), _req(dqkv, _BF16, "dqkv")
     ws_bytes = _lib.load().dolomite_b200_attn_varlen_bwd_workspace_bytes(T, n_groups, q_per_group, head_dim)
     ws = _workspace(ws_bytes, qkv.device)
     if alibi_slopes is not None:
