@@ -89,6 +89,10 @@ SIGNATURES: dict[str, tuple] = {
     "dolomite_b200_moe_combine_bwd": (_I, [_P, _P, _P, _P, _P, _P, _P, _L, _I, _I, _I, _F, _P]),
     "dolomite_b200_moe_token_sum": (_I, [_P, _P, _P, _L, _I, _I, _P]),
     "dolomite_b200_moe_router_bwd": (_I, [_P, _P, _P, _P, _L, _I, _I, _P]),
+    "dolomite_b200_moe_aux_partial_floats": (_L, [_L, _I]),
+    "dolomite_b200_moe_aux_stats": (_I, [_P, _P, _L, _L, _I, _I, _P, _P, _P]),
+    "dolomite_b200_moe_aux_finalize": (_I, [_P, _I, _L, _F, _P, _P, _P, _P]),
+    "dolomite_b200_moe_router_bwd_aux": (_I, [_P, _P, _P, _P, _P, _P, _P, _L, _L, _I, _I, _P]),
     "dolomite_b200_attn_varlen_fwd": (_I, [_P, _L, _P, _P, _P, _I, _L, _I, _I, _I, _I, _F, _P]),
     "dolomite_b200_attn_decode": (_I, [_P, _L, _P, _P, _P, _P, _I, _L, _I, _I, _I, _F, _P]),
     "dolomite_b200_attn_varlen_bwd_workspace_bytes": (_L, [_L, _I, _I, _I]),
@@ -160,6 +164,7 @@ KERNELS_PER_CALL = {
     "dolomite_b200_attn_varlen_bwd": 3, "dolomite_b200_attn_varlen_fwd_dropout": 1, "dolomite_b200_attn_varlen_bwd_dropout": 3,
     "dolomite_b200_attn_varlen_fwd_alibi": 1, "dolomite_b200_attn_varlen_bwd_alibi": 3, "dolomite_b200_attn_decode_alibi": 1,
     "dolomite_b200_dropout_fwd": 1, "dolomite_b200_dropout_bwd": 1, "dolomite_b200_gemm_bf16_tile_n": 0,
+    "dolomite_b200_moe_aux_stats": 2,
 }
 launch_counts: dict[str, int] = {}
 

@@ -8,6 +8,7 @@
 //   gather     : X_g[row] = x[token(row)] (zero rows for padding) -- operand of the grouped c_fc GEMM
 //   combine    : y[t] = sum_j w[t,j] * Y_g[row(t,j)]            -- after the grouped c_proj GEMM
 //   backward   : dY_g rows / gate-weight grads, token-sum of dX_g rows, softmax-over-k backward to dense dlogits
+//   aux loss   : load-balancing statistics over the layers of a forward, the loss and its dense router gradient
 // The expert GEMMs themselves are the wgmma GEMM in grouped mode (gemm.cu).
 #include "common.cuh"
 #include "../../include/dolomite_b200.h"
@@ -276,6 +277,133 @@ __global__ void moe_router_bwd_kernel(const int32_t* __restrict__ sel_idx, const
     }
 }
 
+// ---- load-balancing loss (transformers' Mixtral load_balancing_loss_func, called by moe_dolomite/base.py:24-43) ----
+// Over the L MoE layers of one forward and the T_real real tokens of each (N = L * T_real):
+//   P_e = sum_{l,t} softmax(logits[l,t])_e,  C_e = #(l, t, slot) selecting e,  aux = E * sum_e C_e P_e / N^2
+// Every sum runs in a fixed order (no float atomics), so the step stays bit-identical run to run.
+constexpr int AUX_TOK_PER_CTA = 64;  // 8 warps x 8 tokens
+
+// fp32 softmax over all E experts of one bf16 logits row; lane holds experts lane + 32 i (0 past E).  The statistics and
+// the backward both call this, so the backward differentiates exactly the probabilities the forward summed.
+__device__ __forceinline__ void row_softmax(const __nv_bfloat16* __restrict__ row, int E, int lane, float (&p)[8]) {
+    float m = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        const int e = lane + i * 32;
+        p[i] = e < E ? __bfloat162float(row[e]) : -INFINITY;
+        m = fmaxf(m, p[i]);
+    }
+    m = warp_max(m);
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        p[i] = lane + i * 32 < E ? expf(p[i] - m) : 0.f;
+        s += p[i];
+    }
+    s = warp_sum(s);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) p[i] /= s;
+}
+
+// one warp per token, 64 tokens per CTA; CTA b writes partial[b] = [P_e of its tokens | C_e of its tokens] ([2, E] fp32)
+__global__ void __launch_bounds__(256) moe_aux_stats_kernel(const __nv_bfloat16* __restrict__ logits,
+                                                            const int32_t* __restrict__ sel_idx, int64_t T_real, int E,
+                                                            int k, float* __restrict__ partial) {
+    __shared__ float s_p[8][256];
+    __shared__ int s_c[256];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    for (int e = threadIdx.x; e < E; e += blockDim.x) s_c[e] = 0;
+    __syncthreads();
+    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    for (int j = 0; j < AUX_TOK_PER_CTA / 8; ++j) {
+        const int64_t t = int64_t(blockIdx.x) * AUX_TOK_PER_CTA + w + 8 * j;
+        if (t >= T_real) break;
+        float p[8];
+        row_softmax(logits + t * E, E, lane, p);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) acc[i] += p[i];
+        if (lane < k) atomicAdd(&s_c[sel_idx[t * k + lane]], 1);  // integer: the total does not depend on the order
+    }
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+        if (lane + i * 32 < E) s_p[w][lane + i * 32] = acc[i];
+    __syncthreads();
+    float* out = partial + int64_t(blockIdx.x) * 2 * E;
+    for (int e = threadIdx.x; e < E; e += blockDim.x) {
+        float s = 0.f;
+        for (int q = 0; q < 8; ++q) s += s_p[q][e];
+        out[e] = s;
+        out[E + e] = float(s_c[e]);
+    }
+}
+
+// acc[i] += sum_b partial[b][i] in CTA order (one CTA)
+__global__ void moe_aux_reduce_kernel(const float* __restrict__ partial, int n_parts, int E, float* __restrict__ acc) {
+    for (int i = threadIdx.x; i < 2 * E; i += blockDim.x) {
+        float s = 0.f;
+        for (int b = 0; b < n_parts; ++b) s += partial[int64_t(b) * 2 * E + i];
+        acc[i] += s;
+    }
+}
+
+// aux = E * sum_e C_e P_e / N^2, backward coefficients c_e = E * C_e / N^2, loss += coef * aux (one CTA of 256 threads;
+// the products are formed and summed in fp64 and rounded once)
+__global__ void moe_aux_finalize_kernel(const float* __restrict__ acc, int E, int64_t N, float coef, float* __restrict__ aux,
+                                        float* __restrict__ c, float* __restrict__ loss) {
+    __shared__ double s_prod[256];
+    const double scale = double(E) / (double(N) * double(N));
+    const int e = threadIdx.x;
+    s_prod[e] = e < E ? double(acc[E + e]) * double(acc[e]) : 0.0;
+    if (e < E) c[e] = float(scale * double(acc[E + e]));
+    __syncthreads();
+    if (e == 0) {
+        double s = 0.0;
+        for (int q = 0; q < E; ++q) s += s_prod[q];
+        const float a = float(scale * s);
+        aux[0] = a;
+        if (loss != nullptr) loss[0] += coef * a;
+    }
+}
+
+// moe_router_bwd plus the load-balancing term, one warp per token:
+//   dlogits[t,e] = [e selected] w_e (dw_e - sum_j w_j dw_j) + s p[t,e] (c_e - sum_j p[t,j] c_j)     (rows t < T_real)
+// s (= coef * dL/dloss + dL/daux) is read from the device; one bf16 rounding per element
+__global__ void __launch_bounds__(256) moe_router_bwd_aux_kernel(
+    const __nv_bfloat16* __restrict__ logits, const int32_t* __restrict__ sel_idx, const float* __restrict__ sel_w,
+    const float* __restrict__ dw, const float* __restrict__ c, const float* __restrict__ s_ptr,
+    __nv_bfloat16* __restrict__ dlogits, int64_t T, int64_t T_real, int E, int k) {
+    const int64_t t = (int64_t(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (t >= T) return;
+    float g[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    if (t < T_real) {
+        float p[8], ce[8];
+        row_softmax(logits + t * E, E, lane, p);
+        float pc = 0.f;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+            ce[i] = lane + i * 32 < E ? c[lane + i * 32] : 0.f;
+            pc += p[i] * ce[i];
+        }
+        pc = warp_sum(pc);
+        const float s = *s_ptr;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) g[i] = s * p[i] * (ce[i] - pc);
+    }
+    float dot = 0.f;
+    for (int j = 0; j < k; ++j) dot += sel_w[t * k + j] * dw[t * k + j];
+    for (int j = 0; j < k; ++j) {
+        const int e = sel_idx[t * k + j];
+        const float v = sel_w[t * k + j] * (dw[t * k + j] - dot);
+#pragma unroll
+        for (int i = 0; i < 8; ++i)
+            if (lane + i * 32 == e) g[i] += v;
+    }
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+        if (lane + i * 32 < E) dlogits[t * E + lane + i * 32] = __float2bfloat16_rn(g[i]);
+}
+
 inline int64_t align256(int64_t x) { return (x + 255) & ~int64_t(255); }
 
 }  // namespace
@@ -363,5 +491,50 @@ extern "C" int dolomite_b200_moe_router_bwd(const int32_t* sel_idx, const float*
     moe_router_bwd_kernel<<<(unsigned)((T + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         sel_idx, sel_w, dw, static_cast<__nv_bfloat16*>(dlogits), T, E, k);
     DOLO_LAUNCH_OK("moe_router_bwd");
+    return DOLO_OK;
+}
+
+extern "C" int64_t dolomite_b200_moe_aux_partial_floats(int64_t T_real, int E) {
+    return (T_real + AUX_TOK_PER_CTA - 1) / AUX_TOK_PER_CTA * 2 * int64_t(E);
+}
+
+extern "C" int dolomite_b200_moe_aux_stats(const void* router_logits, const int32_t* sel_idx, int64_t T, int64_t T_real,
+                                           int E, int k, float* partial, float* acc, void* stream) {
+    DOLO_REQUIRE(E > 0 && E <= 256, "moe_aux_stats: num_experts=%d must be in [1, 256]", E);
+    DOLO_REQUIRE(k > 0 && k <= 8 && k <= E, "moe_aux_stats: top-k=%d must be in [1, min(8, E)]", k);
+    DOLO_REQUIRE(T_real >= 0 && T_real <= T, "moe_aux_stats: T_real=%lld must be in [0, T=%lld]", (long long)T_real,
+                 (long long)T);
+    if (T_real == 0) return DOLO_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int64_t parts = (T_real + AUX_TOK_PER_CTA - 1) / AUX_TOK_PER_CTA;
+    moe_aux_stats_kernel<<<(unsigned)parts, 256, 0, st>>>(static_cast<const __nv_bfloat16*>(router_logits), sel_idx, T_real,
+                                                          E, k, partial);
+    DOLO_LAUNCH_OK("moe_aux_stats");
+    moe_aux_reduce_kernel<<<1, 256, 0, st>>>(partial, int(parts), E, acc);
+    DOLO_LAUNCH_OK("moe_aux_reduce");
+    return DOLO_OK;
+}
+
+extern "C" int dolomite_b200_moe_aux_finalize(const float* acc, int E, int64_t n_tokens, float coef, float* aux, float* c,
+                                              float* loss, void* stream) {
+    DOLO_REQUIRE(E > 0 && E <= 256, "moe_aux_finalize: num_experts=%d must be in [1, 256]", E);
+    DOLO_REQUIRE(n_tokens > 0, "moe_aux_finalize: the load-balancing loss needs at least one real token");
+    moe_aux_finalize_kernel<<<1, 256, 0, static_cast<cudaStream_t>(stream)>>>(acc, E, n_tokens, coef, aux, c, loss);
+    DOLO_LAUNCH_OK("moe_aux_finalize");
+    return DOLO_OK;
+}
+
+extern "C" int dolomite_b200_moe_router_bwd_aux(const void* router_logits, const int32_t* sel_idx, const float* sel_w,
+                                                const float* dw, const float* c, const float* s, void* dlogits, int64_t T,
+                                                int64_t T_real, int E, int k, void* stream) {
+    DOLO_REQUIRE(E > 0 && E <= 256, "moe_router_bwd_aux: num_experts=%d must be in [1, 256]", E);
+    DOLO_REQUIRE(k > 0 && k <= 8 && k <= E, "moe_router_bwd_aux: top-k=%d must be in [1, min(8, E)]", k);
+    DOLO_REQUIRE(T_real >= 0 && T_real <= T, "moe_router_bwd_aux: T_real=%lld must be in [0, T=%lld]", (long long)T_real,
+                 (long long)T);
+    if (T == 0) return DOLO_OK;
+    moe_router_bwd_aux_kernel<<<(unsigned)((T * 32 + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<const __nv_bfloat16*>(router_logits), sel_idx, sel_w, dw, c, s, static_cast<__nv_bfloat16*>(dlogits), T,
+        T_real, E, k);
+    DOLO_LAUNCH_OK("moe_router_bwd_aux");
     return DOLO_OK;
 }

@@ -310,6 +310,11 @@ class DolomiteEngine:
         # weights are cast once per pass anyway and are not kept, which would hold an fp8 copy of the whole model)
         self._fp8_wcache: dict = {}
         self._fp8_keep: set = set()
+        # MoE load-balancing loss (forward(router_aux=True)): `_aux_fwd` = (accumulator [2, E], T_real, router logits list)
+        # while a forward collects the statistics -- never while backward re-runs a checkpointed block; `_aux_bwd` =
+        # (c [E], s [1], T_real) while its backward runs
+        self._aux_fwd = None
+        self._aux_bwd = None
         if cfg.attention_multiplier is not None:
             self.softmax_scale = float(cfg.attention_multiplier)
         elif cfg.scale_attn_weights:
@@ -569,13 +574,25 @@ class DolomiteEngine:
         return h, (x_in, rstd1, ln1, qkv, attn, lse, h_mid, rstd2, ln2, fc, act)
 
     def forward(self, input_ids, position_ids, cu_seqlens, max_seqlen: int, labels=None, ignore_index: int = -100,
-                save_for_backward: bool = True, fuse_head_loss: bool = False, alibi: bool = False):
+                save_for_backward: bool = True, fuse_head_loss: bool = False, alibi: bool = False,
+                router_aux: bool = False, T_real: int | None = None, coef: float = 0.0):
         """Returns (logits_or_None, loss_or_None).  input_ids int64 [T]; cu_seqlens int32 [B+1].
         `fuse_head_loss`: the caller will backpropagate d(loss) = 1 (what train_step does), so the LM head's backward can run
         chunk-wise inside the loss computation and the [T, V] logits are never materialised.
         `alibi`: add the ALiBi bias of an alibi model to the attention logits (the key's index inside its document);
-        False runs an alibi model as NoPE, which is what the reference's SDPA attention does without an attention mask."""
+        False runs an alibi model as NoPE, which is what the reference's SDPA attention does without an attention mask.
+        `router_aux` (MoE): also compute the load-balancing loss aux over the first `T_real` token rows (default: all) of
+        every layer, add `coef * aux` to the loss, and return (logits_or_None, loss_or_None, aux [1] fp32, router logits:
+        one bf16 [T, E] tensor per layer).  backward(aux_grad_dev=...) then takes s = coef * dL/dloss + dL/daux."""
         cfg = self.cfg
+        self._aux_fwd = None
+        if router_aux:
+            if not self.is_moe:
+                raise ValueError("router_aux needs an MoE model (model_type moe_dolomite)")
+            T_real = input_ids.numel() if T_real is None else int(T_real)
+            if not 0 < T_real <= input_ids.numel():
+                raise ValueError(f"T_real={T_real} must be in [1, {input_ids.numel()}]")
+            self._aux_fwd = (K.moe_aux_acc(cfg.num_experts, self.device), T_real, [])
         self._begin_dropout_pass()
         self._alibi_now = self._alibi_slopes_for(alibi)
         self._fp8_now = self.fp8 is not None and self.fp8_autocast and self.training and save_for_backward
@@ -645,12 +662,21 @@ class DolomiteEngine:
                 loss, _, dlogits = K.cross_entropy_fwd_bwd(logits, labels, ignore_index=ignore_index, dlogits=None)
             else:
                 logits_out = logits.contiguous()  # [T, V] as the reference returns it: a copy when V % 8 != 0
+        router_aux_saved = None
+        if self._aux_fwd is not None:
+            acc, T_real, router_logits = self._aux_fwd
+            self._aux_fwd = None
+            aux, c = K.moe_aux_finalize(acc, cfg.n_layer * T_real, coef, loss)  # loss += coef * aux on the device
+            router_aux_saved = (c, T_real, float(coef))
         if save_for_backward:
             self._saved = dict(input_ids=input_ids, position_ids=position_ids, cu_seqlens=cu_seqlens, max_seqlen=max_seqlen,
                                layers=saved_layers, h_last=h, rstd_f=rstd_f, hf=hf, dlogits=dlogits, d_hf=d_hf, T=T,
-                               dropout_seed=self._dropout_now, fp8=self._fp8_now, alibi=self._alibi_now)
+                               dropout_seed=self._dropout_now, fp8=self._fp8_now, alibi=self._alibi_now,
+                               router_aux=router_aux_saved)
         self._fp8_now = False
         self._fp8_wcache.clear()
+        if router_aux_saved is not None:
+            return logits_out, loss, aux, tuple(router_logits)
         return logits_out, loss
 
     def _alibi_slopes_for(self, alibi: bool):
@@ -851,11 +877,22 @@ class DolomiteEngine:
         if self._wgrad_stream is not None:
             (torch.cuda.current_stream() if stream is None else stream).wait_stream(self._wgrad_stream)
 
-    def backward(self, dlogits=None, grad_scale_dev=None) -> None:
-        """Backward of the last forward.  `dlogits` overrides the CE gradient (logits-mode autograd)."""
+    def backward(self, dlogits=None, grad_scale_dev=None, aux_grad_dev=None) -> None:
+        """Backward of the last forward.  `dlogits` overrides the CE gradient (logits-mode autograd).
+        After forward(router_aux=True), `aux_grad_dev` (fp32 device scalar) is the factor s = coef * dL/dloss + dL/daux of
+        the load-balancing term's router gradient; by default that of backpropagating the returned loss,
+        coef * (grad_scale_dev or 1)."""
         s = self._saved
         if s is None:
             raise RuntimeError("backward called without a saved forward")
+        self._aux_bwd = None
+        if s.get("router_aux") is not None:
+            c, T_real, coef = s["router_aux"]
+            if aux_grad_dev is None:
+                aux_grad_dev = torch.full((1,), coef, dtype=torch.float32, device=c.device)
+                if grad_scale_dev is not None:
+                    aux_grad_dev = aux_grad_dev * grad_scale_dev.reshape(1).float()
+            self._aux_bwd = (c, aux_grad_dev.reshape(1).float().contiguous(), T_real)
         cfg = self.cfg
         root = self.units[0]
         comm = self.comm
@@ -963,6 +1000,7 @@ class DolomiteEngine:
             self.fp8.update(all_reduce=self.comm is not None and self.world_size > 1)
             self._fp8_now = False
             self._fp8_wcache.clear()
+        self._aux_bwd = None
         self._saved = None
 
     # ------------------------------------------------------------------------------------------

@@ -33,38 +33,78 @@ class CausalLMOutputWithPast:
         return tuple(v for v in (self.loss, self.logits) if v is not None)[i]
 
 
+@dataclass
+class MoeCausalLMOutputWithPast:
+    """transformers' MoeCausalLMOutputWithPast, returned by MoEDolomiteForCausalLM with output_router_logits=True
+    (moe_dolomite/main.py:123-131)"""
+
+    loss: torch.Tensor | None = None
+    aux_loss: torch.Tensor | None = None
+    logits: torch.Tensor | None = None
+    past_key_values: None = None
+    hidden_states: None = None
+    attentions: None = None
+    router_logits: tuple | None = None
+
+    def to_tuple(self) -> tuple:
+        """the return_dict=False order of the reference (main.py:117-121): (loss, aux_loss, logits, router_logits)"""
+        return tuple(v for v in (self.loss, self.aux_loss, self.logits, self.router_logits) if v is not None)
+
+    def __getitem__(self, i):
+        return self.to_tuple()[i]
+
+
 class _EngineFunction(torch.autograd.Function):
     """Bridges autograd to the explicit engine: the only differentiable input is a dummy anchor; parameter gradients
     are accumulated by the engine into its flat fp32 gradient buffers (exactly where FSDP would leave them)."""
 
     @staticmethod
     def forward(ctx, anchor, model, input_ids, position_ids, cu_seqlens, max_seqlen, labels, ignore_index, save=True,
-                alibi=False):
+                alibi=False, router_aux=None):
         # `save`: the caller's torch.is_grad_enabled() (always False in here); under no_grad (evaluation) no activation is kept
         # `alibi`: the pass adds the ALiBi bias (DolomitePreTrainedModel._alibi_pass)
+        # `router_aux`: None, or (T_real, coef) of the MoE load-balancing loss.  The outputs are then (loss or logits,
+        # aux_loss, router logits of every layer); the router logits are not differentiable
         engine = model.engine
+        ctx.model = model
+        ctx.loss_mode = labels is not None
+        ctx.router_aux = router_aux
+        if router_aux is not None:
+            T_real, coef = router_aux
+            logits, loss, aux, router_logits = engine.forward(
+                input_ids, position_ids, cu_seqlens, max_seqlen, labels=labels, ignore_index=ignore_index,
+                save_for_backward=bool(save), alibi=bool(alibi), router_aux=True, T_real=T_real, coef=coef)
+            ctx.mark_non_differentiable(*router_logits)
+            return (loss.reshape(()) if ctx.loss_mode else logits, aux.reshape(())) + tuple(router_logits)
         # `assume_unit_loss_grad` (set by the training wrappers: train_step calls loss.backward() on the raw loss) lets the
         # engine run the LM head's backward chunk-wise inside the loss computation without ever materialising [T, V]
         logits, loss = engine.forward(input_ids, position_ids, cu_seqlens, max_seqlen, labels=labels,
                                       ignore_index=ignore_index, save_for_backward=bool(save),
                                       fuse_head_loss=bool(save) and labels is not None and model.assume_unit_loss_grad,
                                       alibi=bool(alibi))
-        ctx.model = model
-        ctx.loss_mode = labels is not None
         return loss.reshape(()) if ctx.loss_mode else logits
 
     @staticmethod
-    def backward(ctx, grad_out):
+    def backward(ctx, grad_out, *more):
         model = ctx.model
         engine = model.engine
-        if ctx.loss_mode:
+        if ctx.router_aux is not None:
+            # loss = CE + coef * aux: the router's load-balancing gradient is scaled by s = coef * dL/dloss + dL/daux,
+            # formed on the device (no host sync); both upstream gradients are general here (no unit-gradient shortcut)
+            g_aux = more[0].reshape(1).float()
+            if ctx.loss_mode:
+                g_loss = grad_out.reshape(1).float()
+                engine.backward(grad_scale_dev=g_loss, aux_grad_dev=ctx.router_aux[1] * g_loss + g_aux)
+            else:
+                engine.backward(dlogits=grad_out.contiguous(), aux_grad_dev=g_aux)
+        elif ctx.loss_mode:
             # d(loss)/d(loss) arrives as a 0-d device tensor; it is 1 for `loss.backward()` (the only thing
             # train_utils.train_step does).  Anything else is applied on the device, without a host sync.
             scale = None if model.assume_unit_loss_grad else grad_out.reshape(1).float()
             engine.backward(grad_scale_dev=scale)
         else:
             engine.backward(dlogits=grad_out.contiguous())
-        return (None,) * 10
+        return (None,) * 11
 
 
 def _pad_packed_stream(input_ids, position_ids, cu_seqlens, shift_labels, multiple: int = 8):
@@ -163,13 +203,14 @@ class DolomitePreTrainedModel(nn.Module):
     def forward(self, input_ids=None, past_key_values=None, attention_mask=None, token_type_ids=None, position_ids=None,
                 inputs_embeds=None, labels=None, use_cache=None, output_attentions=None, output_hidden_states=None,
                 return_dict=True, cu_seqlens=None, max_seqlen=None, output_router_logits=None):
-        if output_router_logits:
+        if output_router_logits and self._use_padding_free_transformer:
             # moe_dolomite/main.py:47-48
-            raise NotImplementedError("router loss is not implemented with padding_free transformer")
+            raise NotImplementedError("padding_free is not supported with load_balancing_loss_func currently")
         assert not output_hidden_states, "output_hidden_states is not supported on the B200 path"
         if not self._use_padding_free_transformer:
             return self._forward_padded(input_ids, attention_mask, position_ids, labels, return_dict, past_key_values,
-                                        use_cache, inputs_embeds, token_type_ids, cu_seqlens)
+                                        use_cache, inputs_embeds, token_type_ids, cu_seqlens,
+                                        output_router_logits=bool(output_router_logits))
         input_ids, position_ids, token_type_ids, labels, cu_seqlens, max_seqlen = self.prepare_inputs_for_model(
             input_ids, inputs_embeds, position_ids, token_type_ids, labels, cu_seqlens, max_seqlen, past_key_values,
             attention_mask, use_cache, output_attentions,
@@ -216,11 +257,16 @@ class DolomitePreTrainedModel(nn.Module):
         return 16 if e.fp8 is not None and e.fp8_autocast and e.training and torch.is_grad_enabled() else 8
 
     def _forward_padded(self, input_ids, attention_mask, position_ids, labels, return_dict, past_key_values, use_cache,
-                        inputs_embeds, token_type_ids, cu_seqlens):
+                        inputs_embeds, token_type_ids, cu_seqlens, output_router_logits: bool = False):
         """Padded batch path (gpt_dolomite/base.py:374-522 non-padding-free branch + attention/flash.py unpad/pad):
         input_ids [B, S], attention_mask [B, S] (1 = token, left or right padding), labels [B, S] (-100 at padding).
         position_ids default to `cumsum(mask) - 1` (base.py:524-534); loss = CE(logits[:, :-1], labels[:, 1:]) over the
-        non-ignored positions (main.py:179-202).  Every row becomes one document of the packed stream."""
+        non-ignored positions (main.py:179-202).  Every row becomes one document of the packed stream.
+        `output_router_logits` (MoE, moe_dolomite/main.py:30-130): also the load-balancing loss over the real tokens
+        (`aux_loss`; `loss` = CE + router_aux_loss_coef * aux_loss) and every layer's router logits as [B*S, E], zero at
+        padding."""
+        if output_router_logits and not self.engine.is_moe:
+            raise ValueError("output_router_logits needs an MoE model (MoEDolomiteForCausalLM)")
         if use_cache or past_key_values is not None:
             raise NotImplementedError("KV caching / generation is not implemented on the B200 training path")
         if inputs_embeds is not None or token_type_ids is not None:
@@ -257,14 +303,28 @@ class DolomitePreTrainedModel(nn.Module):
             nxt = torch.where(nxt_valid & mask, nxt, torch.full_like(nxt, -100))
             shift_labels = nxt.reshape(-1)[keep].contiguous()
         ids_p, pos_p, cu, shift_labels, T_real = _pad_packed_stream(ids_p, pos_p, cu, shift_labels, self._token_multiple())
+        router_aux = (T_real, float(self.config.router_aux_loss_coef)) if output_router_logits else None
         out = _EngineFunction.apply(self._anchor, self, ids_p, pos_p, cu, int(max(max_seqlen, 1)), shift_labels, -100,
-                                    torch.is_grad_enabled(), self._alibi_pass(attention_mask is not None))
+                                    torch.is_grad_enabled(), self._alibi_pass(attention_mask is not None), router_aux)
+        aux_loss = router_logits = None
+        if router_aux is not None:
+            out, aux_loss, packed_router = out[0], out[1], out[2:]
+            router_logits = []
+            for lg in packed_router:  # [T, E] of the packed stream -> [B*S, E] rows of the batch, zeros at padding
+                full = lg.new_zeros(B * S, lg.shape[-1])
+                full[keep] = lg[:T_real]
+                router_logits.append(full)
+            router_logits = tuple(router_logits)
         if shift_labels is not None:
-            result = CausalLMOutputWithPast(loss=out, logits=None)
+            loss, logits = out, None
         else:
             full = out.new_zeros(B * S, out.shape[-1])
             full[keep] = out[:T_real]
-            result = CausalLMOutputWithPast(loss=None, logits=full.view(B, S, -1))
+            loss, logits = None, full.view(B, S, -1)
+        if router_aux is not None:
+            result = MoeCausalLMOutputWithPast(loss=loss, aux_loss=aux_loss, logits=logits, router_logits=router_logits)
+            return result if return_dict else result.to_tuple()
+        result = CausalLMOutputWithPast(loss=loss, logits=logits)
         if not return_dict:
             return tuple(v for v in (result.loss, result.logits) if v is not None)
         return result

@@ -753,6 +753,48 @@ def moe_router_bwd(plan: MoEPlan, dw):
     return dl
 
 
+# MoE load-balancing loss (moe_dolomite/base.py:24-43, transformers' Mixtral load_balancing_loss_func)
+def moe_aux_acc(E: int, device) -> torch.Tensor:
+    """cleared [2, E] fp32 accumulator of the load-balancing statistics of one forward: [sum of probabilities | counts]"""
+    return torch.zeros(2, E, dtype=torch.float32, device=device)
+
+
+def moe_aux_stats(router_logits, plan: MoEPlan, T_real: int, acc) -> None:
+    """acc += this layer's statistics over its first T_real token rows (fixed summation order: bit-identical run to run)"""
+    _req(router_logits, _BF16, "router_logits"), _req(acc, torch.float32, "acc")
+    T, E = router_logits.shape
+    assert router_logits.is_contiguous() and acc.is_contiguous() and acc.numel() == 2 * E and T == plan.T and E == plan.E
+    n = _lib.load().dolomite_b200_moe_aux_partial_floats(T_real, E)
+    partial = torch.empty(max(n, 1), dtype=torch.float32, device=acc.device)
+    _lib.call("dolomite_b200_moe_aux_stats", router_logits.data_ptr(), plan.sel_idx.data_ptr(), T, T_real, E, plan.k,
+              partial.data_ptr(), acc.data_ptr(), _stream())
+
+
+def moe_aux_finalize(acc, n_tokens: int, coef: float = 0.0, loss=None):
+    """-> (aux [1] fp32, backward coefficients c [E] fp32) of the statistics in `acc` over n_tokens = layers * real tokens;
+    adds coef * aux into the fp32 device scalar `loss` when it is given.  No host sync."""
+    _req(acc, torch.float32, "acc")
+    E = acc.shape[-1]
+    if loss is not None:
+        _req(loss, torch.float32, "loss")
+        assert loss.numel() == 1
+    aux = torch.empty(1, dtype=torch.float32, device=acc.device)
+    c = torch.empty(E, dtype=torch.float32, device=acc.device)
+    _lib.call("dolomite_b200_moe_aux_finalize", acc.data_ptr(), E, int(n_tokens), float(coef), aux.data_ptr(), c.data_ptr(),
+              _ptr(loss), _stream())
+    return aux, c
+
+
+def moe_router_bwd_aux(router_logits, plan: MoEPlan, dw, c, s, T_real: int):
+    """moe_router_bwd + the load-balancing term s * p * (c - <p, c>) on the first T_real rows; s: fp32 device scalar"""
+    _req(router_logits, _BF16, "router_logits"), _req(c, torch.float32, "c"), _req(s, torch.float32, "s")
+    assert router_logits.is_contiguous() and tuple(router_logits.shape) == (plan.T, plan.E) and c.numel() == plan.E
+    dl = torch.empty(plan.T, plan.E, dtype=_BF16, device=dw.device)
+    _lib.call("dolomite_b200_moe_router_bwd_aux", router_logits.data_ptr(), plan.sel_idx.data_ptr(), plan.sel_w.data_ptr(),
+              dw.data_ptr(), c.data_ptr(), s.data_ptr(), dl.data_ptr(), plan.T, T_real, plan.E, plan.k, _stream())
+    return dl
+
+
 def gemm_grouped_m(a, w3, plan: MoEPlan, *, b_mn: bool, alpha: float = 1.0, flags=None):
     """rows of `a` grouped by expert.  b_mn=False: w3 [E, N, K] -> D = A W[e]^T;  b_mn=True: w3 [E, K, N] -> D = A W[e]"""
     _req(a, _BF16, "a"), _req(w3, _BF16, "w3")

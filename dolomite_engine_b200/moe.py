@@ -32,6 +32,10 @@ def forward(engine, unit, p: str, x, residual, m_res: float, layer: int = 0):
         raise NotImplementedError("expert biases are not supported by the grouped-GEMM MoE path (moe/scatter.py:22)")
     logits = engine._linear(unit, p + "mlp.gate.weight", x, flags=0)  # [T, E] bf16 (tiny N: direct-store epilogue)
     plan = K.moe_route(logits, k)
+    if engine._aux_fwd is not None:  # load-balancing statistics of this layer (once per forward: not in recomputed blocks)
+        acc, T_real, router_logits = engine._aux_fwd
+        K.moe_aux_stats(logits, plan, T_real, acc)
+        router_logits.append(logits)
     if FUSED_GATHER:
         # scattermoe `parallel_linear(grouped_in=False, grouped_out=True)`: the expert GEMM reads the token rows straight
         # out of x (copied by its producer warp); no grouped copy of x is written in forward
@@ -70,8 +74,13 @@ def backward(engine, unit, p: str, x, dh, m_res: float, saved, layer: int = 0):
     del xg
     dxg = K.gemm_grouped_m(d_fc, w_fc, plan, b_mn=True)                               # [rows, H]
     dx = K.moe_token_sum(dxg, plan)
-    # router path: softmax-over-k backward -> dense dlogits -> gate wgrad and dx contribution
-    dlogits = K.moe_router_bwd(plan, dw)
+    # router path: softmax-over-k backward (+ the load-balancing term) -> dense dlogits -> gate wgrad and dx contribution;
+    # an FP8 router casts (and takes the amax of) dlogits with the term in it, as te.Linear would see it
+    if engine._aux_bwd is not None:
+        c, s, T_real = engine._aux_bwd
+        dlogits = K.moe_router_bwd_aux(logits, plan, dw, c, s, T_real)
+    else:
+        dlogits = K.moe_router_bwd(plan, dw)
     if engine._is_fp8(p + "mlp.gate.weight"):  # the router as te.Linear (num_experts % 16 == 0)
         return engine._linear_bwd_fp8(unit, p + "mlp.gate.weight", None, x, dlogits, dx_add=dx)
     gate = unit.views[p + "mlp.gate.weight"]

@@ -394,6 +394,26 @@ int dolomite_b200_moe_router_bwd(const int32_t* sel_idx, const float* sel_w, con
                                  int E, int k, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * MoE load-balancing loss (moe_dolomite/base.py:24-43 -> transformers' Mixtral load_balancing_loss_func), accumulated
+ * over the L MoE layers of one forward; rows t >= T_real (alignment rows) are not tokens.  With N = L * T_real:
+ *   moe_aux_stats:    acc[0][e] += sum_t softmax(logits[t])_e (fp32 softmax over all E of the bf16 row),
+ *                     acc[1][e] += #(t, slot) with sel_idx[t, slot] == e (exact below 2^24 per expert).  acc is [2, E]
+ *                     fp32, partial is scratch of moe_aux_partial_floats(T_real, E) floats; fixed-order sums only.
+ *   moe_aux_finalize: aux = E * sum_e acc[1][e] acc[0][e] / N^2, c[e] = E * acc[1][e] / N^2, and loss[0] += coef * aux
+ *                     when loss != NULL (all on the device).
+ *   moe_router_bwd_aux: moe_router_bwd plus, on rows t < T_real, s * p[t,e] * (c[e] - sum_j p[t,j] c[j]) with the scalar
+ *                     s = *s (coef * dL/dloss + dL/daux) read on the device; dlogits rounded to bf16 once.
+ * ------------------------------------------------------------------------------------------------ */
+int64_t dolomite_b200_moe_aux_partial_floats(int64_t T_real, int E);
+int dolomite_b200_moe_aux_stats(const void* router_logits, const int32_t* sel_idx, int64_t T, int64_t T_real, int E, int k,
+                                float* partial, float* acc, void* stream);
+int dolomite_b200_moe_aux_finalize(const float* acc, int E, int64_t n_tokens, float coef, float* aux, float* c,
+                                   float* loss, void* stream);
+int dolomite_b200_moe_router_bwd_aux(const void* router_logits, const int32_t* sel_idx, const float* sel_w,
+                                     const float* dw, const float* c, const float* s, void* dlogits, int64_t T,
+                                     int64_t T_real, int E, int k, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Packed var-len causal attention (replaces flash_attn_varlen_func at attention/padding_free.py:51-62).
  *   qkv: packed projection output [T, row_stride] in the slot layout described at rope_qk_inplace.
  *   out: [T, n_heads*head_dim] bf16; lse: fp32 [n_heads, T] (natural log-sum-exp of scale*s).
