@@ -41,6 +41,7 @@ SIGNATURES: dict[str, tuple] = {
     "dolomite_b200_layernorm_bwd": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _L, _I, _P]),
     "dolomite_b200_act_fwd": (_I, [_I, _I, _P, _P, _L, _L, _P]),
     "dolomite_b200_act_bwd": (_I, [_I, _I, _P, _P, _P, _P, _L, _L, _P]),
+    "dolomite_b200_act_bwd_segmented": (_I, [_I, _I, _P, _P, _P, _P, _L, _L, _P, _I, _P]),
     "dolomite_b200_gelu_fwd": (_I, [_P, _P, _L, _P]),
     "dolomite_b200_gelu_bwd": (_I, [_P, _P, _P, _P, _L, _L, _P]),
     "dolomite_b200_swiglu_fwd": (_I, [_P, _P, _L, _L, _P]),
@@ -53,6 +54,7 @@ SIGNATURES: dict[str, tuple] = {
     "dolomite_b200_cross_entropy_rows": (_I, [_P, _L, _P, _P, _P, _P, _L, _L, _L, _F, _F, _P]),
     "dolomite_b200_cross_entropy_mean": (_I, [_P, _L, _P, _P, _P]),
     "dolomite_b200_colsum_accum": (_I, [_P, _L, _P, _L, _L, _F, _P]),
+    "dolomite_b200_colsum_accum_segmented": (_I, [_P, _L, _P, _L, _L, _P, _I, _F, _P]),
     "dolomite_b200_scale_bf16_by_device_scalar": (_I, [_P, _L, _P, _P]),
     "dolomite_b200_add_scaled": (_I, [_P, _P, _P, _F, _L, _P]),
     "dolomite_b200_dropout_fwd": (_I, [_P, _P, _P, _L, _F, _F, _U, _U, _P]),
@@ -84,6 +86,10 @@ SIGNATURES: dict[str, tuple] = {
     "dolomite_b200_moe_max_rows": (_L, [_L, _I, _I]),
     "dolomite_b200_moe_route": (_I, [_P, _L, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "dolomite_b200_gemm_bf16_grouped_m_gather": (_I, [_P, _L, _L, _P, _P, _L, _P, _L, _F, _L, _L, _L, _P, _I, _I, _P]),
+    "dolomite_b200_gemm_bf16_grouped_m_bias": (
+        _I,
+        [_P, _L, _L, _P, _P, _L, _I, _P, _L, _P, _L, _F, _L, _L, _L, _P, _I, _I, _P],
+    ),
     "dolomite_b200_moe_gather": (_I, [_P, _P, _P, _P, _L, _I, _I, _I, _P]),
     "dolomite_b200_moe_combine": (_I, [_P, _P, _P, _P, _P, _L, _I, _I, _F, _P]),
     "dolomite_b200_moe_combine_bwd": (_I, [_P, _P, _P, _P, _P, _P, _P, _L, _I, _I, _I, _F, _P]),

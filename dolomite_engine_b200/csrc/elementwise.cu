@@ -45,10 +45,12 @@ __device__ __forceinline__ void cluster_colsum_apply(const float* part, float* o
     }
     cluster_sync_all();  // the partials stay alive until rank 0 has read them
 }
+// Grid (column tiles, one cluster of row splits, segments): the row splits of segment z cover its rows in kColsumCluster
+// equal parts (segment_rows); a dense launch is the one segment [0, T).
 template <typename Kern, typename... Args>
-static int launch_row_cluster(Kern kern, int col_tiles, cudaStream_t st, Args... args) {
+static int launch_row_cluster(Kern kern, int col_tiles, int segments, cudaStream_t st, Args... args) {
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(unsigned(col_tiles), kColsumCluster, 1);
+    cfg.gridDim = dim3(unsigned(col_tiles), kColsumCluster, unsigned(segments));
     cfg.blockDim = dim3(kThreads);
     cfg.stream = st;
     cudaLaunchAttribute attr[1];
@@ -59,6 +61,23 @@ static int launch_row_cluster(Kern kern, int col_tiles, cudaStream_t st, Args...
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     return int(cudaLaunchKernelEx(&cfg, kern, args...));
+}
+
+// Rows [r0, r1) of this CTA's row split.  seg == NULL: one segment [0, T) cut into rows_per_block rows per split.
+// Otherwise segment blockIdx.z is rows [seg[z], seg[z + 1]) (an empty one gives every split an empty range).  Returns
+// the offset of the segment's row of the per-segment sums, out_seg_stride floats apart (0 for the dense launch).
+__device__ __forceinline__ int64_t segment_rows(const int* seg, int64_t T, int rows_per_block, int64_t out_seg_stride,
+                                                int64_t& r0, int64_t& r1) {
+    int64_t base = 0, n = T, rpb = rows_per_block, out_off = 0;
+    if (seg != nullptr) {
+        base = seg[blockIdx.z];
+        n = seg[blockIdx.z + 1] - base;
+        rpb = (n + kColsumCluster - 1) / kColsumCluster;
+        out_off = int64_t(blockIdx.z) * out_seg_stride;
+    }
+    r0 = base + int64_t(blockIdx.y) * rpb;
+    r1 = base + min(n, int64_t(blockIdx.y + 1) * rpb);
+    return out_off;
 }
 
 __device__ __forceinline__ void unpack8(const uint4& v, float (&f)[8]) {
@@ -550,17 +569,19 @@ __global__ void __launch_bounds__(kThreads) act_bwd_kernel(const uint4* __restri
 // Backward that also accumulates the bias gradient of the producing linear layer (column sums of the bf16 dx it
 // writes): saves the separate pass that re-read the whole dx.  Block = 32 column vectors (256 columns of each half)
 // x 8 row lanes over `rows_per_block` rows; per-thread fp32 column sums, smem combine, and the row splits of a column
-// tile (one cluster) combined in a fixed order (cluster_colsum_apply).
+// tile (one cluster) combined in a fixed order (cluster_colsum_apply).  With a segment table (grouped MoE rows) the
+// grid's z enumerates the segments and each gets its own bias-gradient row (segment_rows).
 template <class Op, bool Glu>
 __global__ void __launch_bounds__(kThreads)
     act_bwd_bias_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x, uint4* __restrict__ dx,
-                        float* __restrict__ dbias, int64_t T, int64_t F8, int rows_per_block) {
+                        float* __restrict__ dbias, int64_t T, int64_t F8, int rows_per_block,
+                        const int* __restrict__ seg, int64_t dbias_seg_stride) {
     constexpr int NP = Glu ? 2 : 1;
     __shared__ float sm[8][NP][256];
     const int lane = threadIdx.x & 31, rl = threadIdx.x >> 5;
     const int64_t c = int64_t(blockIdx.x) * 32 + lane;
-    const int64_t r0 = int64_t(blockIdx.y) * rows_per_block;
-    const int64_t r1 = min(T, r0 + rows_per_block);
+    int64_t r0, r1;
+    float* const dbias_seg = dbias + segment_rows(seg, T, rows_per_block, dbias_seg_stride, r0, r1);
     float s[NP][8];
 #pragma unroll
     for (int p = 0; p < NP; ++p)
@@ -597,7 +618,7 @@ __global__ void __launch_bounds__(kThreads)
     const int64_t gc = int64_t(blockIdx.x) * 256 + col;
     const bool ok = gc < F8 * 8;
 #pragma unroll
-    for (int p = 0; p < NP; ++p) cluster_colsum_apply(&part[p][col], dbias + (ok ? p * F8 * 8 + gc : 0), ok, 1.f);
+    for (int p = 0; p < NP; ++p) cluster_colsum_apply(&part[p][col], dbias_seg + (ok ? p * F8 * 8 + gc : 0), ok, 1.f);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -995,16 +1016,17 @@ __global__ void ce_mean_kernel(const float* __restrict__ loss_tok, int64_t T, co
 
 // ------------------------------------------------------------------------------------------
 // column sums: grid (col tiles of 256 columns, row splits = one cluster).  each thread owns 8 columns (one 16-B vector)
-// of 32 lanes; 8 warps stride rows; smem combine; row splits combined in a fixed order (cluster_colsum_apply).
+// of 32 lanes; 8 warps stride rows; smem combine; row splits combined in a fixed order (cluster_colsum_apply).  With a
+// segment table, grid z enumerates the segments (segment_rows): per-expert bias gradients of grouped MoE rows.
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kThreads)
     colsum_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx, float* __restrict__ out, int64_t T, int64_t N,
-                  int rows_per_block, float scale) {
+                  int rows_per_block, float scale, const int* __restrict__ seg, int64_t out_seg_stride) {
     __shared__ float sm[8][256];
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     const int64_t col = int64_t(blockIdx.x) * 256 + lane * 8;
-    const int64_t r0 = int64_t(blockIdx.y) * rows_per_block;
-    const int64_t r1 = min(T, r0 + rows_per_block);
+    int64_t r0, r1;
+    float* const out_seg = out + segment_rows(seg, T, rows_per_block, out_seg_stride, r0, r1);
     float acc[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) acc[j] = 0.f;
@@ -1027,7 +1049,7 @@ __global__ void __launch_bounds__(kThreads)
     part[c] = s;
     const int64_t gc = int64_t(blockIdx.x) * 256 + c;
     const bool ok = gc < N;
-    cluster_colsum_apply(&part[c], out + (ok ? gc : 0), ok, scale);
+    cluster_colsum_apply(&part[c], out_seg + (ok ? gc : 0), ok, scale);
 }
 
 __global__ void __launch_bounds__(kThreads) add_scaled_kernel(const uint4* __restrict__ a, const uint4* __restrict__ b,
@@ -1405,9 +1427,11 @@ void launch_act_fwd(int form, const void* x, void* y, int64_t T, int64_t F8, cud
     }
 }
 
+// seg / segments: segment table of the rows (NULL: the dense launch, one segment of T rows); dbias_seg_stride floats
+// between the bias-gradient rows of consecutive segments
 template <class Op, bool Glu>
 cudaError_t launch_act_bwd_form(const void* dy, const void* x, void* dx, float* dbias, int64_t T, int64_t F8,
-                                cudaStream_t st) {
+                                const int* seg, int segments, int64_t dbias_seg_stride, cudaStream_t st) {
     auto DY = static_cast<const uint4*>(dy);
     auto X = static_cast<const uint4*>(x);
     auto DX = static_cast<uint4*>(dx);
@@ -1417,8 +1441,8 @@ cudaError_t launch_act_bwd_form(const void* dy, const void* x, void* dx, float* 
     }
     const int col_tiles = int((F8 + 31) / 32);
     const int rows_per_block = int((T + kColsumCluster - 1) / kColsumCluster);  // one cluster of row splits per column tile
-    return cudaError_t(launch_row_cluster(act_bwd_bias_kernel<Op, Glu>, col_tiles, st, DY, X, DX, dbias, T, F8,
-                                          rows_per_block));
+    return cudaError_t(launch_row_cluster(act_bwd_bias_kernel<Op, Glu>, col_tiles, segments, st, DY, X, DX, dbias, T, F8,
+                                          rows_per_block, seg, dbias_seg_stride));
 }
 
 int check_act(const char* what, int act_id, int form, int64_t F) {
@@ -1451,8 +1475,30 @@ extern "C" int dolomite_b200_act_bwd(int act_id, int form, const void* dy, const
     visit_act(act_id, [&](auto op) {
         using Op = decltype(op);
         const cudaStream_t st = static_cast<cudaStream_t>(stream);
-        e = form == DOLO_ACT_PLAIN ? launch_act_bwd_form<Op, false>(dy, x, dx, dbias_accum, T, F / 8, st)
-                                   : launch_act_bwd_form<Op, true>(dy, x, dx, dbias_accum, T, F / 8, st);
+        e = form == DOLO_ACT_PLAIN ? launch_act_bwd_form<Op, false>(dy, x, dx, dbias_accum, T, F / 8, nullptr, 1, 0, st)
+                                   : launch_act_bwd_form<Op, true>(dy, x, dx, dbias_accum, T, F / 8, nullptr, 1, 0, st);
+    });
+    DOLO_CUDA_OK(e);
+    return DOLO_OK;
+}
+
+extern "C" int dolomite_b200_act_bwd_segmented(int act_id, int form, const void* dy, const void* x, void* dx,
+                                               float* dbias_accum, int64_t ld_dbias, int64_t F,
+                                               const int32_t* seg_offsets, int num_segments, void* stream) {
+    if (const int rc = check_act("act_bwd_segmented", act_id, form, F)) return rc;
+    DOLO_REQUIRE(aligned16(x) && aligned16(dy) && aligned16(dx), "act_bwd_segmented: pointers must be 16-byte aligned");
+    DOLO_REQUIRE(dbias_accum != nullptr && seg_offsets != nullptr && num_segments > 0 && num_segments <= 65535,
+                 "act_bwd_segmented: bias gradient, segment table and 1..65535 segments needed");
+    const int64_t fc_out = form == DOLO_ACT_PLAIN ? F : 2 * F;
+    DOLO_REQUIRE(ld_dbias >= fc_out, "act_bwd_segmented: ld_dbias=%lld < %lld columns", (long long)ld_dbias,
+                 (long long)fc_out);
+    cudaError_t e = cudaSuccess;
+    visit_act(act_id, [&](auto op) {
+        using Op = decltype(op);
+        const cudaStream_t st = static_cast<cudaStream_t>(stream);
+        e = form == DOLO_ACT_PLAIN
+                ? launch_act_bwd_form<Op, false>(dy, x, dx, dbias_accum, 0, F / 8, seg_offsets, num_segments, ld_dbias, st)
+                : launch_act_bwd_form<Op, true>(dy, x, dx, dbias_accum, 0, F / 8, seg_offsets, num_segments, ld_dbias, st);
     });
     DOLO_CUDA_OK(e);
     return DOLO_OK;
@@ -1576,9 +1622,24 @@ extern "C" int dolomite_b200_colsum_accum(const void* x, int64_t ldx, float* out
     if (T == 0) return DOLO_OK;
     const int col_tiles = int((N + 255) / 256);
     const int rows_per_block = int((T + kColsumCluster - 1) / kColsumCluster);  // one cluster of row splits per column tile
-    DOLO_CUDA_OK(cudaError_t(launch_row_cluster(colsum_kernel, col_tiles, static_cast<cudaStream_t>(stream),
+    DOLO_CUDA_OK(cudaError_t(launch_row_cluster(colsum_kernel, col_tiles, 1, static_cast<cudaStream_t>(stream),
                                                 static_cast<const __nv_bfloat16*>(x), ldx, out, T, N, rows_per_block,
-                                                scale)));
+                                                scale, static_cast<const int*>(nullptr), int64_t(0))));
+    return DOLO_OK;
+}
+
+extern "C" int dolomite_b200_colsum_accum_segmented(const void* x, int64_t ldx, float* out, int64_t ld_out, int64_t N,
+                                                    const int32_t* seg_offsets, int num_segments, float scale,
+                                                    void* stream) {
+    DOLO_REQUIRE(N > 0 && N % 8 == 0 && ldx % 8 == 0, "colsum_segmented: N=%lld / ld=%lld must be multiples of 8",
+                 (long long)N, (long long)ldx);
+    DOLO_REQUIRE(aligned16(x), "colsum_segmented: pointer must be 16-byte aligned");
+    DOLO_REQUIRE(seg_offsets != nullptr && num_segments > 0 && num_segments <= 65535 && ld_out >= N,
+                 "colsum_segmented: segment table, 1..65535 segments and ld_out >= N needed");
+    const int col_tiles = int((N + 255) / 256);
+    DOLO_CUDA_OK(cudaError_t(launch_row_cluster(colsum_kernel, col_tiles, num_segments, static_cast<cudaStream_t>(stream),
+                                                static_cast<const __nv_bfloat16*>(x), ldx, out, int64_t(0), N, 0, scale,
+                                                static_cast<const int*>(seg_offsets), ld_out)));
     return DOLO_OK;
 }
 

@@ -104,6 +104,7 @@ struct GemmParams {
     int b_group_rows;
     const int* group_k_offsets;
     int num_groups;
+    int64_t bias_group_stride;  // M-grouped: group g reads its bias row at pr.bias + g * bias_group_stride (0: dense)
     const float* a_scale_inv[MAXP];  // fp8: scale_inv of A and of B per problem (device scalars)
     const float* b_scale_inv[MAXP];
 };
@@ -512,14 +513,16 @@ __device__ __forceinline__ void gemm_body(const GemmMaps& maps, const GemmParams
         }
         const bool has_bias = pr.bias != nullptr;
         const bool has_c = pr.C != nullptr;
-        // the tile's bias slice: loaded now, kept in shared memory for the epilogue.  An odd N ends in a half pair, whose
-        // upper element (column N) is not read; its value only ever reaches the clipped column N of the slab.
+        // the tile's bias slice (of the tile's group's bias row in the M-grouped mode): loaded now, kept in shared memory
+        // for the epilogue.  An odd N ends in a half pair, whose upper element (column N) is not read; its value only ever
+        // reaches the clipped column N of the slab.
         uint32_t bias_v = 0;
         if (has_bias && wt < TN / 2 && col0 + 2 * wt < pr.N) {
+            const __nv_bfloat16* brow = pr.bias + ti.grp * p.bias_group_stride;
             if (col0 + 2 * wt + 1 < pr.N)
-                bias_v = __ldg(reinterpret_cast<const uint32_t*>(pr.bias + col0 + 2 * wt));
+                bias_v = __ldg(reinterpret_cast<const uint32_t*>(brow + col0 + 2 * wt));
             else
-                bias_v = __bfloat16_as_ushort(pr.bias[col0 + 2 * wt]);
+                bias_v = __bfloat16_as_ushort(brow[col0 + 2 * wt]);
         }
         int prev_stage = -1;
         for (int kb = ti.kb0; kb < ti.kb1; ++kb) {
@@ -654,6 +657,7 @@ struct GroupArgs {
     int num_groups = 1;
     int64_t d_group_stride = 0;
     int64_t b_total_outer = 0;  // rows of B's outer TMA dimension over all groups
+    int64_t bias_group_stride = 0;  // mode 1 with bias: elements between the bias rows of consecutive groups
 };
 
 // one problem of a launch
@@ -837,6 +841,7 @@ static int gemm_impl(const void* A, int64_t lda, int a_mn_major, const void* B, 
     p.b_group_rows = int(ga.b_group_rows);
     p.group_k_offsets = ga.group_k_offsets;
     p.num_groups = ga.num_groups;
+    p.bias_group_stride = ga.bias_group_stride;
     return dispatch(tile_n, a_mn_major, b_mn_major, maps, p, static_cast<cudaStream_t>(stream));
 }
 
@@ -909,44 +914,68 @@ extern "C" int dolomite_b200_gemm_bf16(const void* A, int64_t lda, int a_mn_majo
                      stream, GroupArgs());
 }
 
-extern "C" int dolomite_b200_gemm_bf16_grouped_m(const void* A, int64_t lda, const void* B, int64_t ldb, int b_mn_major,
-                                                 void* D, int64_t ldd, float alpha, int64_t M_max, int64_t N, int64_t K,
-                                                 const int32_t* m_tile_group, int num_groups, int flags, void* stream) {
+// M-grouped expert GEMM (fwd / dgrad of the expert linears), with the gather fused into the operand load when a_row_index
+// is given (A is then the UNGROUPED activation matrix [a_rows, K] and a_row_index[r] names the source row of grouped row r;
+// padding rows may name any valid row: their products are never read), and with a per-group bias row
+// bias[g * ld_bias .. + N) added to group g's rows when bias is given.
+static int grouped_m_impl(const void* A, int64_t lda, int64_t a_rows, const int32_t* a_row_index, const void* B,
+                          int64_t ldb, int b_mn_major, void* D, int64_t ldd, const void* bias, int64_t ld_bias,
+                          float alpha, int64_t M_max, int64_t N, int64_t K, const int32_t* m_tile_group, int num_groups,
+                          int flags, void* stream) {
     DOLO_REQUIRE(M_max % BM == 0, "grouped gemm: M_max=%lld must be a multiple of %d (padded expert segments)",
                  (long long)M_max, BM);
     DOLO_REQUIRE(!b_mn_major || K % BK == 0, "grouped gemm: MN-major B needs K %% %d == 0", BK);
     DOLO_REQUIRE(m_tile_group != nullptr && num_groups > 0, "grouped gemm: missing group table");
-    GroupArgs ga;
-    ga.mode = 1;
-    ga.m_tile_group = m_tile_group;
-    ga.num_groups = num_groups;
-    ga.b_group_rows = b_mn_major ? K : N;
-    ga.b_total_outer = ga.b_group_rows * num_groups;
-    return gemm_impl(A, lda, 0, B, ldb, b_mn_major, D, ldd, 0, nullptr, 0, alpha, 0.f, nullptr, M_max, N, K, flags, stream,
-                     ga);
-}
-
-// Same, with the ScatterMoE gather fused into the operand load: A is the UNGROUPED activation matrix [a_rows, K] and
-// a_row_index[r] names the source row of grouped row r (padding rows may name any valid row: their products are never read)
-extern "C" int dolomite_b200_gemm_bf16_grouped_m_gather(const void* A, int64_t lda, int64_t a_rows,
-                                                        const int32_t* a_row_index, const void* B, int64_t ldb, void* D,
-                                                        int64_t ldd, float alpha, int64_t M_max, int64_t N, int64_t K,
-                                                        const int32_t* m_tile_group, int num_groups, int flags,
-                                                        void* stream) {
-    DOLO_REQUIRE(M_max % BM == 0, "grouped gemm: M_max=%lld must be a multiple of %d (padded expert segments)",
-                 (long long)M_max, BM);
-    DOLO_REQUIRE(m_tile_group != nullptr && num_groups > 0 && a_row_index != nullptr && a_rows > 0,
-                 "grouped gemm (gather): missing group table / row index");
-    DOLO_REQUIRE((reinterpret_cast<uintptr_t>(a_row_index) & 15) == 0, "grouped gemm (gather): row index must be 16-byte aligned");
+    if (a_row_index != nullptr) {
+        DOLO_REQUIRE(!b_mn_major && a_rows > 0, "grouped gemm (gather): K-major B and a_rows > 0 needed");
+        DOLO_REQUIRE((reinterpret_cast<uintptr_t>(a_row_index) & 15) == 0,
+                     "grouped gemm (gather): row index must be 16-byte aligned");
+    }
+    // every group's bias row must keep the 4-byte alignment of the epilogue's paired loads
+    DOLO_REQUIRE(bias == nullptr || (ld_bias >= N && ld_bias % 2 == 0),
+                 "grouped gemm: ld_bias=%lld must be even and >= N=%lld", (long long)ld_bias, (long long)N);
     GroupArgs ga;
     ga.mode = 1;
     ga.a_row_index = a_row_index;
     ga.a_rows = a_rows;
     ga.m_tile_group = m_tile_group;
     ga.num_groups = num_groups;
-    ga.b_group_rows = N;
-    ga.b_total_outer = N * num_groups;
-    return gemm_impl(A, lda, 0, B, ldb, 0, D, ldd, 0, nullptr, 0, alpha, 0.f, nullptr, M_max, N, K, flags, stream, ga);
+    ga.b_group_rows = b_mn_major ? K : N;
+    ga.b_total_outer = ga.b_group_rows * num_groups;
+    ga.bias_group_stride = bias != nullptr ? ld_bias : 0;
+    return gemm_impl(A, lda, 0, B, ldb, b_mn_major, D, ldd, 0, nullptr, 0, alpha, 0.f, bias, M_max, N, K, flags, stream,
+                     ga);
+}
+
+extern "C" int dolomite_b200_gemm_bf16_grouped_m(const void* A, int64_t lda, const void* B, int64_t ldb, int b_mn_major,
+                                                 void* D, int64_t ldd, float alpha, int64_t M_max, int64_t N, int64_t K,
+                                                 const int32_t* m_tile_group, int num_groups, int flags, void* stream) {
+    return grouped_m_impl(A, lda, 0, nullptr, B, ldb, b_mn_major, D, ldd, nullptr, 0, alpha, M_max, N, K, m_tile_group,
+                          num_groups, flags, stream);
+}
+
+// Same, with the ScatterMoE gather fused into the operand load
+extern "C" int dolomite_b200_gemm_bf16_grouped_m_gather(const void* A, int64_t lda, int64_t a_rows,
+                                                        const int32_t* a_row_index, const void* B, int64_t ldb, void* D,
+                                                        int64_t ldd, float alpha, int64_t M_max, int64_t N, int64_t K,
+                                                        const int32_t* m_tile_group, int num_groups, int flags,
+                                                        void* stream) {
+    DOLO_REQUIRE(a_row_index != nullptr, "grouped gemm (gather): missing row index");
+    return grouped_m_impl(A, lda, a_rows, a_row_index, B, ldb, 0, D, ldd, nullptr, 0, alpha, M_max, N, K, m_tile_group,
+                          num_groups, flags, stream);
+}
+
+// Expert linears with bias (moe/base.py:12-50 ParameterizedExperts with add_bias): D = (A W[g]^T + bias[g]) * alpha, plain
+// (a_row_index NULL) or gather-on-load
+extern "C" int dolomite_b200_gemm_bf16_grouped_m_bias(const void* A, int64_t lda, int64_t a_rows,
+                                                      const int32_t* a_row_index, const void* B, int64_t ldb,
+                                                      int b_mn_major, void* D, int64_t ldd, const void* bias,
+                                                      int64_t ld_bias, float alpha, int64_t M_max, int64_t N, int64_t K,
+                                                      const int32_t* m_tile_group, int num_groups, int flags,
+                                                      void* stream) {
+    DOLO_REQUIRE(bias != nullptr, "grouped gemm (bias): missing bias");
+    return grouped_m_impl(A, lda, a_rows, a_row_index, B, ldb, b_mn_major, D, ldd, bias, ld_bias, alpha, M_max, N, K,
+                          m_tile_group, num_groups, flags, stream);
 }
 
 extern "C" int dolomite_b200_gemm_bf16_grouped_k(const void* A, int64_t lda, const void* B, int64_t ldb, float* D,

@@ -191,10 +191,11 @@ def _root_specs(cfg: CommonConfig) -> list[tuple[str, tuple, str]]:
 
 
 def check_supported(cfg: CommonConfig, *, attention_implementation: str = "flash_attention_2",
-                    use_padding_free_transformer: bool = True) -> None:
+                    use_padding_free_transformer: bool = True, moe_implementation: str = "eager") -> None:
     """The B200 hot path implements the configurations SURVEY.md section 8 puts in scope; everything else raises
     (mirrors the reference's NotImplementedError / ValueError conventions, SURVEY section 8b).  The keyword arguments are
-    the model's `attn_implementation` / `use_padding_free_transformer`; only alibi depends on them."""
+    the model's `attn_implementation` / `use_padding_free_transformer` / `moe_implementation`; only alibi and MoE expert
+    biases depend on them."""
     if cfg.position_embedding_type not in ("rope", "nope", "learned_absolute", "alibi"):
         raise NotImplementedError(
             f"position_embedding_type={cfg.position_embedding_type!r}: the B200 path implements rope, nope, "
@@ -229,8 +230,9 @@ def check_supported(cfg: CommonConfig, *, attention_implementation: str = "flash
     if cfg.model_type == "moe_dolomite":
         if cfg.num_experts % 8 or not (1 <= cfg.num_experts_per_tok <= min(8, cfg.num_experts)):
             raise NotImplementedError("MoE: num_experts must be a multiple of 8 (<= 256) and 1 <= top-k <= 8")
-        if cfg.add_bias:
-            raise NotImplementedError("MoE experts with bias are not supported (ScatterMoE asserts the same, moe/scatter.py:22)")
+        if cfg.add_bias and moe_implementation == "scattermoe":
+            # the reference's ScatterMoE asserts this (moe/scatter.py:22); its eager experts carry the bias
+            raise AssertionError("scattermoe doesn't support bias")
         if cfg.n_inner % 64 or cfg.n_embd % 64:
             raise NotImplementedError("MoE: n_embd and n_inner must be multiples of 64 (grouped GEMM K tiles)")
     # vocab_size may be any value: [T, V] logits live in buffers with 16-byte row strides (kernels.rows_empty)
@@ -243,9 +245,9 @@ class DolomiteEngine:
 
     def __init__(self, cfg: CommonConfig, device, world_size: int = 1, rank: int = 0, seed: int | None = 42,
                  init_on_device: bool = False, attention_implementation: str = "flash_attention_2",
-                 use_padding_free_transformer: bool = True):
+                 use_padding_free_transformer: bool = True, moe_implementation: str = "eager"):
         check_supported(cfg, attention_implementation=attention_implementation,
-                        use_padding_free_transformer=use_padding_free_transformer)
+                        use_padding_free_transformer=use_padding_free_transformer, moe_implementation=moe_implementation)
         self.cfg = cfg
         self.device = torch.device(device)
         self.world_size, self.rank = world_size, rank

@@ -138,7 +138,7 @@ class DolomitePreTrainedModel(nn.Module):
         self.attention_implementation = kwargs.pop("attn_implementation", "flash_attention_2")
         self._use_padding_free_transformer = kwargs.pop("use_padding_free_transformer", True)
         self.normalization_implementation = kwargs.pop("normalization_implementation", "torch")
-        self.moe_implementation = kwargs.pop("moe_implementation", "scattermoe")
+        self.moe_implementation = kwargs.pop("moe_implementation", "eager")  # moe_dolomite/base.py:21
         kwargs.pop("torch_dtype", None)
         kwargs.pop("trust_remote_code", None)
         device = kwargs.pop("device", None)
@@ -166,7 +166,8 @@ class DolomitePreTrainedModel(nn.Module):
             device = torch.device("cuda", torch.cuda.current_device())
         self.engine = DolomiteEngine(config, device, world_size=world_size, rank=rank, seed=seed, init_on_device=init_on_device,
                                      attention_implementation=self.attention_implementation,
-                                     use_padding_free_transformer=self._use_padding_free_transformer)
+                                     use_padding_free_transformer=self._use_padding_free_transformer,
+                                     moe_implementation=self.moe_implementation)
         self.flat_params = nn.ParameterList([u.master for u in self.engine.units])
         self._anchor = torch.zeros(1, device=device, requires_grad=True)
         self.assume_unit_loss_grad = False

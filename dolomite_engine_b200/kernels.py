@@ -169,6 +169,22 @@ def act_bwd(dy, x, act_id: int, form: int, out=None, bias_grad_accum=None):
     return dx
 
 
+def act_bwd_segmented(dy, x, act_id: int, form: int, seg_offsets, bias_grad_accum, out=None):
+    """act_bwd on the rows of the segments [seg_offsets[s], seg_offsets[s + 1]) (int32 device table, e.g. a MoE plan's
+    offsets); bias_grad_accum fp32 [segments, columns of x]: row s += column sums of segment s's dx.  Rows outside every
+    segment are not written."""
+    _req(dy, _BF16, "dy"), _req(x, _BF16, "x"), _req(bias_grad_accum, torch.float32, "bias_grad_accum")
+    _req(seg_offsets, torch.int32, "seg_offsets")
+    T, W = x.shape
+    S = seg_offsets.numel() - 1
+    assert bias_grad_accum.dim() == 2 and bias_grad_accum.shape == (S, W) and bias_grad_accum.stride(1) == 1
+    dx = torch.empty_like(x) if out is None else out
+    _lib.call("dolomite_b200_act_bwd_segmented", act_id, form, dy.data_ptr(), x.data_ptr(), dx.data_ptr(),
+              bias_grad_accum.data_ptr(), bias_grad_accum.stride(0), W if form == 0 else W // 2, seg_offsets.data_ptr(), S,
+              _stream())
+    return dx
+
+
 def gelu_fwd(x, out=None):
     _req(x, _BF16, "x")
     y = torch.empty_like(x) if out is None else out
@@ -272,6 +288,17 @@ def colsum_accum(x, out, scale: float = 1.0):
     _req(x, _BF16, "x"), _req(out, torch.float32, "out")
     T, N = x.shape
     _lib.call("dolomite_b200_colsum_accum", x.data_ptr(), x.stride(0), out.data_ptr(), T, N, scale, _stream())
+
+
+def colsum_accum_segmented(x, seg_offsets, out, scale: float = 1.0):
+    """out[s] += scale * column sums of x over the rows [seg_offsets[s], seg_offsets[s + 1]) (int32 device table);
+    out fp32 [segments, N]"""
+    _req(x, _BF16, "x"), _req(out, torch.float32, "out"), _req(seg_offsets, torch.int32, "seg_offsets")
+    T, N = x.shape
+    S = seg_offsets.numel() - 1
+    assert out.dim() == 2 and out.shape == (S, N) and out.stride(1) == 1 and x.stride(1) == 1
+    _lib.call("dolomite_b200_colsum_accum_segmented", x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), N,
+              seg_offsets.data_ptr(), S, scale, _stream())
 
 
 def scale_by_device_scalar(x, scale):
@@ -795,8 +822,15 @@ def moe_router_bwd_aux(router_logits, plan: MoEPlan, dw, c, s, T_real: int):
     return dl
 
 
-def gemm_grouped_m(a, w3, plan: MoEPlan, *, b_mn: bool, alpha: float = 1.0, flags=None):
-    """rows of `a` grouped by expert.  b_mn=False: w3 [E, N, K] -> D = A W[e]^T;  b_mn=True: w3 [E, K, N] -> D = A W[e]"""
+def _expert_bias(bias, E: int, N: int):
+    _req(bias, _BF16, "bias")
+    assert bias.shape == (E, N) and bias.stride(1) == 1, (tuple(bias.shape), E, N)
+    return bias
+
+
+def gemm_grouped_m(a, w3, plan: MoEPlan, *, b_mn: bool, alpha: float = 1.0, flags=None, bias=None):
+    """rows of `a` grouped by expert.  b_mn=False: w3 [E, N, K] -> D = A W[e]^T;  b_mn=True: w3 [E, K, N] -> D = A W[e].
+    bias bf16 [E, N]: D = (A W[e]^T + bias[e]) * alpha on expert e's rows"""
     _req(a, _BF16, "a"), _req(w3, _BF16, "w3")
     rows, K = a.shape
     E = w3.shape[0]
@@ -805,14 +839,21 @@ def gemm_grouped_m(a, w3, plan: MoEPlan, *, b_mn: bool, alpha: float = 1.0, flag
     out = torch.empty(rows, N, dtype=_BF16, device=a.device)
     if flags is None:
         flags = _default_gemm_flags
+    if bias is not None:
+        bias = _expert_bias(bias, E, N)
+        _lib.call("dolomite_b200_gemm_bf16_grouped_m_bias", a.data_ptr(), a.stride(0), 0, None, w3.data_ptr(), w3.shape[2],
+                  int(b_mn), out.data_ptr(), N, bias.data_ptr(), bias.stride(0), alpha, rows, N, K,
+                  plan.tile_group.data_ptr(), E, flags, _stream())
+        return out
     _lib.call("dolomite_b200_gemm_bf16_grouped_m", a.data_ptr(), a.stride(0), w3.data_ptr(), w3.shape[2], int(b_mn),
               out.data_ptr(), N, alpha, rows, N, K, plan.tile_group.data_ptr(), E, flags, _stream())
     return out
 
 
-def gemm_grouped_m_gather(x, w3, plan: MoEPlan, alpha: float = 1.0, flags=None):
+def gemm_grouped_m_gather(x, w3, plan: MoEPlan, alpha: float = 1.0, flags=None, bias=None):
     """expert forward with the gather fused into the operand load (rows copied by the producer warp): x [T, K] UNGROUPED, w3 [E, N, K] ->
-    D[row] = x[token_of_row[row]] W[expert(row)]^T for every grouped row (moe/scatter.py:38-49 `parallel_linear`)"""
+    D[row] = x[token_of_row[row]] W[expert(row)]^T (+ bias[expert(row)]) for every grouped row (moe/scatter.py:38-49
+    `parallel_linear`)"""
     _req(x, _BF16, "x"), _req(w3, _BF16, "w3")
     T, K = x.shape
     E, N = w3.shape[0], w3.shape[1]
@@ -823,9 +864,15 @@ def gemm_grouped_m_gather(x, w3, plan: MoEPlan, alpha: float = 1.0, flags=None):
     if gemm_timer is not None:
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-    _lib.call("dolomite_b200_gemm_bf16_grouped_m_gather", x.data_ptr(), x.stride(0), T, plan.token_of_row.data_ptr(),
-              w3.data_ptr(), w3.shape[2], out.data_ptr(), N, alpha, plan.max_rows, N, K, plan.tile_group.data_ptr(), E, flags,
-              _stream())
+    if bias is not None:
+        bias = _expert_bias(bias, E, N)
+        _lib.call("dolomite_b200_gemm_bf16_grouped_m_bias", x.data_ptr(), x.stride(0), T, plan.token_of_row.data_ptr(),
+                  w3.data_ptr(), w3.shape[2], 0, out.data_ptr(), N, bias.data_ptr(), bias.stride(0), alpha, plan.max_rows,
+                  N, K, plan.tile_group.data_ptr(), E, flags, _stream())
+    else:
+        _lib.call("dolomite_b200_gemm_bf16_grouped_m_gather", x.data_ptr(), x.stride(0), T, plan.token_of_row.data_ptr(),
+                  w3.data_ptr(), w3.shape[2], out.data_ptr(), N, alpha, plan.max_rows, N, K, plan.tile_group.data_ptr(), E,
+                  flags, _stream())
     if gemm_timer is not None:
         e1.record()
         gemm_timer.append((2.0 * T * plan.k * N * K, e0, e1))

@@ -6,12 +6,18 @@ ScatterMoE, moe_dolomite/layer.py:51-95 SparseMoEBlock).
     activations.resolve accepts) -> grouped GEMM c_proj -> gate-weighted combine (+ m_residual scale + residual add fused)
 
 Padding rows of a segment are zeros in the gathered input (or a copy of token 0's row with the fused gather), so their
-`act` rows are finite but not zero for functions with f(0) != 0 (sigmoid, softplus, hard_sigmoid, laplace, log_sigmoid).
-They never reach a result: the combine reads only the rows of `row_of_slot`, and the combine backward writes zero `dyg`
-rows for them, so they add exact zeros to the c_proj weight gradient and give zero `d_fc` rows to the c_fc one.
+`act` rows are finite but not zero for functions with f(0) != 0 (sigmoid, softplus, hard_sigmoid, laplace, log_sigmoid),
+and with expert biases their `fc` rows are the bias (plus the copied row's product).  They never reach a result: the
+combine reads only the rows of `row_of_slot`, and the combine backward writes zero `dyg` rows for them, so they add exact
+zeros to the c_proj weight gradient and give zero `d_fc` rows to the c_fc one.
 
-ScatterMoE forbids biases (moe/scatter.py:22); so does this path.  Activations stay grouped between the two expert
-GEMMs exactly like `parallel_linear(grouped_out=True)` -> `parallel_linear(grouped_in=True, gates=...)`.
+Expert biases (ParameterizedExperts with add_bias, moe/base.py:12-50; the reference's `eager` experts -- ScatterMoE
+forbids them, moe/scatter.py:22): bias[e] is added in the grouped GEMMs' fp32 epilogue on expert e's rows, one rounding to
+bf16 as in the dense biased linear.  Their gradients are per-segment column sums over the padded expert segments
+`plan.offsets` (whose padding rows add exact zeros): d c_proj.bias[e] of `dyg` (which carries the gate weight and
+m_residual), d c_fc.bias[e] of `d_fc`, fused into the activation backward.  Both reduce in a fixed order with no float
+atomics, and an expert without tokens adds exact zeros.  Activations stay grouped between the two expert GEMMs exactly
+like `parallel_linear(grouped_out=True)` -> `parallel_linear(grouped_in=True, gates=...)`.
 """
 
 from __future__ import annotations
@@ -28,8 +34,7 @@ FUSED_GATHER = os.environ.get("DOLO_MOE_FUSED_GATHER", "0") == "1"
 def forward(engine, unit, p: str, x, residual, m_res: float, layer: int = 0):
     cfg = engine.cfg
     k = cfg.num_experts_per_tok
-    if (p + "mlp.c_fc.bias") in unit.views:
-        raise NotImplementedError("expert biases are not supported by the grouped-GEMM MoE path (moe/scatter.py:22)")
+    b_fc, b_proj = unit.views.get(p + "mlp.c_fc.bias"), unit.views.get(p + "mlp.c_proj.bias")
     logits = engine._linear(unit, p + "mlp.gate.weight", x, flags=0)  # [T, E] bf16 (tiny N: direct-store epilogue)
     plan = K.moe_route(logits, k)
     if engine._aux_fwd is not None:  # load-balancing statistics of this layer (once per forward: not in recomputed blocks)
@@ -39,11 +44,11 @@ def forward(engine, unit, p: str, x, residual, m_res: float, layer: int = 0):
     if FUSED_GATHER:
         # scattermoe `parallel_linear(grouped_in=False, grouped_out=True)`: the expert GEMM reads the token rows straight
         # out of x (copied by its producer warp); no grouped copy of x is written in forward
-        fc = K.gemm_grouped_m_gather(x, unit.views[p + "mlp.c_fc.weight"], plan)
+        fc = K.gemm_grouped_m_gather(x, unit.views[p + "mlp.c_fc.weight"], plan, bias=b_fc)
     else:
-        fc = K.gemm_grouped_m(K.moe_gather(x, plan), unit.views[p + "mlp.c_fc.weight"], plan, b_mn=False)
+        fc = K.gemm_grouped_m(K.moe_gather(x, plan), unit.views[p + "mlp.c_fc.weight"], plan, b_mn=False, bias=b_fc)
     act = K.act_fwd(fc, *engine.act)
-    yg = K.gemm_grouped_m(act, unit.views[p + "mlp.c_proj.weight"], plan, b_mn=False)
+    yg = K.gemm_grouped_m(act, unit.views[p + "mlp.c_proj.weight"], plan, b_mn=False, bias=b_proj)
     p_res = engine._drop_p("resid_pdrop")
     if p_res > 0:  # moe/base.py:106-120: dropout on the combined expert output, then layer.py's `* m_residual` / `+ residual`
         y = K.moe_combine(yg, plan)
@@ -67,8 +72,16 @@ def backward(engine, unit, p: str, x, dh, m_res: float, saved, layer: int = 0):
     beta_proj = 0.0 if engine.take_fresh(p + "mlp.c_proj.weight") else 1.0
     beta_fc = 0.0 if engine.take_fresh(p + "mlp.c_fc.weight") else 1.0
     K.gemm_grouped_k(dyg, act, plan, unit.gviews[p + "mlp.c_proj.weight"], beta=beta_proj)  # dWproj[e] (+)= dY_e^T act_e
+    # expert biases: their gradient buffers are cleared by zero_grad (not lazily), so the segment sums accumulate; dyg
+    # already holds m_residual (the dense c_proj's colsum alpha)
+    gb_fc, gb_proj = unit.gviews.get(p + "mlp.c_fc.bias"), unit.gviews.get(p + "mlp.c_proj.bias")
+    if gb_proj is not None:
+        K.colsum_accum_segmented(dyg, plan.offsets, gb_proj)                          # dbproj[e] += sum of dY_e rows
     d_act = K.gemm_grouped_m(dyg, w_proj, plan, b_mn=True)                            # [rows, F]
-    d_fc = K.act_bwd(d_act, fc, *engine.act)
+    if gb_fc is not None:  # dbfc[e] += sum of d_fc_e rows, fused into the activation backward
+        d_fc = K.act_bwd_segmented(d_act, fc, *engine.act, plan.offsets, gb_fc)
+    else:
+        d_fc = K.act_bwd(d_act, fc, *engine.act)
     xg = K.moe_gather(x, plan)  # grouped (zero-padded) copy of the block input: the contraction operand of the c_fc wgrad
     K.gemm_grouped_k(d_fc, xg, plan, unit.gviews[p + "mlp.c_fc.weight"], beta=beta_fc)  # dWfc[e] (+)= dfc_e^T x_e
     del xg

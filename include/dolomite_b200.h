@@ -133,6 +133,13 @@ enum { DOLO_ACT_PLAIN = 0, DOLO_ACT_GLU = 1, DOLO_ACT_SIGMOID_GLU = 2 };
 int dolomite_b200_act_fwd(int act_id, int form, const void* x, void* y, int64_t T, int64_t F, void* stream);
 int dolomite_b200_act_bwd(int act_id, int form, const void* dy, const void* x, void* dx, float* dbias_accum, int64_t T,
                           int64_t F, void* stream);
+/* act_bwd on rows grouped into segments (MoE expert rows): segment s is rows [seg_offsets[s], seg_offsets[s+1]) (int32
+ * device table of num_segments + 1 entries, e.g. the offsets_padded of moe_route), dx is written on those rows only, and
+ * row s of dbias_accum (fp32 [num_segments, ld_dbias]) += the column sums of the segment's bf16 dx, in the fixed order of
+ * the dense launch.  An empty segment adds exact zeros. */
+int dolomite_b200_act_bwd_segmented(int act_id, int form, const void* dy, const void* x, void* dx, float* dbias_accum,
+                                    int64_t ld_dbias, int64_t F, const int32_t* seg_offsets, int num_segments,
+                                    void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * tanh-GELU -- activation_function "gelu_pytorch_tanh" (hf_models/modeling_utils/activations/base.py), the non-GLU MLP
@@ -194,6 +201,11 @@ int dolomite_b200_cross_entropy_mean(const float* loss_per_token, int64_t T, con
  * ------------------------------------------------------------------------------------------------ */
 int dolomite_b200_colsum_accum(const void* x, int64_t ldx, float* out, int64_t T, int64_t N, float scale,
                                void* stream);
+/* Per-segment column sums (bias gradient of the MoE expert linears): out[s * ld_out + n] += scale * sum of x[t, n] over
+ * the rows t of segment s, [seg_offsets[s], seg_offsets[s+1]) (int32 device table of num_segments + 1 entries).  Same
+ * summation order per segment as colsum_accum over those rows; no float atomics; an empty segment adds exact zeros. */
+int dolomite_b200_colsum_accum_segmented(const void* x, int64_t ldx, float* out, int64_t ld_out, int64_t N,
+                                         const int32_t* seg_offsets, int num_segments, float scale, void* stream);
 /* x[i] *= scale[0]  (bf16 in place; scale is a DEVICE scalar: the upstream gradient autograd hands to the loss when the
  * caller does anything but `loss.backward()`, train_utils.py:61-90) */
 int dolomite_b200_scale_bf16_by_device_scalar(void* x, int64_t n, const float* scale, void* stream);
@@ -362,6 +374,15 @@ int dolomite_b200_gemm_bf16_grouped_m_gather(const void* A, int64_t lda, int64_t
                                              const void* B, int64_t ldb, void* D, int64_t ldd, float alpha, int64_t M_max,
                                              int64_t N, int64_t K, const int32_t* m_tile_group, int num_groups, int flags,
                                              void* stream);
+/* grouped_m with a per-expert bias (ParameterizedExperts with add_bias, moe/base.py:12-50):
+ *   D[rows of g] = (A . W[g]^T + bias[g]) * alpha, fp32 epilogue, one rounding to bf16 (as the dense biased linear).
+ * bias bf16 [G, N] with row stride ld_bias (even, >= N).  a_row_index NULL: A is grouped (as grouped_m); otherwise the
+ * fused gather of grouped_m_gather (a_rows, a_row_index as there, b_mn_major must be 0). */
+int dolomite_b200_gemm_bf16_grouped_m_bias(const void* A, int64_t lda, int64_t a_rows, const int32_t* a_row_index,
+                                           const void* B, int64_t ldb, int b_mn_major, void* D, int64_t ldd,
+                                           const void* bias, int64_t ld_bias, float alpha, int64_t M_max, int64_t N,
+                                           int64_t K, const int32_t* m_tile_group, int num_groups, int flags,
+                                           void* stream);
 int dolomite_b200_gemm_bf16_grouped_k(const void* A, int64_t lda, const void* B, int64_t ldb, float* D, int64_t ldd,
                                       float alpha, float beta, int64_t M, int64_t N, int64_t K_max,
                                       const int32_t* group_k_offsets, int num_groups, void* stream);
