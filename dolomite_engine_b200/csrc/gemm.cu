@@ -91,8 +91,9 @@ struct GemmParams {
     int num_tiles;  // over all problems (grouped modes: single problem, includes the group factor)
     int d_is_f32;
     // grouped modes (MoE experts; moe_dolomite/moe/scatter.py:38-49 parallel_linear):
-    //   1 = M-grouped: every 128-row tile of A/D belongs to one group (m_tile_group[m_blk], -1 = unused tile); B's outer
-    //       TMA coordinate is offset by group * b_group_rows (fwd / dgrad of the expert linears)
+    //   1 = M-grouped: every 128-row tile of A/D belongs to one group (m_tile_group[m_blk], -1 = unused tile); a K-major
+    //       B's outer TMA coordinate is offset by group * b_group_rows, an MN-major B's rank-3 map takes the group as its
+    //       third coordinate (fwd / dgrad of the expert linears)
     //   2 = K-grouped: tile index also enumerates the group; the contraction runs over rows
     //       [group_k_offsets[g], group_k_offsets[g+1]) and D/C are slice g of their rank-3 maps (expert wgrad)
     int grouped;
@@ -456,7 +457,7 @@ __device__ __forceinline__ void gemm_body(const GemmMaps& maps, const GemmParams
                 const CUtensorMap* tmap_b = &maps.b[ti.q];
                 const uint64_t ha = p.pr[ti.q].hint_a, hb = p.pr[ti.q].hint_b;
                 const int m_blk = ti.m_blk, n_blk = ti.n_blk;
-                const int b_outer = (Op::GROUPED && p.grouped == 1) ? ti.grp * p.b_group_rows : 0;
+                const int b_outer = (Op::GROUPED && p.grouped == 1 && !B_MN) ? ti.grp * p.b_group_rows : 0;
                 for (int kb = ti.kb0; kb < ti.kb1; ++kb) {
                     mbar_wait(&empty_bar[stage], phase ^ 1, 1);
                     uint8_t* sa = smem_a + stage * A_STAGE_BYTES;
@@ -471,6 +472,12 @@ __device__ __forceinline__ void gemm_body(const GemmMaps& maps, const GemmParams
                     }
                     if (!B_MN) {
                         tma_load_2d_hint(sb, tmap_b, &full_bar[stage], kb * Op::KB_ELEMS, b_outer + n_blk * TN, hb);
+                    } else if (Op::GROUPED && p.grouped == 1) {
+                        // M-grouped dgrad: B's rank-3 map {N, K, groups} zero-fills the K tail of the tile's own expert
+                        // (grouped launches load with the normal L2 priority, so no hint)
+#pragma unroll
+                        for (int i = 0; i < TN / 64; ++i)
+                            tma_load_3d(sb + i * (BK * 128), tmap_b, &full_bar[stage], n_blk * TN + i * 64, kb * BK, ti.grp);
                     } else {
 #pragma unroll
                         for (int i = 0; i < TN / 64; ++i)
@@ -652,11 +659,11 @@ struct GroupArgs {
     const int* a_row_index = nullptr;  // mode 1 only: gather the rows of A on load (A is the ungrouped matrix of a_rows rows)
     int64_t a_rows = 0;
     const int* m_tile_group = nullptr;
-    int64_t b_group_rows = 0;
+    int64_t b_group_rows = 0;   // mode 1, K-major B: rows of one group's B
     const int* group_k_offsets = nullptr;
     int num_groups = 1;
     int64_t d_group_stride = 0;
-    int64_t b_total_outer = 0;  // rows of B's outer TMA dimension over all groups
+    int64_t b_total_outer = 0;  // mode 1, K-major B: rows of B's outer TMA dimension over all groups
     int64_t bias_group_stride = 0;  // mode 1 with bias: elements between the bias rows of consecutive groups
 };
 
@@ -734,13 +741,24 @@ static int setup_problem(GemmMaps& maps, GemmParams& p, int q, const GemmProblem
     }
     strides[0] = ab;
     if (!b_mn_major) {
+        // M-grouped: the experts' [N, K] matrices stacked into one [groups * N, K]; an N tail of expert g reads rows of
+        // expert g + 1, which only reach the clipped output columns >= N
         dims[0] = uint64_t(K); dims[1] = uint64_t(ga.mode == 1 ? ga.b_total_outer : N); strides[1] = uint64_t(g.ldb) * ab;
         box[0] = 128 / ab; box[1] = uint32_t(tile_n);
+        rc = dolo_make_tmap(&maps.b[q], g.B, ab, 2, dims, strides, box, DOLO_SW_128);
+    } else if (ga.mode == 1) {
+        // M-grouped, MN-major: dims {N, K, groups}, box {64, 64, 1}.  Expert g's contraction ends at its own row K, so the
+        // K tail of its last k-block is zero-filled rather than read from expert g + 1 (whose rows, multiplied by A's
+        // zero-filled columns, would turn a non-finite weight into NaN).
+        const uint64_t dims3[3] = {uint64_t(N), uint64_t(K), uint64_t(ga.num_groups)};
+        const uint64_t strides3[3] = {2, uint64_t(g.ldb) * 2, uint64_t(K * g.ldb) * 2};
+        const uint32_t box3[3] = {64, BK, 1};
+        rc = dolo_make_tmap(&maps.b[q], g.B, ab, 3, dims3, strides3, box3, DOLO_SW_128);
     } else {
-        dims[0] = uint64_t(N); dims[1] = uint64_t(ga.mode == 1 ? ga.b_total_outer : K); strides[1] = uint64_t(g.ldb) * 2;
+        dims[0] = uint64_t(N); dims[1] = uint64_t(K); strides[1] = uint64_t(g.ldb) * 2;
         box[0] = 64; box[1] = BK;
+        rc = dolo_make_tmap(&maps.b[q], g.B, ab, 2, dims, strides, box, DOLO_SW_128);
     }
-    rc = dolo_make_tmap(&maps.b[q], g.B, ab, 2, dims, strides, box, DOLO_SW_128);
     if (rc) return rc;
     {
         // D and C: dims {N, M, groups}, box = one epilogue slab {128 B of columns, 64 rows, 1}
@@ -924,7 +942,8 @@ static int grouped_m_impl(const void* A, int64_t lda, int64_t a_rows, const int3
                           int flags, void* stream) {
     DOLO_REQUIRE(M_max % BM == 0, "grouped gemm: M_max=%lld must be a multiple of %d (padded expert segments)",
                  (long long)M_max, BM);
-    DOLO_REQUIRE(!b_mn_major || K % BK == 0, "grouped gemm: MN-major B needs K %% %d == 0", BK);
+    // MN-major B: the experts' [K, N] matrices follow each other, so K % 8 == 0 keeps every expert's base 16-byte aligned
+    DOLO_REQUIRE(!b_mn_major || K % 8 == 0, "grouped gemm: MN-major B needs K %% 8 == 0 (K=%lld)", (long long)K);
     DOLO_REQUIRE(m_tile_group != nullptr && num_groups > 0, "grouped gemm: missing group table");
     if (a_row_index != nullptr) {
         DOLO_REQUIRE(!b_mn_major && a_rows > 0, "grouped gemm (gather): K-major B and a_rows > 0 needed");
@@ -940,8 +959,8 @@ static int grouped_m_impl(const void* A, int64_t lda, int64_t a_rows, const int3
     ga.a_rows = a_rows;
     ga.m_tile_group = m_tile_group;
     ga.num_groups = num_groups;
-    ga.b_group_rows = b_mn_major ? K : N;
-    ga.b_total_outer = ga.b_group_rows * num_groups;
+    ga.b_group_rows = N;  // K-major B only (an MN-major B has a rank-3 map with one slice per group)
+    ga.b_total_outer = N * num_groups;
     ga.bias_group_stride = bias != nullptr ? ld_bias : 0;
     return gemm_impl(A, lda, 0, B, ldb, b_mn_major, D, ldd, 0, nullptr, 0, alpha, 0.f, bias, M_max, N, K, flags, stream,
                      ga);

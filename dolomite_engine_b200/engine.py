@@ -228,13 +228,13 @@ def check_supported(cfg: CommonConfig, *, attention_implementation: str = "flash
     if hd not in (16, 32, 64, 80, 96, 128):
         raise NotImplementedError(f"head_dim={hd}: supported head dims are 16, 32, 64, 80, 96, 128")
     if cfg.model_type == "moe_dolomite":
-        if cfg.num_experts % 8 or not (1 <= cfg.num_experts_per_tok <= min(8, cfg.num_experts)):
-            raise NotImplementedError("MoE: num_experts must be a multiple of 8 (<= 256) and 1 <= top-k <= 8")
+        # any expert count up to the routing kernels' 256 (router buffers: kernels.router_logits / router_grad) and any
+        # width the dense model takes (the grouped expert GEMMs zero-fill each expert's own K and N tails)
+        if not (1 <= cfg.num_experts <= 256) or not (1 <= cfg.num_experts_per_tok <= min(8, cfg.num_experts)):
+            raise NotImplementedError("MoE: num_experts must be in [1, 256] and 1 <= top-k <= min(8, num_experts)")
         if cfg.add_bias and moe_implementation == "scattermoe":
             # the reference's ScatterMoE asserts this (moe/scatter.py:22); its eager experts carry the bias
             raise AssertionError("scattermoe doesn't support bias")
-        if cfg.n_inner % 64 or cfg.n_embd % 64:
-            raise NotImplementedError("MoE: n_embd and n_inner must be multiples of 64 (grouped GEMM K tiles)")
     # vocab_size may be any value: [T, V] logits live in buffers with 16-byte row strides (kernels.rows_empty)
     if cfg.n_embd % 8 or cfg.n_inner % 8:
         raise NotImplementedError("n_embd and n_inner must be multiples of 8 (16-byte vector kernels / TMA)")

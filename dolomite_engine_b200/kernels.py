@@ -66,6 +66,22 @@ def rows_aligned(t: torch.Tensor) -> torch.Tensor:
     return out
 
 
+# Router buffers of an MoE layer with E experts.  The gate GEMM writes its [T, E] logits in 16-byte rows (rows_empty); the
+# routing, load-balancing statistics and router backward kernels index a contiguous [T, E] (row stride E), and the router
+# backward writes its dlogits that way; both GEMMs that read dlogits need 16-byte rows again.  For E % 8 == 0 the two
+# layouts are the same tensor and nothing is copied.  Otherwise each side gets a copy of T * E * 2 bytes (under 1 MB at
+# 8192 tokens and E = 60): two small copies keep the three router kernels and their entry points as they are, where a row
+# stride argument would need a second entry point for each.
+def router_logits(gate_out: torch.Tensor) -> torch.Tensor:
+    """the gate GEMM's [T, E] output as the router kernels index it (and as output_router_logits returns it): contiguous"""
+    return gate_out if gate_out.is_contiguous() else gate_out.contiguous()
+
+
+def router_grad(dlogits: torch.Tensor) -> torch.Tensor:
+    """the router backward's contiguous [T, E] dlogits as the gate GEMMs' operand: 16-byte rows"""
+    return rows_aligned(dlogits)
+
+
 # ------------------------------------------------------------------------------------------------
 # RMSNorm (normalization/rmsnorm/base.py:18-25)
 # ------------------------------------------------------------------------------------------------

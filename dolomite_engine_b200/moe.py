@@ -18,6 +18,11 @@ bf16 as in the dense biased linear.  Their gradients are per-segment column sums
 m_residual), d c_fc.bias[e] of `d_fc`, fused into the activation backward.  Both reduce in a fixed order with no float
 atomics, and an expert without tokens adds exact zeros.  Activations stay grouped between the two expert GEMMs exactly
 like `parallel_linear(grouped_out=True)` -> `parallel_linear(grouped_in=True, gates=...)`.
+
+Shapes: any E in [1, 256] and any n_embd / n_inner that are multiples of 8.  The grouped GEMMs zero-fill each expert's
+K and N tails from its own extent, so no product ever reads another expert's weights.  The router kernels index
+contiguous [T, E] buffers while the gate GEMMs need 16-byte rows: kernels.router_logits / router_grad convert between
+the two, copies only when E % 8 != 0.
 """
 
 from __future__ import annotations
@@ -35,7 +40,8 @@ def forward(engine, unit, p: str, x, residual, m_res: float, layer: int = 0):
     cfg = engine.cfg
     k = cfg.num_experts_per_tok
     b_fc, b_proj = unit.views.get(p + "mlp.c_fc.bias"), unit.views.get(p + "mlp.c_proj.bias")
-    logits = engine._linear(unit, p + "mlp.gate.weight", x, flags=0)  # [T, E] bf16 (tiny N: direct-store epilogue)
+    # [T, E] bf16 (tiny N: direct-store epilogue), contiguous for the router kernels (a copy when E % 8 != 0)
+    logits = K.router_logits(engine._linear(unit, p + "mlp.gate.weight", x, flags=0))
     plan = K.moe_route(logits, k)
     if engine._aux_fwd is not None:  # load-balancing statistics of this layer (once per forward: not in recomputed blocks)
         acc, T_real, router_logits = engine._aux_fwd
@@ -94,6 +100,7 @@ def backward(engine, unit, p: str, x, dh, m_res: float, saved, layer: int = 0):
         dlogits = K.moe_router_bwd_aux(logits, plan, dw, c, s, T_real)
     else:
         dlogits = K.moe_router_bwd(plan, dw)
+    dlogits = K.router_grad(dlogits)  # 16-byte rows for the GEMMs below (a copy when E % 8 != 0)
     if engine._is_fp8(p + "mlp.gate.weight"):  # the router as te.Linear (num_experts % 16 == 0)
         return engine._linear_bwd_fp8(unit, p + "mlp.gate.weight", None, x, dlogits, dx_add=dx)
     gate = unit.views[p + "mlp.gate.weight"]

@@ -364,6 +364,12 @@ int dolomite_b200_fp8_scaling_update(float* amax_history, int history_len, int64
  *   grouped_k:  D[g][M, N] = alpha * A_g^T B_g + beta * D[g]  (expert wgrad, fp32): A [K_max, M], B [K_max, N] row-major,
  *               contraction over the rows [group_k_offsets[g], group_k_offsets[g+1]) of expert g.  beta = 0 OVERWRITES: D need not
  *               be initialised, and the slice of an expert with an empty row range is written as zeros; beta != 0 leaves it alone.
+ * Extents: N and K may take any value that keeps the row strides 16-byte aligned (lda, ldb, ldd multiples of 8 bf16 / 4
+ * fp32 elements; an MN-major B, and the fused gather, need K % 8 == 0).  Every K and N tail is expert-local: TMA
+ * zero-fills the last k-block of expert g from its own rows (a K-major B as one [G * N, K] map whose N tail only reaches
+ * the clipped output columns >= N; an MN-major B as a rank-3 {N, K, G} map), so another expert's weights, finite or not,
+ * never enter a product.  grouped_k stops every tile at row M and column N of its own group (D is a rank-3 {N, M, G}
+ * map with group stride M * ldd), for the overwrite, the accumulate and the zero slices of experts without rows.
  * ------------------------------------------------------------------------------------------------ */
 int dolomite_b200_gemm_bf16_grouped_m(const void* A, int64_t lda, const void* B, int64_t ldb, int b_mn_major, void* D,
                                       int64_t ldd, float alpha, int64_t M_max, int64_t N, int64_t K,
@@ -397,6 +403,8 @@ int dolomite_b200_gemm_bf16_grouped_k(const void* A, int64_t lda, const void* B,
  *              dolomite_b200_gemm_bf16_grouped_m_gather.  Segments are padded to 256 rows.
  *   moe_gather: X_g[row] = x[slot_of_row[row] / k] or 0.     moe_combine: out = c + alpha * sum_j w_j * Y_g[row_j].
  *   moe_combine_bwd / moe_token_sum / moe_router_bwd: their backward pieces.
+ * Any E in [1, 256]: router logits and dlogits are contiguous [T, E] (row stride E); a caller whose GEMMs need 16-byte
+ * rows (E % 8 != 0) stages them (kernels.router_logits / router_grad in the Python package).
  * ------------------------------------------------------------------------------------------------ */
 int64_t dolomite_b200_moe_max_rows(int64_t T, int E, int k);
 int dolomite_b200_moe_route(const void* router_logits, int64_t T, int E, int k, int32_t* sel_idx, float* sel_w,
