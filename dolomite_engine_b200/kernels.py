@@ -421,7 +421,7 @@ def set_default_gemm_flags(flags: int) -> None:
 
 
 def gemm(a, b, *, a_mn=False, b_mn=False, out=None, out_dtype=_BF16, c=None, alpha=1.0, beta=0.0, bias=None, flags=None):
-    """D[M,N] = alpha * A·Bᵀ + bias + beta*C.  A logical [M,K] (stored [K,M] if a_mn), B logical [N,K] (stored [K,N] if b_mn)."""
+    """D[M,N] = alpha * (A·Bᵀ + bias) + beta*C.  A logical [M,K] (stored [K,M] if a_mn), B logical [N,K] (stored [K,N] if b_mn)."""
     _req(a, _BF16, "a"), _req(b, _BF16, "b")
     assert a.dim() == 2 and b.dim() == 2 and a.stride(1) == 1 and b.stride(1) == 1
     if a_mn:

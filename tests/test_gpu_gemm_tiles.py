@@ -1,5 +1,5 @@
 """GPU: the 128 x 256 output tile of the dense bf16 GEMM (wgmma m64n256k16) against the 128 x 128 tile and against fp64,
-and the per-launch choice of the tile width.
+the same bits on fewer SMs (gemm_sm_margin), and the per-launch choice of the tile width.
 
 Each output element sees the same k16 MMA sequence in the same order at both widths, so the results are bit-identical."""
 
@@ -40,6 +40,22 @@ def at_both_widths(fn):
         with tile_n(width):
             outs.append(fn())
     torch.cuda.synchronize()
+    return outs
+
+
+SM_MARGINS = (1, 37, 64)  # SMs left out of the persistent schedule: each worker then runs more tiles through the ring
+
+
+def at_sm_margins(fn):
+    """fn at both tile widths with each gemm_sm_margin (0 is the library default)"""
+    outs = []
+    old = K().get_option("gemm_sm_margin")
+    try:
+        for margin in SM_MARGINS:
+            K().set_option("gemm_sm_margin", margin)
+            outs.extend(at_both_widths(fn))
+    finally:
+        K().set_option("gemm_sm_margin", old)
     return outs
 
 
@@ -95,6 +111,8 @@ def test_tile_widths_bit_identical_and_accurate(a_mn, b_mn, case):
 
     o128, o256 = at_both_widths(run)
     assert torch.equal(o128, o256), (M, N, Kd, a_mn, b_mn, (o128.float() - o256.float()).abs().max().item())
+    for i, o in enumerate(at_sm_margins(run)):
+        assert torch.equal(o, o128), (M, N, Kd, a_mn, b_mn, SM_MARGINS[i // 2])
 
     ref = _reference(A, B, b, C, ab)
     for out in (o128, o256):
@@ -124,8 +142,10 @@ def test_wgrad_multi_tile_widths_bit_identical_and_accurate():
         return dws
 
     w128, w256 = at_both_widths(run)
+    margins = at_sm_margins(run)
     for q in range(len(shapes)):
         assert torch.equal(w128[q], w256[q]), q
+        assert all(torch.equal(w[q], w128[q]) for w in margins), q
         ref = alphas[q] * (dys[q].double().t() @ xs[q].double()) + (dw0[q].double() if accumulate[q] else 0.0)
         for w in (w128[q], w256[q]):
             assert torch.allclose(w.double().cpu(), ref, atol=1e-3, rtol=1e-4), (q, (w.double().cpu() - ref).abs().max())
