@@ -385,6 +385,8 @@ __device__ __forceinline__ float tanh_fast(float z) {
 }
 
 namespace act {
+// min(max(x, lo), hi) that keeps a NaN (fminf / fmaxf return the other operand), as torch's clamp and relu do
+__device__ __forceinline__ float clamp_nan(float x, float lo, float hi) { return x < lo ? lo : (x > hi ? hi : x); }
 // elu / celu (alpha 1; CELU with alpha 1 is ELU) and selu: torch's elu kernel, x <= 0 ? expm1(x) * a * s : x * s
 template <int kSelu>
 struct EluT {
@@ -419,7 +421,7 @@ struct HardShrink {  // lambda 0.5; zero on [-0.5, 0.5], ends included (value an
     __device__ static float d(float x) { return (x >= -0.5f && x <= 0.5f) ? 0.f : 1.f; }
 };
 struct HardSigmoid {
-    __device__ static float f(float x) { return fminf(fmaxf(x + 3.f, 0.f), 6.f) / 6.f; }
+    __device__ static float f(float x) { return clamp_nan(x + 3.f, 0.f, 6.f) / 6.f; }
     __device__ static float d(float x) { return (x > -3.f && x < 3.f) ? 1.f / 6.f : 0.f; }
 };
 struct HardSwish {  // gradient x/3 + 1/2 inside (-3, 3); 0 at -3 and 1 at 3, as torch autograd gives
@@ -427,7 +429,7 @@ struct HardSwish {  // gradient x/3 + 1/2 inside (-3, 3); 0 at -3 and 1 at 3, as
     __device__ static float d(float x) { return x <= -3.f ? 0.f : (x < 3.f ? x / 3.f + 0.5f : 1.f); }
 };
 struct HardTanh {  // [-1, 1]; gradient 0 at the bounds
-    __device__ static float f(float x) { return fminf(fmaxf(x, -1.f), 1.f); }
+    __device__ static float f(float x) { return clamp_nan(x, -1.f, 1.f); }
     __device__ static float d(float x) { return (x > -1.f && x < 1.f) ? 1.f : 0.f; }
 };
 // transformers' LaplaceActivation, mu 0.707107, sigma 0.282095: 0.5 * (1 + erf((x - mu) / (sigma sqrt 2))), every eager
@@ -464,15 +466,15 @@ struct Mish {
     }
 };
 struct Relu {
-    __device__ static float f(float x) { return fmaxf(x, 0.f); }
+    __device__ static float f(float x) { return x < 0.f ? 0.f : x; }
     __device__ static float d(float x) { return x > 0.f ? 1.f : 0.f; }
 };
 struct Relu2 {  // square(relu(x)): relu is exact, so one rounding
-    __device__ static float f(float x) { const float r = fmaxf(x, 0.f); return r * r; }
+    __device__ static float f(float x) { const float r = x < 0.f ? 0.f : x; return r * r; }
     __device__ static float d(float x) { return x > 0.f ? 2.f * x : 0.f; }
 };
 struct Relu6 {  // hardtanh(0, 6): gradient 0 at both bounds
-    __device__ static float f(float x) { return fminf(fmaxf(x, 0.f), 6.f); }
+    __device__ static float f(float x) { return clamp_nan(x, 0.f, 6.f); }
     __device__ static float d(float x) { return (x > 0.f && x < 6.f) ? 1.f : 0.f; }
 };
 struct Sigmoid {
@@ -488,7 +490,7 @@ struct Softplus {  // beta 1, threshold 20: linear (gradient 1) above the thresh
     __device__ static float d(float x) { const float z = expf(x); return x > 20.f ? 1.f : z / (z + 1.f); }
 };
 struct SoftShrink {  // lambda 0.5; zero gradient on [-0.5, 0.5], ends included
-    __device__ static float f(float x) { return x > 0.5f ? x - 0.5f : (x < -0.5f ? x + 0.5f : 0.f); }
+    __device__ static float f(float x) { return (x >= -0.5f && x <= 0.5f) ? 0.f : (x > 0.f ? x - 0.5f : x + 0.5f); }
     __device__ static float d(float x) { return (x >= -0.5f && x <= 0.5f) ? 0.f : 1.f; }
 };
 struct SoftSign {  // x / (|x| + 1), the sum rounded first

@@ -162,46 +162,88 @@ def layernorm_bwd(dy, x, w, mean, rstd, dw_accum, db_accum, dx_add=None, out=Non
     return dx
 
 
+def _rows_layout(t, shape: tuple, name: str) -> None:
+    """`t` must be a contiguous tensor of `shape`: the 16-byte vector kernels address rows of exactly shape[-1] elements"""
+    if tuple(t.shape) != tuple(shape) or not t.is_contiguous():
+        raise ValueError(f"{name} must be a contiguous {list(shape)} tensor, got shape {tuple(t.shape)} and strides "
+                         f"{tuple(t.stride())}")
+
+
+def _act_layout(x, form: int, name: str = "x") -> tuple[int, int, int]:
+    """(T, W, F) of an activation input: x contiguous [T, W], W = F (plain) or 2F (GLU forms); checked before any launch"""
+    if x.dim() != 2 or not x.is_contiguous():
+        raise ValueError(f"{name} must be a contiguous 2-D tensor, got shape {tuple(x.shape)} and strides {tuple(x.stride())}")
+    T, W = x.shape
+    if form != 0 and W % 2:
+        raise ValueError(f"{name} must have an even width [u | g] for a GLU form, got {W} columns")
+    return T, W, (W if form == 0 else W // 2)
+
+
+def _bias_accum_layout(b, W: int) -> None:
+    if b.numel() != W or not b.is_contiguous():
+        raise ValueError(f"bias_grad_accum must be a contiguous tensor of {W} elements, got shape {tuple(b.shape)} and "
+                         f"strides {tuple(b.stride())}")
+
+
 def act_fwd(x, act_id: int, form: int, out=None):
     """MLP activation (activations.resolve gives `act_id`, `form`): plain [T, F] -> [T, F]; GLU forms [T, 2F] -> [T, F]"""
+    T, W, F = _act_layout(x, form)
+    if out is not None:
+        _rows_layout(out, (T, F), "out")
     _req(x, _BF16, "x")
-    T, W = x.shape
-    F = W if form == 0 else W // 2
     y = torch.empty(T, F, dtype=_BF16, device=x.device) if out is None else out
     _lib.call("dolomite_b200_act_fwd", act_id, form, x.data_ptr(), y.data_ptr(), T, F, _stream())
     return y
 
 
+def _act_bwd_layout(dy, x, form: int, out) -> tuple[int, int, int]:
+    T, W, F = _act_layout(x, form)
+    _rows_layout(dy, (T, F), "dy")
+    if out is not None:
+        _rows_layout(out, (T, W), "out")
+    return T, W, F
+
+
 def act_bwd(dy, x, act_id: int, form: int, out=None, bias_grad_accum=None):
     """dx of act_fwd; with `bias_grad_accum` (fp32, one per column of x) also += column sums of dx (bias gradient of c_fc)"""
+    T, W, F = _act_bwd_layout(dy, x, form, out)
+    if bias_grad_accum is not None:
+        _bias_accum_layout(bias_grad_accum, W)
     _req(dy, _BF16, "dy"), _req(x, _BF16, "x")
-    T, W = x.shape
     dx = torch.empty_like(x) if out is None else out
     if bias_grad_accum is not None:
         _req(bias_grad_accum, torch.float32, "bias_grad_accum")
-        assert bias_grad_accum.numel() == W
     _lib.call("dolomite_b200_act_bwd", act_id, form, dy.data_ptr(), x.data_ptr(), dx.data_ptr(), _ptr(bias_grad_accum), T,
-              W if form == 0 else W // 2, _stream())
+              F, _stream())
     return dx
 
 
 def act_bwd_segmented(dy, x, act_id: int, form: int, seg_offsets, bias_grad_accum, out=None):
     """act_bwd on the rows of the segments [seg_offsets[s], seg_offsets[s + 1]) (int32 device table, e.g. a MoE plan's
-    offsets); bias_grad_accum fp32 [segments, columns of x]: row s += column sums of segment s's dx.  Rows outside every
-    segment are not written."""
+    offsets); bias_grad_accum fp32 [segments, columns of x] (unit column stride, any row stride >= the width): row s +=
+    column sums of segment s's dx.  Rows outside every segment are not written."""
+    T, W, F = _act_bwd_layout(dy, x, form, out)
+    S = seg_offsets.numel() - 1
+    b = bias_grad_accum
+    if b.dim() != 2 or tuple(b.shape) != (S, W) or b.stride(1) != 1 or (S > 1 and b.stride(0) < W):
+        raise ValueError(f"bias_grad_accum must be a [{S}, {W}] tensor with unit column stride, got shape "
+                         f"{tuple(b.shape)} and strides {tuple(b.stride())}")
+    if seg_offsets.dim() != 1 or not seg_offsets.is_contiguous():
+        raise ValueError(f"seg_offsets must be a contiguous 1-D tensor, got strides {tuple(seg_offsets.stride())}")
     _req(dy, _BF16, "dy"), _req(x, _BF16, "x"), _req(bias_grad_accum, torch.float32, "bias_grad_accum")
     _req(seg_offsets, torch.int32, "seg_offsets")
-    T, W = x.shape
-    S = seg_offsets.numel() - 1
-    assert bias_grad_accum.dim() == 2 and bias_grad_accum.shape == (S, W) and bias_grad_accum.stride(1) == 1
     dx = torch.empty_like(x) if out is None else out
     _lib.call("dolomite_b200_act_bwd_segmented", act_id, form, dy.data_ptr(), x.data_ptr(), dx.data_ptr(),
-              bias_grad_accum.data_ptr(), bias_grad_accum.stride(0), W if form == 0 else W // 2, seg_offsets.data_ptr(), S,
-              _stream())
+              bias_grad_accum.data_ptr(), max(bias_grad_accum.stride(0), W), F, seg_offsets.data_ptr(), S, _stream())
     return dx
 
 
 def gelu_fwd(x, out=None):
+    """tanh-GELU of any contiguous tensor with a multiple of 8 elements (act_fwd(GELU_TANH, PLAIN) on [n / 8, 8])"""
+    if not x.is_contiguous():
+        raise ValueError(f"x must be a contiguous tensor, got strides {tuple(x.stride())}")
+    if out is not None:
+        _rows_layout(out, tuple(x.shape), "out")
     _req(x, _BF16, "x")
     y = torch.empty_like(x) if out is None else out
     _lib.call("dolomite_b200_gelu_fwd", x.data_ptr(), y.data_ptr(), x.numel(), _stream())
@@ -209,33 +251,39 @@ def gelu_fwd(x, out=None):
 
 
 def gelu_bwd(dy, x, out=None, bias_grad_accum=None):
+    T, W, F = _act_bwd_layout(dy, x, 0, out)
+    if bias_grad_accum is not None:
+        _bias_accum_layout(bias_grad_accum, W)
+        _req(bias_grad_accum, torch.float32, "bias_grad_accum")
     _req(dy, _BF16, "dy"), _req(x, _BF16, "x")
-    T, F = x.shape
     dx = torch.empty_like(x) if out is None else out
     _lib.call("dolomite_b200_gelu_bwd", dy.data_ptr(), x.data_ptr(), dx.data_ptr(), _ptr(bias_grad_accum), T, F, _stream())
     return dx
 
 
 def swiglu_fwd(x, out=None):
+    T, W, F = _act_layout(x, 1)
+    if out is not None:
+        _rows_layout(out, (T, F), "out")
     _req(x, _BF16, "x")
-    T, F2 = x.shape
-    y = torch.empty(T, F2 // 2, dtype=_BF16, device=x.device) if out is None else out
-    _lib.call("dolomite_b200_swiglu_fwd", x.data_ptr(), y.data_ptr(), T, F2 // 2, _stream())
+    y = torch.empty(T, F, dtype=_BF16, device=x.device) if out is None else out
+    _lib.call("dolomite_b200_swiglu_fwd", x.data_ptr(), y.data_ptr(), T, F, _stream())
     return y
 
 
 def swiglu_bwd(dy, x, out=None, bias_grad_accum=None):
     """dx of y = up * silu(gate); with `bias_grad_accum` (fp32 [2F]) also += column sums of dx (bias gradient of c_fc)"""
+    T, W, F = _act_bwd_layout(dy, x, 1, out)
+    if bias_grad_accum is not None:
+        _bias_accum_layout(bias_grad_accum, W)
     _req(dy, _BF16, "dy"), _req(x, _BF16, "x")
-    T, F2 = x.shape
     dx = torch.empty_like(x) if out is None else out
     if bias_grad_accum is not None:
         _req(bias_grad_accum, torch.float32, "bias_grad_accum")
-        assert bias_grad_accum.numel() == F2
         _lib.call("dolomite_b200_swiglu_bwd_bias", dy.data_ptr(), x.data_ptr(), dx.data_ptr(), bias_grad_accum.data_ptr(),
-                  T, F2 // 2, _stream())
+                  T, F, _stream())
     else:
-        _lib.call("dolomite_b200_swiglu_bwd", dy.data_ptr(), x.data_ptr(), dx.data_ptr(), T, F2 // 2, _stream())
+        _lib.call("dolomite_b200_swiglu_bwd", dy.data_ptr(), x.data_ptr(), dx.data_ptr(), T, F, _stream())
     return dx
 
 
@@ -261,10 +309,33 @@ def embedding_bwd(ids, dout, dwte_accum, scale: float = 1.0):
 # ------------------------------------------------------------------------------------------------
 # Cross entropy fwd+bwd (model_wrapper/pretraining.py:124-125)
 # ------------------------------------------------------------------------------------------------
-def cross_entropy_fwd_bwd(logits, labels, ignore_index=-100, logit_scale=1.0, grad_scale=1.0, dlogits=None):
-    _req(logits, _BF16, "logits"), _req(labels, torch.int64, "labels")
+def _ce_layout(logits, labels) -> tuple[int, int]:
+    """(T, V): logits 2-D with unit column stride (any row stride: the kernel takes it), labels a contiguous int64 [T]"""
+    if logits.dim() != 2 or logits.stride(1) != 1:
+        raise ValueError(f"logits must be a 2-D tensor with unit column stride, got shape {tuple(logits.shape)} and "
+                         f"strides {tuple(logits.stride())}")
     T, V = logits.shape
-    assert logits.stride(1) == 1
+    if labels.dtype != torch.int64 or labels.numel() != T or not labels.is_contiguous():
+        raise ValueError(f"labels must be a contiguous int64 tensor of {T} elements, got {labels.dtype} shape "
+                         f"{tuple(labels.shape)} and strides {tuple(labels.stride())}")
+    return T, V
+
+
+def cross_entropy_fwd_bwd(logits, labels, ignore_index=-100, logit_scale=1.0, grad_scale=1.0, dlogits=None):
+    """mean cross entropy of the rows of `logits` [T, V] * logit_scale and its gradient (times grad_scale) -> (loss [1],
+    loss_tok [T], dlogits).  dlogits overwrites the logits unless a `dlogits` of the same shape and strides is given (the
+    kernel writes it with the logits' row stride).  The kernel works in log2 units in fp32 with one FMA per logit, x *
+    scale2 - m, scale2 = logit_scale * log2(e) and m the row's largest fp32 x * scale2.  Two limits follow, where torch's
+    fp32 cross entropy stays finite: above |x * logit_scale| ~ 2^31 that FMA of the largest logit can be its rounding
+    residual, more than 128, whose ex2 is inf (loss inf, NaN gradient); and |x * logit_scale| of 2.36e38 or more
+    overflows x * scale2 and gives NaN."""
+    T, V = _ce_layout(logits, labels)
+    if dlogits is not None and (dlogits.shape != logits.shape or dlogits.stride() != logits.stride()):
+        raise ValueError(f"dlogits must have logits' shape {tuple(logits.shape)} and strides {tuple(logits.stride())}, "
+                         f"got {tuple(dlogits.shape)} and {tuple(dlogits.stride())}")
+    _req(logits, _BF16, "logits"), _req(labels, torch.int64, "labels")
+    if dlogits is not None:
+        _req(dlogits, _BF16, "dlogits")
     dl = logits if dlogits is None else dlogits
     loss_tok = torch.empty(T, dtype=torch.float32, device=logits.device)
     loss = torch.empty(1, dtype=torch.float32, device=logits.device)
@@ -278,6 +349,8 @@ def cross_entropy_fwd_bwd(logits, labels, ignore_index=-100, logit_scale=1.0, gr
 
 def cross_entropy_count(labels, ignore_index=-100):
     """-> scratch (fp32 [2]); scratch[0] = number of labels != ignore_index (the divisor of the mean loss and its gradient)"""
+    if not labels.is_contiguous():
+        raise ValueError(f"labels must be a contiguous int64 tensor, got strides {tuple(labels.stride())}")
     _req(labels, torch.int64, "labels")
     scratch = torch.empty(2, dtype=torch.float32, device=labels.device)
     _lib.call("dolomite_b200_cross_entropy_count", labels.data_ptr(), labels.numel(), ignore_index, scratch.data_ptr(), _stream())
@@ -286,9 +359,11 @@ def cross_entropy_count(labels, ignore_index=-100):
 
 def cross_entropy_rows(logits, labels, loss_tok, scratch, ignore_index=-100, logit_scale=1.0, grad_scale=1.0):
     """one chunk of rows: logits [t, V] are overwritten by their gradient, loss_tok [t] receives the per-token losses"""
+    t, V = _ce_layout(logits, labels)
+    if loss_tok.numel() != t or not loss_tok.is_contiguous():
+        raise ValueError(f"loss_tok must be a contiguous tensor of {t} elements, got shape {tuple(loss_tok.shape)} and "
+                         f"strides {tuple(loss_tok.stride())}")
     _req(logits, _BF16, "logits"), _req(labels, torch.int64, "labels"), _req(loss_tok, torch.float32, "loss_tok")
-    t, V = logits.shape
-    assert logits.stride(1) == 1 and labels.numel() == t and loss_tok.numel() == t
     _lib.call("dolomite_b200_cross_entropy_rows", logits.data_ptr(), logits.stride(0), labels.data_ptr(), logits.data_ptr(),
               loss_tok.data_ptr(), scratch.data_ptr(), t, V, ignore_index, logit_scale, grad_scale, _stream())
     return logits
