@@ -88,23 +88,7 @@ static_assert(ATT_PRODUCER_REGS * 128 + 2 * ATT_CONSUMER_REGS * 128 <= 65536, "r
 // gradient is summed in a fixed order and the backward is bit-identical from run to run -- adding the dQ contributions
 // of the key-tile CTAs with atomics would not be.
 constexpr int BWD_QT = 64;  // query rows per step
-
-// Hides a shared-memory base address from the compiler's loop-invariant code motion, so that the wgmma descriptors built
-// from it are recomputed next to each MMA instead of being hoisted out of the step loop and held in registers.
-__device__ __forceinline__ void opaque(uint32_t& x) { asm volatile("" : "+r"(x)); }
-// Wait without the watchdog of mbar_wait, for waits with an MMA group in flight: ptxas serialises every wgmma of a kernel
-// that has a trap path (or any other divergent branch) while a group is in flight.
-__device__ __forceinline__ void mbar_spin(uint64_t* bar, uint32_t parity) {
-    asm volatile("{\n\t.reg .pred P1;\n\tWAIT_%=:\n\tmbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t@!P1 bra WAIT_%=;\n\t}"
-                 ::"r"(smem_u32(bar)), "r"(parity)
-                 : "memory");
-}
-// Arrive of lane 0 only, as a predicated instruction rather than a branch, for the same reason.
-__device__ __forceinline__ void mbar_arrive_lane0(uint64_t* bar, int lane) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.eq.s32 p, %1, 0;\n\t@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}" ::"r"(smem_u32(bar)),
-                 "r"(lane)
-                 : "memory");
-}
+// opaque, mbar_spin and mbar_arrive_lane0: attention_common.cuh
 constexpr int QDO_STAGES = 4;
 
 // P^T (into st) and dS^T (into dpt) of one step from S^T, dP^T; MASK = test causality and the document end per element
@@ -672,8 +656,8 @@ int attn_bwd(const void* dout, const void* qkv, int64_t row_stride, const void* 
     const int nh = n_groups * q_per_group;
     DOLO_REQUIRE(int64_t(nh) * T < (1ll << 31), "attn_bwd: heads * T too large for the dQ tile reduce");
     switch (head_dim) {
-        case 16: case 32: case 64: case 80: case 96: case 128: break;
-        default: return dolo_set_error("attn_bwd: unsupported head_dim %d (supported: 16,32,64,80,96,128)", head_dim);
+        case 16: case 32: case 64: case 80: case 96: case 128: case 160: case 192: case 256: break;
+        default: return dolo_set_error("attn_bwd: unsupported head_dim %d (supported: 16,32,64,80,96,128,160,192,256)", head_dim);
     }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     float* delta = static_cast<float*>(workspace);
@@ -683,6 +667,9 @@ int attn_bwd(const void* dout, const void* qkv, int64_t row_stride, const void* 
             static_cast<const uint4*>(dout), static_cast<const uint4*>(out), delta, T, nh, head_dim / 8);
         DOLO_LAUNCH_OK("attn_delta");
     }
+    if (head_dim > 128)
+        return dolo_attn_wide_bwd(dout, qkv, row_stride, lse, delta, dqkv, cu_seqlens, n_docs, T, n_groups, q_per_group,
+                                  head_dim, softmax_scale, dropout_p, key0, key1, alibi_slopes, st);
     BwdParams p;
     p.lse = lse;
     p.delta = delta;

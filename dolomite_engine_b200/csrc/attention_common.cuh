@@ -20,7 +20,7 @@ constexpr int ATT_TILE = 128;  // query rows (forward) / key rows (backward) per
 
 template <int HD>
 struct HeadChunks {
-    static_assert(HD % 16 == 0 && HD >= 16 && HD <= 128, "head_dim must be a multiple of 16 in [16, 128]");
+    static_assert(HD % 16 == 0 && HD >= 16 && HD <= 256, "head_dim must be a multiple of 16 in [16, 256]");
     static constexpr int NC64 = HD / 64;
     static constexpr int REM = HD % 64;
     static_assert(REM == 0 || REM == 16 || REM == 32, "head_dim % 64 must be 0, 16 or 32");
@@ -133,6 +133,23 @@ inline int attn_head_chunk(int option, int n, int align) {
     return best > 0 ? best : n;
 }
 
+// Hides a shared-memory base address from the compiler's loop-invariant code motion, so that the wgmma descriptors built
+// from it are recomputed next to each MMA instead of being hoisted out of the step loop and held in registers.
+__device__ __forceinline__ void opaque(uint32_t& x) { asm volatile("" : "+r"(x)); }
+// Wait without the watchdog of mbar_wait, for waits with an MMA group in flight: ptxas serialises every wgmma of a kernel
+// that has a trap path (or any other divergent branch) while a group is in flight.
+__device__ __forceinline__ void mbar_spin(uint64_t* bar, uint32_t parity) {
+    asm volatile("{\n\t.reg .pred P1;\n\tWAIT_%=:\n\tmbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t@!P1 bra WAIT_%=;\n\t}"
+                 ::"r"(smem_u32(bar)), "r"(parity)
+                 : "memory");
+}
+// Arrive of lane 0 only, as a predicated instruction rather than a branch, for the same reason.
+__device__ __forceinline__ void mbar_arrive_lane0(uint64_t* bar, int lane) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.eq.s32 p, %1, 0;\n\t@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}" ::"r"(smem_u32(bar)),
+                 "r"(lane)
+                 : "memory");
+}
+
 // Locate the (document, q-tile) of a linear tile index by scanning cu_seqlens (B is small: a few docs per row).
 struct TileLoc {
     int doc_start;  // first token of the document
@@ -159,3 +176,17 @@ __device__ __forceinline__ TileLoc locate_tile(const int32_t* __restrict__ cu, i
 }
 
 }  // namespace dolo
+
+// Wide heads (head_dim 160, 192, 256; attention_wide.cu): the launches behind the head_dim switches of the attention entry
+// points, called after those have checked their arguments.  Same arguments and semantics as the narrow kernels'.
+int dolo_attn_wide_fwd(const void* qkv, int64_t row_stride, void* out, float* lse, const int32_t* cu_seqlens, int n_docs,
+                       int64_t T, int n_groups, int q_per_group, int head_dim, float softmax_scale, float dropout_p,
+                       uint32_t key0, uint32_t key1, const float* alibi_slopes, cudaStream_t st);
+// dK / dV and dQ, given Delta (attn_delta_kernel) in `delta` [n_heads, T]
+int dolo_attn_wide_bwd(const void* dout, const void* qkv, int64_t row_stride, const float* lse, const float* delta,
+                       void* dqkv, const int32_t* cu_seqlens, int n_docs, int64_t T, int n_groups, int q_per_group,
+                       int head_dim, float softmax_scale, float dropout_p, uint32_t key0, uint32_t key1,
+                       const float* alibi_slopes, cudaStream_t st);
+int dolo_attn_wide_decode(const void* qkv, int64_t row_stride, const void* k_cache, const void* v_cache,
+                          const int32_t* lens, void* out, int batch, int64_t L_max, int n_groups, int q_per_group,
+                          int head_dim, float softmax_scale, const float* alibi_slopes, cudaStream_t st);

@@ -148,7 +148,10 @@ int attn_decode(const void* qkv, int64_t row_stride, const void* k_cache, const 
         case 80: return launch_decode_any<80>(qkv, row_stride, k_cache, v_cache, lens, out, batch, L_max, n_groups, q_per_group, softmax_scale, alibi_slopes, st);
         case 96: return launch_decode_any<96>(qkv, row_stride, k_cache, v_cache, lens, out, batch, L_max, n_groups, q_per_group, softmax_scale, alibi_slopes, st);
         case 128: return launch_decode_any<128>(qkv, row_stride, k_cache, v_cache, lens, out, batch, L_max, n_groups, q_per_group, softmax_scale, alibi_slopes, st);
-        default: return dolo_set_error("attn_decode: unsupported head_dim %d (supported: 16,32,64,80,96,128)", head_dim);
+        case 160: case 192: case 256:
+            return dolo_attn_wide_decode(qkv, row_stride, k_cache, v_cache, lens, out, batch, L_max, n_groups, q_per_group,
+                                         head_dim, softmax_scale, alibi_slopes, st);
+        default: return dolo_set_error("attn_decode: unsupported head_dim %d (supported: 16,32,64,80,96,128,160,192,256)", head_dim);
     }
 }
 

@@ -293,7 +293,10 @@ int attn_fwd(const void* qkv, int64_t row_stride, void* out, float* lse, const i
         case 80: return ab ? launch_fwd<80, true>(qkv, row_stride, p, st) : launch_fwd<80, false>(qkv, row_stride, p, st);
         case 96: return ab ? launch_fwd<96, true>(qkv, row_stride, p, st) : launch_fwd<96, false>(qkv, row_stride, p, st);
         case 128: return ab ? launch_fwd<128, true>(qkv, row_stride, p, st) : launch_fwd<128, false>(qkv, row_stride, p, st);
-        default: return dolo_set_error("attn_fwd: unsupported head_dim %d (supported: 16,32,64,80,96,128)", head_dim);
+        case 160: case 192: case 256:
+            return dolo_attn_wide_fwd(qkv, row_stride, out, lse, cu_seqlens, n_docs, T, n_groups, q_per_group, head_dim,
+                                      softmax_scale, dropout_p, key0, key1, alibi_slopes, st);
+        default: return dolo_set_error("attn_fwd: unsupported head_dim %d (supported: 16,32,64,80,96,128,160,192,256)", head_dim);
     }
 }
 

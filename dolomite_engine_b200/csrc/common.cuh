@@ -132,6 +132,11 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// producer side of a named barrier: signals without waiting; the shared-memory writes before it are visible to the
+// threads that pass named_bar_sync on the same barrier
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t nthreads) {
+    asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 
 // ---------------- 8x8 b16 matrix moves (the register layout of an m64nNk16 accumulator's bf16 pairs) ----------------
 // Lane t names row t % 8 of matrix t / 8; register i holds, for matrix i, row lane / 4, columns 2 (lane % 4) and +1.

@@ -225,8 +225,9 @@ def check_supported(cfg: CommonConfig, *, attention_implementation: str = "flash
     # dropout > 0: identity in eval mode; in training mode the residual / embedding dropouts are elementwise kernels
     # (csrc/dropout.cu) and the attention-probability dropout lives inside the attention kernels
     hd = cfg.n_embd // cfg.n_head
-    if hd not in (16, 32, 64, 80, 96, 128):
-        raise NotImplementedError(f"head_dim={hd}: supported head dims are 16, 32, 64, 80, 96, 128")
+    # 16 .. 128: the attention kernels of attention_fwd.cu / attention_bwd.cu; 160, 192, 256: attention_wide.cu
+    if hd not in (16, 32, 64, 80, 96, 128, 160, 192, 256):
+        raise NotImplementedError(f"head_dim={hd}: supported head dims are 16, 32, 64, 80, 96, 128, 160, 192, 256")
     if cfg.model_type == "moe_dolomite":
         # any expert count up to the routing kernels' 256 (router buffers: kernels.router_logits / router_grad) and any
         # width the dense model takes (the grouped expert GEMMs zero-fill each expert's own K and N tails)

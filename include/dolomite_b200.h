@@ -447,6 +447,7 @@ int dolomite_b200_moe_router_bwd_aux(const void* router_logits, const int32_t* s
  *   qkv: packed projection output [T, row_stride] in the slot layout described at rope_qk_inplace.
  *   out: [T, n_heads*head_dim] bf16; lse: fp32 [n_heads, T] (natural log-sum-exp of scale*s).
  *   cu_seqlens int32 [B+1] (same for q and k), causal within each document.
+ *   head_dim: 16, 32, 64, 80, 96, 128, 160, 192 or 256 (the same for attn_decode); any other value returns an error.
  *   bwd: dqkv has the same layout as qkv (dq, dk, dv written into their slots; bf16).
  *   workspace sizes via the *_workspace_bytes helpers.
  * ------------------------------------------------------------------------------------------------ */
