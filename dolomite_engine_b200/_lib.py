@@ -49,6 +49,7 @@ SIGNATURES: dict[str, tuple] = {
     "dolomite_b200_swiglu_bwd_bias": (_I, [_P, _P, _P, _P, _L, _L, _P]),
     "dolomite_b200_embedding_fwd": (_I, [_P, _P, _P, _L, _I, _L, _F, _P]),
     "dolomite_b200_embedding_bwd": (_I, [_P, _P, _P, _L, _I, _L, _F, _P]),
+    "dolomite_b200_embedding_fwd_neft": (_I, [_P, _P, _P, _L, _I, _L, _U, _U, _F, _P]),
     "dolomite_b200_cross_entropy_fwd_bwd": (_I, [_P, _L, _P, _P, _P, _P, _P, _L, _L, _L, _F, _F, _P]),
     "dolomite_b200_cross_entropy_count": (_I, [_P, _L, _L, _P, _P]),
     "dolomite_b200_cross_entropy_rows": (_I, [_P, _L, _P, _P, _P, _P, _L, _L, _L, _F, _F, _P]),
@@ -162,7 +163,7 @@ KERNELS_PER_CALL = {
     "dolomite_b200_layernorm_fwd": 1, "dolomite_b200_layernorm_bwd": 3, "dolomite_b200_gelu_fwd": 1,
     "dolomite_b200_gelu_bwd": 1, "dolomite_b200_swiglu_fwd": 1, "dolomite_b200_swiglu_bwd": 1, "dolomite_b200_swiglu_bwd_bias": 1,
     "dolomite_b200_act_fwd": 1, "dolomite_b200_act_bwd": 1,
-    "dolomite_b200_embedding_fwd": 1,
+    "dolomite_b200_embedding_fwd": 1, "dolomite_b200_embedding_fwd_neft": 1,
     "dolomite_b200_embedding_bwd": 1, "dolomite_b200_cross_entropy_fwd_bwd": 3, "dolomite_b200_colsum_accum": 1,
     "dolomite_b200_scale_bf16_by_device_scalar": 1, "dolomite_b200_add_scaled": 1, "dolomite_b200_sumsq_accum": 2,
     "dolomite_b200_clip_coef": 1, "dolomite_b200_adamw_step": 1, "dolomite_b200_cast_f32_to_bf16": 1,

@@ -142,7 +142,8 @@ def save_checkpoint(args, model, optimizer, lr_scheduler, train_dataloader, expe
     rng = {"random_rng_state": random.getstate(), "np_rng_state": np.random.get_state(), "torch_rng_state": torch.get_rng_state(),
            "cuda_rng_state": torch.cuda.get_rng_state() if torch.cuda.is_available() else None}
     eng = _engine(model)
-    if getattr(eng, "has_dropout", False):  # counter-based dropout masks: (seed, passes so far) is the whole generator state
+    # counter-based dropout masks and NEFTune noise: (seed, passes so far) is the whole generator state
+    if getattr(eng, "uses_pass_seed", False):
         rng["dolomite_b200_dropout_state"] = (eng.dropout_seed, eng._dropout_passes)
     if rank == 0 and getattr(eng, "fp8", None) is not None:  # identical on every rank (amaxes are all-reduced)
         torch.save(eng.fp8.state_dict(), os.path.join(save_path, FP8_RECIPE_FILE))

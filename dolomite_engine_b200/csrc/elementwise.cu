@@ -783,6 +783,37 @@ __global__ void __launch_bounds__(kThreads)
     }
 }
 
+// wte(ids) + NEFTune noise (model_wrapper/base.py:246-267 in training mode): x + zeros_like(x).uniform_(-mag, mag) on a bf16
+// x, with the rounding points of torch's CUDA uniform kernel (ATen/native/cuda/DistributionTemplates.h `uniform_kernel`):
+//   from = bf16(-mag), to = bf16(mag), range = fp32(bf16(to - from)),
+//   v = bf16(u * range + from) in fp32 with u in (0, 1] -- here __fmul_rn then __fadd_rn: no contraction to an FMA --
+//   v == to -> from, out = bf16(x + v).
+// u = ((h >> 8) + 1) * 2^-24 with h = dropout_hash_flat(t * H + c, key0, key1): 2^24 equally likely values in (0, 1], each
+// exact in fp32.  The caller passes bf16(-mag) / bf16(mag) / range as floats (`from`, `to`, `range`).
+__global__ void __launch_bounds__(kThreads)
+    embedding_fwd_neft_kernel(const int64_t* __restrict__ ids, const uint4* __restrict__ wte, uint4* __restrict__ out,
+                              int64_t T, int H8, int64_t V, uint32_t key0, uint32_t key1, float from, float to, float range) {
+    for (int64_t t = blockIdx.x; t < T; t += gridDim.x) {
+        int64_t id = ids[t];
+        id = id < 0 ? 0 : (id >= V ? V - 1 : id);
+        const uint4* src = wte + id * H8;
+        for (int i = threadIdx.x; i < H8; i += blockDim.x) {
+            float f[8];
+            unpack8(__ldg(src + i), f);
+            const uint64_t e0 = (uint64_t(t) * uint64_t(H8) + uint64_t(i)) * 8;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const uint32_t h = dropout_hash_flat(e0 + j, key0, key1);
+                const float u = float((h >> 8) + 1u) * 5.9604644775390625e-8f;  // 2^-24
+                float v = bf16_round(__fadd_rn(__fmul_rn(u, range), from));
+                v = v == to ? from : v;
+                f[j] = __fadd_rn(f[j], v);
+            }
+            out[t * H8 + i] = pack8(f);
+        }
+    }
+}
+
 // One warp per token.  The warp of the FIRST token with a given id owns that row of dwte and adds the rows of all tokens
 // with that id in ascending token order: a fixed summation order (bit-identical runs) without atomics.
 __device__ __forceinline__ int64_t clamp_id(int64_t id, int64_t V) { return id < 0 ? 0 : (id >= V ? V - 1 : id); }
@@ -1543,6 +1574,23 @@ extern "C" int dolomite_b200_embedding_fwd(const int64_t* ids, const void* wte, 
     embedding_fwd_kernel<<<grid, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
         ids, static_cast<const uint4*>(wte), static_cast<uint4*>(out), T, H / 8, V, scale, scale != 1.f);
     DOLO_LAUNCH_OK("embedding_fwd");
+    return DOLO_OK;
+}
+
+extern "C" int dolomite_b200_embedding_fwd_neft(const int64_t* ids, const void* wte, void* out, int64_t T, int H, int64_t V,
+                                                uint32_t key0, uint32_t key1, float mag, void* stream) {
+    DOLO_REQUIRE(H > 0 && H % 8 == 0, "embedding_fwd_neft: H=%d must be a multiple of 8", H);
+    DOLO_REQUIRE(aligned16(wte) && aligned16(out), "embedding_fwd_neft: pointers must be 16-byte aligned");
+    DOLO_REQUIRE(mag > 0.f && mag < 1e30f, "embedding_fwd_neft: mag=%g must be positive and finite", double(mag));
+    if (T == 0) return DOLO_OK;
+    // the bounds and the range as torch's uniform_kernel forms them for a bf16 tensor
+    const float from = __bfloat162float(__float2bfloat16_rn(-mag));
+    const float to = __bfloat162float(__float2bfloat16_rn(mag));
+    const float range = __bfloat162float(__float2bfloat16_rn(to - from));
+    const int grid = int(T < int64_t(dolo_num_sms()) * 16 ? T : int64_t(dolo_num_sms()) * 16);
+    embedding_fwd_neft_kernel<<<grid, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+        ids, static_cast<const uint4*>(wte), static_cast<uint4*>(out), T, H / 8, V, key0, key1, from, to, range);
+    DOLO_LAUNCH_OK("embedding_fwd_neft");
     return DOLO_OK;
 }
 

@@ -246,7 +246,15 @@ class DolomiteEngine:
 
     def __init__(self, cfg: CommonConfig, device, world_size: int = 1, rank: int = 0, seed: int | None = 42,
                  init_on_device: bool = False, attention_implementation: str = "flash_attention_2",
-                 use_padding_free_transformer: bool = True, moe_implementation: str = "eager"):
+                 use_padding_free_transformer: bool = True, moe_implementation: str = "eager",
+                 resize_vocab_to: int | None = None):
+        """`resize_vocab_to`: build the model at cfg.vocab_size and resize its vocabulary to this size
+        (`resize_token_embeddings`, hf_models.utils.resize_vocab_rows) before the root unit is sharded, so every rank draws the
+        same new rows and the flat layout is that of a model built at the new size.  Updates cfg.vocab_size."""
+        old_root = None
+        if resize_vocab_to is not None and int(resize_vocab_to) != cfg.vocab_size:
+            old_root = FlatUnit("root", _root_specs(cfg))  # layout of the full root at the old size (never allocated)
+            cfg.vocab_size = int(resize_vocab_to)
         check_supported(cfg, attention_implementation=attention_implementation,
                         use_padding_free_transformer=use_padding_free_transformer, moe_implementation=moe_implementation)
         self.cfg = cfg
@@ -268,6 +276,10 @@ class DolomiteEngine:
         self.dropout_seed: int | None = None  # None: torch.initial_seed() mixed with the rank on first use
         self._dropout_passes = 0
         self._dropout_now: int | None = None  # seed of the pass being run / backpropagated; None = no dropout (eval)
+        # NEFTune (research_args.neft_alpha, model_wrapper/base.py:246-267): uniform noise of bound neft_alpha / sqrt(numel) on
+        # wte(ids) in training passes.  Its keys come from the pass seed above (site NEFT_SITE), so a NEFTune model draws a
+        # pass seed even without dropout; models without NEFTune count passes exactly as before.
+        self.neft_alpha: float | None = None
         self.units: list[FlatUnit] = [FlatUnit("root", _root_specs(cfg), world_size, rank)]
         for i in range(cfg.n_layer):
             self.units.append(FlatUnit(f"h.{i}", _block_specs(cfg, i), world_size, rank))
@@ -276,7 +288,14 @@ class DolomiteEngine:
         if seed is not None:
             g = torch.Generator(device=self.device if init_on_device else "cpu").manual_seed(seed)
             for u in self.units:
-                u.full_master_from(u.init_full(g))
+                if u is self.units[0] and old_root is not None:
+                    from .hf_models.utils import resize_vocab_state
+
+                    full = old_root.init_full(g).cpu()
+                    old = {s.name: full[s.offset : s.offset + s.numel].view(s.shape) for s in old_root.specs}
+                    u.full_master_from(self._flat_root(resize_vocab_state(old, cfg.vocab_size)))
+                else:
+                    u.full_master_from(u.init_full(g))
         self._setup_rope()
         # ALiBi: the slopes stay on the device (a non-persistent buffer in the reference: not part of the state dict).
         # Whether a pass applies the bias is decided per forward (`alibi=`), as the reference decides per call
@@ -526,8 +545,16 @@ class DolomiteEngine:
     def _drop_keys(self, site: int) -> tuple[int, int]:
         return K.dropout_keys(self._dropout_now, site)
 
+    # call site of the NEFTune noise: no dropout site is negative
+    NEFT_SITE = -1
+
+    @property
+    def uses_pass_seed(self) -> bool:
+        """whether training passes draw a seed (dropout masks or NEFTune noise): the state checkpoints save"""
+        return self.has_dropout or bool(self.neft_alpha)
+
     def _begin_dropout_pass(self) -> None:
-        if not (self.has_dropout and self.training):
+        if not (self.uses_pass_seed and self.training):
             self._dropout_now = None
             return
         if self.dropout_seed is None:
@@ -578,7 +605,7 @@ class DolomiteEngine:
 
     def forward(self, input_ids, position_ids, cu_seqlens, max_seqlen: int, labels=None, ignore_index: int = -100,
                 save_for_backward: bool = True, fuse_head_loss: bool = False, alibi: bool = False,
-                router_aux: bool = False, T_real: int | None = None, coef: float = 0.0):
+                router_aux: bool = False, T_real: int | None = None, coef: float = 0.0, neft_numel: int | None = None):
         """Returns (logits_or_None, loss_or_None).  input_ids int64 [T]; cu_seqlens int32 [B+1].
         `fuse_head_loss`: the caller will backpropagate d(loss) = 1 (what train_step does), so the LM head's backward can run
         chunk-wise inside the loss computation and the [T, V] logits are never materialised.
@@ -586,7 +613,9 @@ class DolomiteEngine:
         False runs an alibi model as NoPE, which is what the reference's SDPA attention does without an attention mask.
         `router_aux` (MoE): also compute the load-balancing loss aux over the first `T_real` token rows (default: all) of
         every layer, add `coef * aux` to the loss, and return (logits_or_None, loss_or_None, aux [1] fp32, router logits:
-        one bf16 [T, E] tensor per layer).  backward(aux_grad_dev=...) then takes s = coef * dL/dloss + dL/daux."""
+        one bf16 [T, E] tensor per layer).  backward(aux_grad_dev=...) then takes s = coef * dL/dloss + dL/daux.
+        `neft_numel`: the element count of the reference's wte output, which sets the NEFTune bound (default T * n_embd);
+        a padded batch passes B * S * n_embd."""
         cfg = self.cfg
         self._aux_fwd = None
         if router_aux:
@@ -608,10 +637,17 @@ class DolomiteEngine:
             comm.pre_forward_unit(0)
         m_emb = 1.0 if cfg.m_emb is None else float(cfg.m_emb)
         p_emb = self._drop_p("embd_pdrop")
-        # gpt_dolomite/base.py:351-372: drop(wte(ids) [+ wpe(position_ids)]) * m_emb.  Without dropout and learned positions the
-        # scale rides on the gather; otherwise it is a separate bf16 multiply after the sum / the mask (p = 0: all kept).
-        post_scale = p_emb > 0 or (self.learned_positions and m_emb != 1.0)
-        h = K.embedding_fwd(input_ids, root.views["transformer.wte.weight"], 1.0 if post_scale else m_emb)
+        neft = self._dropout_now is not None and bool(self.neft_alpha)
+        # gpt_dolomite/base.py:351-372: drop(wte(ids) [+ wpe(position_ids)]) * m_emb.  Without dropout, NEFTune and learned
+        # positions the scale rides on the gather; otherwise it is a separate bf16 multiply after the sum / the mask (p = 0: all
+        # kept).  NEFTune noise is added to wte(ids) itself, before everything else.
+        post_scale = p_emb > 0 or neft or (self.learned_positions and m_emb != 1.0)
+        if neft:
+            numel = T * cfg.n_embd if neft_numel is None else int(neft_numel)
+            h = K.embedding_fwd_neft(input_ids, root.views["transformer.wte.weight"], self._drop_keys(self.NEFT_SITE),
+                                     K.neft_mag(self.neft_alpha, numel))
+        else:
+            h = K.embedding_fwd(input_ids, root.views["transformer.wte.weight"], 1.0 if post_scale else m_emb)
         if self.learned_positions:  # wte(ids) + wpe(position_ids), one bf16 rounding
             if position_ids.dtype != torch.int64:
                 position_ids = position_ids.long()
@@ -675,7 +711,7 @@ class DolomiteEngine:
             self._saved = dict(input_ids=input_ids, position_ids=position_ids, cu_seqlens=cu_seqlens, max_seqlen=max_seqlen,
                                layers=saved_layers, h_last=h, rstd_f=rstd_f, hf=hf, dlogits=dlogits, d_hf=d_hf, T=T,
                                dropout_seed=self._dropout_now, fp8=self._fp8_now, alibi=self._alibi_now,
-                               router_aux=router_aux_saved)
+                               router_aux=router_aux_saved, emb_post_scale=post_scale)
         self._fp8_now = False
         self._fp8_wcache.clear()
         if router_aux_saved is not None:
@@ -981,7 +1017,7 @@ class DolomiteEngine:
                 comm.post_backward_unit(i + 1)
         m_emb = 1.0 if cfg.m_emb is None else float(cfg.m_emb)
         p_emb = self._drop_p("embd_pdrop")
-        if p_emb > 0 or (self.learned_positions and m_emb != 1.0):
+        if s["emb_post_scale"]:
             dh = K.dropout_bwd(dh, p_emb, self._drop_keys(0) if p_emb > 0 else (0, 0), pre_mul=m_emb, out=dh)
             m_emb = 1.0
         K.embedding_bwd(s["input_ids"], dh, root.gviews["transformer.wte.weight"], m_emb)
@@ -1013,6 +1049,14 @@ class DolomiteEngine:
         if self.world_size == 1:
             return unit.master.detach()
         return self.comm.gather_master(unit)
+
+    def _flat_root(self, sd: dict) -> torch.Tensor:
+        """the full flat fp32 root unit of a state dict holding every root parameter"""
+        root = self.units[0]
+        full = torch.zeros(root.padded, dtype=torch.float32)
+        for s in root.specs:
+            full[s.offset : s.offset + s.numel].view(s.shape).copy_(sd[s.name])
+        return full
 
     def state_dict(self) -> dict:
         out = {}

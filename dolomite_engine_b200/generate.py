@@ -68,7 +68,8 @@ def main() -> None:
                                           model_class=m.model_class, dtype=torch.bfloat16,
                                           attention_implementation=m.attention_implementation or "flash_attention_2",
                                           use_padding_free_transformer=False, random_seed=args.random_args.seed,
-                                          tokenizer_name=args.tokenizer_args.tokenizer_name, device=device)
+                                          tokenizer_name=args.tokenizer_args.tokenizer_name,
+                                          additional_special_tokens=args.tokenizer_args.additional_special_tokens, device=device)
     else:
         from .checkpointing import load_checkpoint_for_inference
 

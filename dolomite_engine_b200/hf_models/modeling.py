@@ -60,11 +60,12 @@ class _EngineFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, anchor, model, input_ids, position_ids, cu_seqlens, max_seqlen, labels, ignore_index, save=True,
-                alibi=False, router_aux=None):
+                alibi=False, router_aux=None, neft_numel=None):
         # `save`: the caller's torch.is_grad_enabled() (always False in here); under no_grad (evaluation) no activation is kept
         # `alibi`: the pass adds the ALiBi bias (DolomitePreTrainedModel._alibi_pass)
         # `router_aux`: None, or (T_real, coef) of the MoE load-balancing loss.  The outputs are then (loss or logits,
         # aux_loss, router logits of every layer); the router logits are not differentiable
+        # `neft_numel`: element count of the reference's wte output (NEFTune bound); None = the packed stream's T * n_embd
         engine = model.engine
         ctx.model = model
         ctx.loss_mode = labels is not None
@@ -73,7 +74,8 @@ class _EngineFunction(torch.autograd.Function):
             T_real, coef = router_aux
             logits, loss, aux, router_logits = engine.forward(
                 input_ids, position_ids, cu_seqlens, max_seqlen, labels=labels, ignore_index=ignore_index,
-                save_for_backward=bool(save), alibi=bool(alibi), router_aux=True, T_real=T_real, coef=coef)
+                save_for_backward=bool(save), alibi=bool(alibi), router_aux=True, T_real=T_real, coef=coef,
+                neft_numel=neft_numel)
             ctx.mark_non_differentiable(*router_logits)
             return (loss.reshape(()) if ctx.loss_mode else logits, aux.reshape(())) + tuple(router_logits)
         # `assume_unit_loss_grad` (set by the training wrappers: train_step calls loss.backward() on the raw loss) lets the
@@ -81,7 +83,7 @@ class _EngineFunction(torch.autograd.Function):
         logits, loss = engine.forward(input_ids, position_ids, cu_seqlens, max_seqlen, labels=labels,
                                       ignore_index=ignore_index, save_for_backward=bool(save),
                                       fuse_head_loss=bool(save) and labels is not None and model.assume_unit_loss_grad,
-                                      alibi=bool(alibi))
+                                      alibi=bool(alibi), neft_numel=neft_numel)
         return loss.reshape(()) if ctx.loss_mode else logits
 
     @staticmethod
@@ -104,7 +106,7 @@ class _EngineFunction(torch.autograd.Function):
             engine.backward(grad_scale_dev=scale)
         else:
             engine.backward(dlogits=grad_out.contiguous())
-        return (None,) * 11
+        return (None,) * 12
 
 
 def _pad_packed_stream(input_ids, position_ids, cu_seqlens, shift_labels, multiple: int = 8):
@@ -146,6 +148,7 @@ class DolomitePreTrainedModel(nn.Module):
         rank = kwargs.pop("rank", 0)
         seed = kwargs.pop("seed", 42)
         init_on_device = kwargs.pop("init_on_device", False)
+        resize_vocab_to = kwargs.pop("resize_vocab_to", None)  # resize_token_embeddings before sharding (DolomiteEngine)
         if kwargs.pop("tensor_parallel_word_embeddings", False) or kwargs.pop("sequence_parallel", False):
             raise NotImplementedError("tensor / sequence parallelism is out of scope of the data-parallel B200 path")
         if kwargs:
@@ -167,7 +170,7 @@ class DolomitePreTrainedModel(nn.Module):
         self.engine = DolomiteEngine(config, device, world_size=world_size, rank=rank, seed=seed, init_on_device=init_on_device,
                                      attention_implementation=self.attention_implementation,
                                      use_padding_free_transformer=self._use_padding_free_transformer,
-                                     moe_implementation=self.moe_implementation)
+                                     moe_implementation=self.moe_implementation, resize_vocab_to=resize_vocab_to)
         self.flat_params = nn.ParameterList([u.master for u in self.engine.units])
         self._anchor = torch.zeros(1, device=device, requires_grad=True)
         self.assume_unit_loss_grad = False
@@ -234,7 +237,9 @@ class DolomitePreTrainedModel(nn.Module):
             shift_labels[drop] = -100
         input_ids, position_ids, cu_seqlens, shift_labels, T_real = _pad_packed_stream(input_ids, position_ids, cu_seqlens,
                                                                                        shift_labels, self._token_multiple())
-        out = _EngineFunction.apply(self._anchor, self, input_ids, position_ids, cu_seqlens, int(max_seqlen), shift_labels, -100, torch.is_grad_enabled())
+        # NEFTune's bound uses the reference's wte output, the T_real tokens of the lists (not the multiple-of-8 pad)
+        out = _EngineFunction.apply(self._anchor, self, input_ids, position_ids, cu_seqlens, int(max_seqlen), shift_labels, -100,
+                                    torch.is_grad_enabled(), False, None, T_real * self.config.n_embd)
         if shift_labels is not None:
             result = CausalLMOutputWithPast(loss=out, logits=None)
         else:
@@ -306,7 +311,8 @@ class DolomitePreTrainedModel(nn.Module):
         ids_p, pos_p, cu, shift_labels, T_real = _pad_packed_stream(ids_p, pos_p, cu, shift_labels, self._token_multiple())
         router_aux = (T_real, float(self.config.router_aux_loss_coef)) if output_router_logits else None
         out = _EngineFunction.apply(self._anchor, self, ids_p, pos_p, cu, int(max(max_seqlen, 1)), shift_labels, -100,
-                                    torch.is_grad_enabled(), self._alibi_pass(attention_mask is not None), router_aux)
+                                    torch.is_grad_enabled(), self._alibi_pass(attention_mask is not None), router_aux,
+                                    B * S * self.config.n_embd)  # NEFTune: the reference's wte sees [B, S], padding included
         aux_loss = router_logits = None
         if router_aux is not None:
             out, aux_loss, packed_router = out[0], out[1], out[2:]
@@ -375,8 +381,16 @@ class DolomitePreTrainedModel(nn.Module):
         with open(os.path.join(path, "config.json")) as f:
             d = json.load(f)
         config = config_class_for(d["model_type"]).from_dict(d)
-        model = cls(config, seed=None, **kwargs)
         sd = SafeTensorsWeightsManager(path).state_dict()
+        resize_vocab_to = kwargs.pop("resize_vocab_to", None)
+        if resize_vocab_to is not None and int(resize_vocab_to) != config.vocab_size:
+            # resize_token_embeddings on the full host tensors, before the model (and so its root unit) is sharded
+            from .utils import resize_vocab_state
+
+            sd = resize_vocab_state({k: v.float() if k in ("transformer.wte.weight", "lm_head.weight") else v
+                                     for k, v in sd.items()}, int(resize_vocab_to))
+            config.vocab_size = int(resize_vocab_to)
+        model = cls(config, seed=None, **kwargs)
         model.load_state_dict(sd)
         return model
 

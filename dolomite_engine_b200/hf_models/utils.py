@@ -7,6 +7,8 @@ SURVEY.md section 3.2).
 
 from __future__ import annotations
 
+import math
+
 import numpy as np
 import torch
 
@@ -102,3 +104,47 @@ def prepare_pretraining_inputs_host(
         "position_ids": pos,
         "max_seqlen": max_seqlen,
     }
+
+
+def resize_vocab_rows(old: torch.Tensor, new_num_tokens: int, lm_head: bool) -> torch.Tensor:
+    """One [V, H] matrix of `PreTrainedModel.resize_token_embeddings(new_num_tokens)` (transformers 5.5, mean_resizing=True,
+    no pad_to_multiple_of): `old` (fp32, host) -> [new_num_tokens, H].  Rows below min(V, new) are copied; added rows are
+    drawn from N(mean, 1e-9 * covariance) of the old rows when that covariance is positive definite, else set to the mean.
+    Draws from torch's global CPU generator in transformers' order: the new module's default init first (nn.Embedding:
+    normal_; the untied head, an nn.Linear: kaiming_uniform_ = uniform_(-1/sqrt(H), 1/sqrt(H))), then the sample."""
+    from torch.distributions import constraints
+    from torch.distributions.multivariate_normal import MultivariateNormal
+
+    V, H = old.shape
+    if new_num_tokens == V:
+        return old
+    new = torch.empty(new_num_tokens, H, dtype=old.dtype)
+    if lm_head:
+        torch.nn.init.kaiming_uniform_(new, a=math.sqrt(5))
+    else:
+        torch.nn.init.normal_(new)
+    if new_num_tokens > V:
+        added = new_num_tokens - V
+        w = old.to(torch.float32)
+        mean = torch.mean(w, axis=0)
+        centered = w - mean
+        covariance = centered.T @ centered / V
+        eps = 1e-9
+        if constraints.positive_definite.check(eps * covariance).all():
+            new[-added:, :] = MultivariateNormal(mean, covariance_matrix=eps * covariance).sample(
+                sample_shape=(added,)).to(old.dtype)
+        else:
+            new[-added:, :] = mean[None, :].repeat(added, 1).to(old.dtype)
+    n = min(V, new_num_tokens)
+    new[:n, :] = old[:n, :]
+    return new
+
+
+def resize_vocab_state(sd: dict, new_num_tokens: int) -> dict:
+    """`resize_token_embeddings(new_num_tokens)` of a GPTDolomite / MoEDolomite state dict (host fp32 tensors): wte, then
+    the untied lm_head (a tied head has no entry of its own); other entries are passed through"""
+    out = dict(sd)
+    out["transformer.wte.weight"] = resize_vocab_rows(sd["transformer.wte.weight"], new_num_tokens, lm_head=False)
+    if "lm_head.weight" in sd:
+        out["lm_head.weight"] = resize_vocab_rows(sd["lm_head.weight"], new_num_tokens, lm_head=True)
+    return out

@@ -299,6 +299,26 @@ def embedding_fwd(ids, wte, scale: float = 1.0, out=None):
     return y
 
 
+def neft_mag(alpha: float, numel: int) -> float:
+    """NEFTune's noise bound as the reference computes it (model_wrapper/base.py:262):
+    `alpha / torch.sqrt(torch.tensor(numel))` on the host, in fp32.  The same expression is evaluated here: numel rounds
+    to fp32 above 2^24, `float / Tensor` is reciprocal(sqrt) * alpha, and torch's CPU sqrt is not always the correctly
+    rounded one, so a restatement in another library differs in the last bit for some numel."""
+    return float(alpha / torch.sqrt(torch.tensor(int(numel))))
+
+
+def embedding_fwd_neft(ids, wte, keys: tuple[int, int], mag: float, out=None):
+    """wte[ids] + uniform(-mag, mag) NEFTune noise in bf16 (csrc/elementwise.cu embedding_fwd_neft_kernel); the noise is a
+    pure function of `keys` (dropout_keys) and the flat element index"""
+    _req(ids, torch.int64, "ids"), _req(wte, _BF16, "wte")
+    T = ids.numel()
+    V, H = wte.shape
+    y = torch.empty(T, H, dtype=_BF16, device=wte.device) if out is None else out
+    _lib.call("dolomite_b200_embedding_fwd_neft", ids.data_ptr(), wte.data_ptr(), y.data_ptr(), T, H, V, keys[0], keys[1],
+              float(mag), _stream())
+    return y
+
+
 def embedding_bwd(ids, dout, dwte_accum, scale: float = 1.0):
     _req(ids, torch.int64, "ids"), _req(dout, _BF16, "dout"), _req(dwte_accum, torch.float32, "dwte")
     T = ids.numel()

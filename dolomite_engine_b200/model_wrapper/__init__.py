@@ -56,17 +56,13 @@ class ModelWrapper(nn.Module):
         self.random_seed = random_seed
         if tensor_parallel_word_embeddings or sequence_parallel:
             raise NotImplementedError("tensor / sequence parallelism is out of scope of the data-parallel B200 path")
-        if neft_alpha is not None and neft_alpha > 0:
-            raise NotImplementedError("NEFTune is out of scope of the B200 hot path (SURVEY.md section 2 #10)")
-        if additional_special_tokens:
-            raise NotImplementedError("tokenizer expansion is out of scope of the B200 hot path")
         if dtype not in (torch.bfloat16, "bf16"):
             raise NotImplementedError("the B200 path computes in bf16 with fp32 masters (mixed_precision_args.dtype: bf16)")
         self._setup_config()
         if self.use_padding_free_transformer:
             # model_wrapper/base.py:94-101
             assert self.attention_implementation == "flash_attention_2", "padding free transformer only works with flash attention"
-        self._setup_tokenizer()
+        self._setup_tokenizer(required=bool(additional_special_tokens))
         kwargs = dict(attn_implementation=self.attention_implementation,
                       use_padding_free_transformer=self.use_padding_free_transformer,
                       device=device, world_size=world_size, rank=rank, seed=random_seed, init_on_device=init_on_device)
@@ -74,11 +70,22 @@ class ModelWrapper(nn.Module):
             kwargs["moe_implementation"] = moe_implementation
         if normalization_implementation is not None:
             kwargs["normalization_implementation"] = normalization_implementation
+        if additional_special_tokens:
+            # model_wrapper/base.py:102-108: the model follows len(tokenizer) only when adding the tokens changed it -- which
+            # also shrinks a model whose vocab_size was padded above the tokenizer's length
+            original_vocab_size = len(self.tokenizer)
+            self.tokenizer.add_special_tokens({"additional_special_tokens": list(additional_special_tokens)})
+            if len(self.tokenizer) != original_vocab_size:
+                kwargs["resize_vocab_to"] = len(self.tokenizer)
         if self.model_name is None:
             self.model = AutoModelForCausalLM.from_config(self.config, **kwargs)
         else:
             kwargs.pop("seed")
             self.model = AutoModelForCausalLM.from_pretrained(self.model_name, **kwargs)
+        self.config.vocab_size = self.model.config.vocab_size
+        # model_wrapper/base.py:97-100: NEFTune in training mode; the engine adds the noise in training passes only
+        if str(getattr(mode, "value", mode)) not in ("inference", "unsharding") and neft_alpha is not None and neft_alpha > 0:
+            self.model.engine.neft_alpha = float(neft_alpha)
 
     def _setup_config(self) -> None:
         """model_wrapper/base.py:151-163"""
@@ -88,11 +95,13 @@ class ModelWrapper(nn.Module):
         else:
             self.config = CommonConfig.from_pretrained(self.model_name)
 
-    def _setup_tokenizer(self) -> None:
+    def _setup_tokenizer(self, required: bool = False) -> None:
         """model_wrapper/base.py:165-169.  Tokenizers come from the HF hub in the reference; offline we only need the
-        eos id, which the config carries."""
+        eos id, which the config carries -- unless tokens are to be added (`required`), which needs a local tokenizer."""
         self.tokenizer = None
         self.eos_token_id = self.config.eos_token_id
+        if self.tokenizer_name is None and required:
+            raise ValueError("additional_special_tokens needs a tokenizer: set tokenizer_args.tokenizer_name or model_args.model_name")
         if self.tokenizer_name is not None:
             try:
                 from transformers import AutoTokenizer
@@ -100,6 +109,9 @@ class ModelWrapper(nn.Module):
                 self.tokenizer = AutoTokenizer.from_pretrained(self.tokenizer_name)
                 self.eos_token_id = self.tokenizer.eos_token_id
             except (OSError, ValueError, ImportError) as e:  # not a local directory and no hub access: keep the config's eos id
+                if required:
+                    raise ValueError(f"additional_special_tokens needs a tokenizer, and {self.tokenizer_name!r} could not be "
+                                     f"loaded ({type(e).__name__}: {e})") from e
                 import warnings
 
                 warnings.warn(f"tokenizer {self.tokenizer_name!r} could not be loaded ({type(e).__name__}); continuing without "
@@ -230,6 +242,9 @@ def get_model(args, mode=None, device=None, world_size: int = 1, rank: int = 0) 
         attention_implementation=margs.attention_implementation or "flash_attention_2",
         use_padding_free_transformer=margs.use_padding_free_transformer,
         random_seed=args.random_args.seed,
+        neft_alpha=args.research_args.neft_alpha,
+        tokenizer_name=args.tokenizer_args.tokenizer_name,
+        additional_special_tokens=args.tokenizer_args.additional_special_tokens,
         moe_implementation=getattr(margs, "moe_implementation", None),
         normalization_implementation=getattr(margs, "normalization_implementation", None),
         device=device,

@@ -60,6 +60,8 @@ def unshard(load_path: str, unsharded_path: str, iteration: int | None = None, d
         if dtype is not None:
             t = t.to(getattr(torch, dtype))
         out[k[len(_PREFIX):]] = t.contiguous()
+    # a run with tokenizer_args.additional_special_tokens resized the vocabulary after building from pretrained_config
+    config.vocab_size = int(out["transformer.wte.weight"].shape[0])
     os.makedirs(unsharded_path, exist_ok=True)
     SafeTensorsWeightsManager.save_state_dict(out, unsharded_path)
     config.save_pretrained(unsharded_path)

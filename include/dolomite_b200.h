@@ -169,6 +169,13 @@ int dolomite_b200_embedding_fwd(const int64_t* ids, const void* wte, void* out, 
                                 float scale, void* stream);
 int dolomite_b200_embedding_bwd(const int64_t* ids, const void* dout, float* dwte, int64_t T, int H, int64_t V,
                                 float scale, void* stream);
+/* The gather with NEFTune noise (model_wrapper/base.py:246-267, training mode): out = bf16(wte[ids] + v) with
+ * v = uniform(-mag, mag) at the rounding points of torch's CUDA uniform kernel on a bf16 tensor (bounds and range in bf16,
+ * bf16(u * range + from) in fp32, a value equal to the upper bound becomes the lower one).  u in (0, 1] is a counter hash of
+ * the flat element index t * H + c under (key0, key1) (kernels.dropout_keys), so a pass's noise is a pure function of
+ * its keys.  mag: the reference's alpha / sqrt(numel), in fp32, > 0. */
+int dolomite_b200_embedding_fwd_neft(const int64_t* ids, const void* wte, void* out, int64_t T, int H, int64_t V,
+                                     uint32_t key0, uint32_t key1, float mag, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Cross entropy (mean over non-ignored tokens), fused forward + backward --
