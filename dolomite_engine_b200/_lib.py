@@ -118,6 +118,8 @@ SIGNATURES: dict[str, tuple] = {
         [_P, _P, _L, _P, _P, _P, _P, _I, _L, _I, _I, _I, _I, _F, _F, _U, _U, _P, _P, _P],
     ),
     "dolomite_b200_attn_decode_alibi": (_I, [_P, _L, _P, _P, _P, _P, _I, _L, _I, _I, _I, _F, _P, _P]),
+    "dolomite_b200_attn_cache": (_I, [_P, _L, _P, _P, _P, _P, _P, _I, _I, _I, _L, _I, _I, _I, _F, _P]),
+    "dolomite_b200_attn_cache_alibi": (_I, [_P, _L, _P, _P, _P, _P, _P, _I, _I, _I, _L, _I, _I, _I, _F, _P, _P]),
 }
 
 _lib = None

@@ -121,7 +121,9 @@ class FlatUnit:
 
 
 class KVCache:
-    """keys / values of every layer by position: k[l], v[l] bf16 [batch, max_len, n_kv_groups * head_dim]; lens int32 [batch]"""
+    """keys / values of every layer by position: k[l], v[l] bf16 [batch, max_len, n_kv_groups * head_dim]; lens int32 [batch]
+    (the real tokens cached per sequence, from position 0); `seen`: attention-mask columns passed so far, padding included,
+    which is what a HuggingFace cache's get_seq_length() reports"""
 
     def __init__(self, engine: "DolomiteEngine", batch: int, max_len: int):
         dim = engine.n_groups * engine.hd
@@ -130,6 +132,24 @@ class KVCache:
         self.v = [mk() for _ in range(engine.cfg.n_layer)]
         self.lens = torch.zeros(batch, dtype=torch.int32, device=engine.device)
         self.max_len = max_len
+        self.seen = 0
+
+    def get_seq_length(self, layer_idx: int = 0) -> int:
+        return self.seen
+
+    def reserve(self, need: int) -> None:
+        """room for `need` positions per sequence: the capacity doubles until it fits and the cached positions are copied"""
+        if need <= self.max_len:
+            return
+        new_len = max(self.max_len, 1)
+        while new_len < need:
+            new_len *= 2
+        for buf in (self.k, self.v):
+            for i, t in enumerate(buf):
+                grown = t.new_zeros(t.shape[0], new_len, t.shape[2])
+                grown[:, : self.max_len].copy_(t)
+                buf[i] = grown
+        self.max_len = new_len
 
 
 def _block_specs(cfg: CommonConfig, i: int) -> list[tuple[str, tuple, str]]:
@@ -773,20 +793,76 @@ class DolomiteEngine:
         with active[b] == False are computed but their cache does not advance) -> logits [B, V].  Every op is the training
         kernel at T = B rows, except attention, which is the single-query cache kernel (csrc/attention_decode.cu).
         `alibi`: ALiBi bias of each cache position (the cache holds the real tokens of a sequence from position 0)."""
-        cfg = self.cfg
         slopes = self._alibi_slopes_for(alibi)
         if self.comm is not None:
             raise NotImplementedError("decoding runs on an unsharded engine (world_size 1)")
         B = input_ids.numel()
-        root = self.units[0]
         pos = cache.lens.long()  # position of the new token = tokens already cached
         rows = torch.arange(B, device=self.device)
+        self._ensure_rope(int(cache.k[0].shape[1]))
+        lens_incl = (cache.lens + 1).contiguous()
+        logits = self._cached_pass(input_ids, pos, cache, rows, pos, lambda i, qkv: K.attn_decode(
+            qkv, cache.k[i], cache.v[i], lens_incl, self.n_groups, self.q_per_group, self.hd, self.softmax_scale,
+            alibi_slopes=slopes))
+        cache.lens.add_(1 if active is None else active.to(torch.int32))
+        return logits
+
+    @torch.no_grad()
+    def extend(self, input_ids, n_new: list[int], cache: "KVCache", position_ids=None, alibi: bool = False):
+        """n_new[b] >= 0 new tokens per sequence (host ints), input_ids int64 [sum n_new] packed sequence by sequence; their
+        keys / values are appended at cache.lens[b] + i, new token i of b attends to cache positions 0 .. cache.lens[b] + i,
+        and the cache grows (KVCache.reserve) when they do not fit -> logits [sum n_new, V].  `position_ids` [sum n_new]
+        (RoPE, learned positions) default to the cache position cache.lens[b] + i; `alibi`: ALiBi bias of each cache
+        position, as decode_step.  Every op is the training kernel at T = sum n_new rows; attention is attn_cache
+        (csrc/attention_cache.cu), or attn_decode when every n_new[b] == 1, the kernel decode_step (and so generate) runs."""
+        cfg = self.cfg
+        slopes = self._alibi_slopes_for(alibi)
+        if self.comm is not None:
+            raise NotImplementedError("decoding runs on an unsharded engine (world_size 1)")
+        B, T = len(n_new), int(sum(n_new))
+        if B != cache.lens.numel() or min(n_new, default=0) < 0 or input_ids.numel() != T:
+            raise ValueError(f"extend: {B} counts (>= 0) for a cache of {cache.lens.numel()} sequences and "
+                             f"{input_ids.numel()} tokens, summing to {T}")
+        dev = self.device
+        n_dev = torch.tensor(n_new, dtype=torch.int32, device=dev)
+        cu = torch.zeros(B + 1, dtype=torch.int32, device=dev)
+        cu[1:] = n_dev.cumsum(0)
+        end = int((cache.lens + n_dev).max()) if B else 0  # one host sync: the capacity check
+        if T == 0:
+            head = self.units[0].views["transformer.wte.weight" if cfg.tie_word_embeddings else "lm_head.weight"]
+            return torch.empty(0, head.shape[0], dtype=torch.bfloat16, device=dev)
+        seq = torch.repeat_interleave(torch.arange(B, device=dev), n_dev.long(), output_size=T)
+        slot = cache.lens.long()[seq] + torch.arange(T, device=dev) - cu.long()[seq]  # cache position of each new token
+        pos = slot if position_ids is None else position_ids.to(dev).long().reshape(-1)
+        top = end if position_ids is None else int(pos.max()) + 1
+        if self.learned_positions and top > cfg.n_positions:
+            raise ValueError(f"position {top - 1} is past the learned position table (n_positions={cfg.n_positions})")
+        cache.reserve(end)
+        self._ensure_rope(max(int(cache.k[0].shape[1]), top))
+        if all(x == 1 for x in n_new):
+            lens_incl = (cache.lens + 1).contiguous()
+            attend = lambda i, qkv: K.attn_decode(  # noqa: E731
+                qkv, cache.k[i], cache.v[i], lens_incl, self.n_groups, self.q_per_group, self.hd, self.softmax_scale,
+                alibi_slopes=slopes)
+        else:
+            past = cache.lens.clone()
+            attend = lambda i, qkv: K.attn_cache(  # noqa: E731
+                qkv, cu, past, cache.k[i], cache.v[i], self.n_groups, self.q_per_group, self.hd, self.softmax_scale,
+                max_new=max(n_new), max_end=end, alibi_slopes=slopes)
+        logits = self._cached_pass(input_ids, pos, cache, seq, slot, attend)
+        cache.lens.add_(n_dev)
+        return logits
+
+    def _cached_pass(self, input_ids, pos, cache: "KVCache", seq, slot, attend):
+        """the model over new tokens against `cache` (decode_step, extend): the keys / values of token t go to position
+        slot[t] of sequence seq[t] and `attend(i, qkv)` is the attention of layer i -> logits [T, V]"""
+        cfg = self.cfg
+        T = input_ids.numel()
+        root = self.units[0]
         h = K.embedding_fwd(input_ids, root.views["transformer.wte.weight"], 1.0 if cfg.m_emb is None else float(cfg.m_emb))
         if self.learned_positions:
             h = K.add_scaled(h, K.embedding_fwd(pos, root.views["transformer.wpe.weight"], 1.0), 1.0)
-        self._ensure_rope(int(cache.k[0].shape[1]))
         m_res = 1.0 if cfg.m_residual is None else float(cfg.m_residual)
-        lens_incl = (cache.lens + 1).contiguous()
         for i in range(cfg.n_layer):
             u = self.units[i + 1]
             p = f"transformer.h.{i}."
@@ -795,10 +871,9 @@ class DolomiteEngine:
             if self.rope_cos is not None:
                 K.rope_qk_inplace(qkv, self.n_groups, self.q_per_group, self.hd, self.rope_cos, self.rope_sin, pos)
             k_new, v_new = self.kv_slices(qkv)
-            cache.k[i][rows, pos] = k_new.reshape(B, -1)
-            cache.v[i][rows, pos] = v_new.reshape(B, -1)
-            attn = K.attn_decode(qkv, cache.k[i], cache.v[i], lens_incl, self.n_groups, self.q_per_group, self.hd, self.softmax_scale,
-                                 alibi_slopes=slopes)
+            cache.k[i][seq, slot] = k_new.reshape(T, -1)
+            cache.v[i][seq, slot] = v_new.reshape(T, -1)
+            attn = attend(i, qkv)
             h_mid = K.gemm(attn, u.views[p + "attn.c_proj.weight"], bias=u.views.get(p + "attn.c_proj.bias"), c=h, alpha=m_res,
                            beta=1.0)
             ln2, _ = self._norm_fwd(h_mid, u, p + "ln_2.")
@@ -814,7 +889,6 @@ class DolomiteEngine:
         hf, _ = self._norm_fwd(h, root, "transformer.ln_f.")
         head = root.views["transformer.wte.weight"] if cfg.tie_word_embeddings else root.views["lm_head.weight"]
         logits = K.gemm(hf, head, alpha=1.0 if cfg.m_width is None else 1.0 / float(cfg.m_width))
-        cache.lens.add_(1 if active is None else active.to(torch.int32))
         return logits.contiguous()
 
     # ------------------------------------------------------------------------------------------

@@ -24,13 +24,16 @@ from .utils import convert_padding_free_lists_to_tensors
 class CausalLMOutputWithPast:
     loss: torch.Tensor | None = None
     logits: torch.Tensor | None = None
-    past_key_values: None = None
+    past_key_values: object | None = None  # engine.KVCache of a call with use_cache=True or past_key_values
     hidden_states: None = None
     attentions: None = None
     router_logits: None = None
 
+    def to_tuple(self) -> tuple:
+        return tuple(v for v in (self.loss, self.logits, self.past_key_values) if v is not None)
+
     def __getitem__(self, i):
-        return tuple(v for v in (self.loss, self.logits) if v is not None)[i]
+        return self.to_tuple()[i]
 
 
 @dataclass
@@ -274,7 +277,8 @@ class DolomitePreTrainedModel(nn.Module):
         if output_router_logits and not self.engine.is_moe:
             raise ValueError("output_router_logits needs an MoE model (MoEDolomiteForCausalLM)")
         if use_cache or past_key_values is not None:
-            raise NotImplementedError("KV caching / generation is not implemented on the B200 training path")
+            return self._forward_cached(input_ids, attention_mask, position_ids, labels, return_dict, past_key_values,
+                                        inputs_embeds, token_type_ids, cu_seqlens, output_router_logits)
         if inputs_embeds is not None or token_type_ids is not None:
             raise NotImplementedError("inputs_embeds / token_type_ids are not supported on the B200 path")
         assert cu_seqlens is None, "cu_seqlens belongs to the padding-free transformer"
@@ -335,6 +339,80 @@ class DolomitePreTrainedModel(nn.Module):
         if not return_dict:
             return tuple(v for v in (result.loss, result.logits) if v is not None)
         return result
+
+    def _forward_cached(self, input_ids, attention_mask, position_ids, labels, return_dict, past_key_values, inputs_embeds,
+                        token_type_ids, cu_seqlens, output_router_logits: bool):
+        """Padded batch with a KV cache (gpt_dolomite/base.py:173-257): `use_cache=True` without `past_key_values` runs the
+        prompt through engine.prefill and returns the filled cache; with `past_key_values` (the KVCache of an earlier call),
+        input_ids [B, S] are the new tokens and engine.extend appends them.  attention_mask is [B, past + S] (HuggingFace:
+        the cache's get_seq_length() columns, then the new ones) or [B, S]; its last S columns decide which new tokens are
+        real, and masked tokens are neither cached nor attended to.  position_ids default to the reference's
+        `cumsum(mask) - 1`, the number of real tokens before each one (base.py:247-257); given ones are used for the new
+        tokens.  ALiBi biases by cache position, under the rule of _alibi_pass.  Logits are [B, S, V], 0 at masked
+        positions; labels give the loss of the chunk as _forward_padded computes it."""
+        from ..engine import KVCache
+        from .. import kernels as K
+
+        if past_key_values is not None and not isinstance(past_key_values, KVCache):
+            raise TypeError(f"past_key_values must be the KVCache an earlier call of this model returned, got "
+                            f"{type(past_key_values).__name__} (tuples and transformers caches are not accepted)")
+        if output_router_logits:
+            raise NotImplementedError("output_router_logits is not supported together with a KV cache")
+        if self.training and torch.is_grad_enabled():
+            raise NotImplementedError("training through a KV cache is not implemented (there is no backward through the "
+                                      "cache): call model.eval() or run under torch.no_grad()")
+        if inputs_embeds is not None or token_type_ids is not None:
+            raise NotImplementedError("inputs_embeds / token_type_ids are not supported on the B200 path")
+        assert cu_seqlens is None, "cu_seqlens belongs to the padding-free transformer"
+        eng = self.engine
+        if eng.comm is not None:
+            raise NotImplementedError("decoding runs on an unsharded engine (world_size 1)")
+        dev = eng.device
+        input_ids = torch.as_tensor(input_ids).to(dev).long()
+        assert input_ids.dim() == 2, "padded batches are [batch, sequence]"
+        B, S = input_ids.shape
+        cache = past_key_values
+        past_width = 0 if cache is None else cache.get_seq_length()
+        if cache is not None and cache.lens.numel() != B:
+            raise ValueError(f"past_key_values holds {cache.lens.numel()} sequences, input_ids {B}")
+        if attention_mask is None:
+            mask = torch.ones(B, S, dtype=torch.bool, device=dev)
+        else:
+            am = torch.as_tensor(attention_mask).to(dev).bool()
+            if am.dim() != 2 or am.shape[0] != B or am.shape[1] not in (S, past_width + S):
+                raise ValueError(f"attention_mask must be [{B}, {past_width + S}] (past and new columns) or [{B}, {S}], "
+                                 f"got {tuple(am.shape)}")
+            mask = am[:, am.shape[1] - S:]
+        n_host = mask.sum(1).tolist()  # one host sync, as _forward_padded
+        keep = mask.reshape(-1).nonzero(as_tuple=True)[0]
+        ids_p = input_ids.reshape(-1)[keep].contiguous()
+        pos_p = None if position_ids is None else torch.as_tensor(position_ids).to(dev).long().reshape(-1)[keep].contiguous()
+        alibi = self._alibi_pass(attention_mask is not None)
+        if cache is None:
+            cache = KVCache(eng, B, max(n_host) + 64)
+            cu = torch.zeros(B + 1, dtype=torch.int32, device=dev)
+            cu[1:] = torch.tensor(n_host, dtype=torch.int32, device=dev).cumsum(0)
+            if pos_p is None:
+                pos_p = (mask.long().cumsum(-1) - 1).reshape(-1)[keep].contiguous()
+            ids_pp, pos_pp, cu_p, _, T_real = _pad_packed_stream(ids_p, pos_p, cu, None)
+            out = eng.prefill(ids_pp, pos_pp, cu_p, max(max(n_host), 1), cache, n_sequences=B, alibi=alibi)[:T_real]
+        else:
+            out = eng.extend(ids_p, n_host, cache, position_ids=pos_p, alibi=alibi)
+        cache.seen = past_width + S
+        loss = None
+        if labels is not None:  # CE(logits[:, :-1], labels[:, 1:]) over the chunk's real positions, as _forward_padded
+            lab = torch.as_tensor(labels).to(dev).long()
+            nxt = torch.full_like(lab, -100)
+            nxt[:, :-1] = lab[:, 1:]
+            nxt_valid = torch.zeros_like(mask)
+            nxt_valid[:, :-1] = mask[:, 1:]
+            nxt = torch.where(nxt_valid & mask, nxt, torch.full_like(nxt, -100))
+            loss = K.cross_entropy_fwd_bwd(out, nxt.reshape(-1)[keep].contiguous(), ignore_index=-100,
+                                           dlogits=torch.empty_like(out))[0].reshape(())
+        full = out.new_zeros(B * S, out.shape[-1])
+        full[keep] = out
+        result = CausalLMOutputWithPast(loss=loss, logits=full.view(B, S, -1), past_key_values=cache)
+        return result if return_dict else result.to_tuple()
 
     # ---- pretraining entry: labels already aligned with positions (model_wrapper/pretraining.py:104-127) ----
     def train(self, mode: bool = True):

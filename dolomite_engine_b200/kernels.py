@@ -818,6 +818,48 @@ def attn_decode(qkv, k_cache, v_cache, lens, n_groups: int, q_per_group: int, he
     return out
 
 
+def attn_cache(qkv, cu_new, past, k_cache, v_cache, n_groups: int, q_per_group: int, head_dim: int, scale: float,
+               max_new: int | None = None, max_end: int | None = None, out=None, alibi_slopes=None):
+    """n[b] = cu_new[b+1] - cu_new[b] >= 0 new tokens per sequence against its KV cache: qkv [sum n, qkv_dim] (roped),
+    cu_new int32 [B+1], past int32 [B] (tokens cached before the new ones), caches [B, L_max, n_groups * head_dim] with the
+    new tokens' keys / values already at past[b] .. past[b] + n[b] - 1 -> [sum n, n_heads * head_dim]; new token i of b
+    attends to cache positions 0 .. past[b] + i.  `max_new` / `max_end`: host bounds of n[b] and past[b] + n[b] (None: read
+    from the tensors, a host sync).  `alibi_slopes`: ALiBi bias of each cache position (see attn_decode)"""
+    nh = n_groups * q_per_group
+    _attn_layout(qkv, nh, head_dim, **({} if out is None else {"out": out}))
+    if k_cache.dim() != 3 or k_cache.shape != v_cache.shape or k_cache.shape[2] != n_groups * head_dim \
+            or not k_cache.is_contiguous() or not v_cache.is_contiguous():
+        raise ValueError(f"k_cache / v_cache must be contiguous [B, L_max, {n_groups * head_dim}] tensors of one shape, got "
+                         f"{tuple(k_cache.shape)} / {tuple(v_cache.shape)}")
+    B, L_max = k_cache.shape[0], k_cache.shape[1]
+    if cu_new.dim() != 1 or cu_new.numel() != B + 1 or past.dim() != 1 or past.numel() != B \
+            or not cu_new.is_contiguous() or not past.is_contiguous():
+        raise ValueError(f"cu_new / past must be contiguous [{B + 1}] / [{B}] tensors, got {tuple(cu_new.shape)} / "
+                         f"{tuple(past.shape)}")
+    n = cu_new[1:] - cu_new[:-1]
+    if max_new is None:
+        max_new = int(n.max()) if B else 0
+    if max_end is None:
+        max_end = int((past + n).max()) if B else 0
+    if max_end > L_max:
+        raise ValueError(f"past + n (up to {max_end}) exceeds the cache length {L_max}")
+    _req(qkv, _BF16, "qkv"), _req(k_cache, _BF16, "k_cache"), _req(v_cache, _BF16, "v_cache")
+    _req(cu_new, torch.int32, "cu_new"), _req(past, torch.int32, "past")
+    if out is not None:
+        _req(out, _BF16, "out")
+    o = torch.empty(qkv.shape[0], nh * head_dim, dtype=_BF16, device=qkv.device) if out is None else out
+    if alibi_slopes is not None:
+        _req_slopes(alibi_slopes, nh)
+        _lib.call("dolomite_b200_attn_cache_alibi", qkv.data_ptr(), qkv.stride(0), cu_new.data_ptr(), past.data_ptr(),
+                  k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(), B, int(max_new), int(max_end), L_max, n_groups,
+                  q_per_group, head_dim, scale, alibi_slopes.data_ptr(), _stream())
+        return o
+    _lib.call("dolomite_b200_attn_cache", qkv.data_ptr(), qkv.stride(0), cu_new.data_ptr(), past.data_ptr(),
+              k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(), B, int(max_new), int(max_end), L_max, n_groups,
+              q_per_group, head_dim, scale, _stream())
+    return o
+
+
 # ------------------------------------------------------------------------------------------------
 # MoE: routing plan, grouped expert GEMMs (moe_dolomite/moe/scatter.py:18-138)
 # ------------------------------------------------------------------------------------------------

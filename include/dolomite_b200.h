@@ -275,6 +275,30 @@ int dolomite_b200_attn_decode_alibi(const void* qkv, int64_t row_stride, const v
                                     int head_dim, float softmax_scale, const float* alibi_slopes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Attention of several new tokens per sequence against a KV cache (a forward with `past_key_values` and a query block of
+ * n tokens: gpt_dolomite/base.py:173-257 and :300-349, the causal mask of a query block that starts past_length keys in;
+ * attention/sdpa.py:11-83).  Sequence b has past[b] cached tokens and n[b] = cu_new[b+1] - cu_new[b] >= 0 new ones;
+ * new token i of b attends to cache positions 0 .. past[b] + i.  fp32 online softmax, output rounded to bf16 once; no
+ * dropout (inference only).  n[b] == 0: nothing is computed or written for b.
+ *   qkv      bf16 [sum n, row_stride]: packed c_attn output of the new tokens (RoPE applied); only the q slots are read
+ *   cu_new   int32 [batch + 1]: token rows of each sequence's new tokens in qkv / out
+ *   past     int32 [batch]: cached tokens before the new ones
+ *   k_cache / v_cache  bf16 [batch, L_max, n_groups * head_dim]: keys / values by position, the new tokens' already
+ *            written at past[b] .. past[b] + n[b] - 1
+ *   out      bf16 [sum n, n_heads * head_dim]
+ *   max_new  host upper bound of n[b] (sets the grid); max_end host upper bound of past[b] + n[b], at most L_max
+ *   head_dim: 16, 32, 64, 80, 96, 128, 160, 192 or 256.  qkv, the caches and out 16-byte aligned, row_stride % 8 == 0.
+ * The _alibi form adds bf16(alibi_slopes[h] * k) to the logit of cache position k of head h, as attn_decode_alibi.
+ * ------------------------------------------------------------------------------------------------ */
+int dolomite_b200_attn_cache(const void* qkv, int64_t row_stride, const int32_t* cu_new, const int32_t* past,
+                             const void* k_cache, const void* v_cache, void* out, int batch, int max_new, int max_end,
+                             int64_t L_max, int n_groups, int q_per_group, int head_dim, float softmax_scale, void* stream);
+int dolomite_b200_attn_cache_alibi(const void* qkv, int64_t row_stride, const int32_t* cu_new, const int32_t* past,
+                                   const void* k_cache, const void* v_cache, void* out, int batch, int max_new, int max_end,
+                                   int64_t L_max, int n_groups, int q_per_group, int head_dim, float softmax_scale,
+                                   const float* alibi_slopes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * bf16 GEMM on Hopper tensor cores (TMA -> smem -> wgmma -> register accumulators -> epilogue), replacing the cuBLAS
  * calls behind nn.Linear (linear.py:5-25; call sites attention/base.py:100, padding_free.py:74,
  * gpt_dolomite/mlp.py:46-48, gpt_dolomite/main.py:172-177) and their autograd (dgrad / wgrad).
